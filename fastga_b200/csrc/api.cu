@@ -21,6 +21,8 @@ int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int b
 int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
                        void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
 long long fgb_sort128_tmp_bytes(long long n);
+int fgb_sort_seeds64_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
+                            void *d_tmp, long long tmp_bytes, unsigned long long *d_flag, void *stream);
 int fgb_stage_genome_device(const void *d_bps, const long long *d_boff, const long long *d_clen,
                             const long long *d_woff, int ncontig, long long total_words,
                             void *d_seq, void *d_rseq, void *stream);
@@ -648,15 +650,27 @@ static int seeds_sort_impl(rec128 *d_a, long long n, const seed_bits &L, long lo
   s->n = n; s->sumlen = sumlen; s->n1_merged = n1m;
   long long tmpb = fgb_sort128_tmp_bytes(n);
   int rc = FGB_OK, inb = 0;
+  //  a key of <= 64 bits leaves hi = 0 in every record: the passes run on the lo words alone.
+  //  FGB_SEED_SORT_WIDE=1 forces the 128-bit passes (both paths can be compared in one process).
+  const char *wide_env = getenv("FGB_SEED_SORT_WIDE");
+  const bool narrow = L.key <= 64 && !(wide_env != NULL && atoi(wide_env) != 0);
+  u64 hiflag = 0, *d_hiflag = NULL;
   if (fgb_dmalloc((void **) &d_b,sizeof(rec128)*(n+1),st) != cudaSuccess ||
-      fgb_dmalloc((void **) &d_tmp,tmpb,st) != cudaSuccess) rc = FGB_ERR_CUDA;
+      fgb_dmalloc((void **) &d_tmp,tmpb + 8,st) != cudaSuccess) rc = FGB_ERR_CUDA;
   if (!rc)
     { stage_timer t(&g_timings.ssort_ms,st);
       //  from bit 6: the lcp field (bits 0..5) cannot break a tie -- two seeds that agree on strand,
       //  contigs, band, anti-diagonal and diagonal remainder are the same pair of positions
-      rc = fgb_sort128_bits_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,&inb,st);
+      if (narrow)
+        { d_hiflag = (u64 *) ((char *) d_tmp + tmpb);
+          rc = fgb_sort_seeds64_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,d_hiflag,st);
+        }
+      else
+        rc = fgb_sort128_bits_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,&inb,st);
     }
+  if (!rc && d_hiflag && cudaMemcpyAsync(&hiflag,d_hiflag,8,cudaMemcpyDeviceToHost,st) != cudaSuccess) rc = FGB_ERR_CUDA;
   if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
+  if (!rc && hiflag) rc = FGB_ERR_ARG;                 // a record with hi != 0: the 64-bit passes mis-ordered it
   if (!rc)
     { s->d_rec = inb ? d_b : d_a;
       if (inb) d_b = NULL; else d_a = NULL;                     // ownership moved to the handle

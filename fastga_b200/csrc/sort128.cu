@@ -307,6 +307,241 @@ extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo
 }
 
 /***********************************************************************************************
+ *  Seed sort on 64-bit words.  When the seed key fits in 64 bits (every 100 Mbp-class pair) the
+ *  merge leaves hi = 0 in every record, yet the 128-bit passes above read and write all 16 bytes.
+ *  Here the first pass reads the 16-byte records and writes only their lo words, the middle passes
+ *  run on 8-byte words and the last pass writes 16-byte records again (hi = 0): per record
+ *  16 + 24 + 16·(passes−2) + 24 bytes instead of 16 + 32·passes.  Same Onesweep method as
+ *  sort_onesweep_kernel (TMA tile, nine-ballot multi-split, counts published first, look-back last,
+ *  next histogram counted while the tile is resident), stable.
+ **********************************************************************************************/
+
+//  records per tile of a pass on 8-byte input (the 16-byte first pass keeps SORT_TILE: the staging
+//  buffer holds one tile of INPUT records, 64 KB either way, so two CTAs still share an SM)
+#ifndef SORT64_ITEMS
+#define SORT64_ITEMS 16
+#endif
+static_assert(SORT_THREADS*SORT64_ITEMS >= SORT_TILE, "fgb_sort128_tmp_bytes sizes the look-back status for SORT_TILE");
+
+template <int IW> struct os64_tile
+{ static constexpr int ITEMS = (IW == 16) ? SORT_ITEMS : SORT64_ITEMS;
+  static constexpr int TILE  = SORT_THREADS*ITEMS;
+  static constexpr size_t SMEM = (size_t) TILE*IW + (SORT_WARPS*256 + 256 + 256 + 8)*sizeof(unsigned)
+                                 + 256*sizeof(unsigned long long);
+};
+
+//  IW / OW: bytes per input / output record.  16: a rec128 whose hi word must be zero (the pass ORs
+//  every hi word it drops into *hiflag); 8: its lo word alone; 16 out: lo, hi = 0.
+template <int IW, int OW>
+__global__ void __launch_bounds__(SORT_THREADS,SORT_MINBLK)
+sort_onesweep64_kernel(const void *__restrict__ in, void *__restrict__ out, long long n, int dsh /* bit offset of the digit */,
+                       int next_dsh /* of the next pass's digit, -1: none */, const unsigned long long *__restrict__ binbase,
+                       unsigned long long *__restrict__ nexthist, unsigned long long *status /* [ntiles][256] */,
+                       unsigned *__restrict__ ticket, unsigned long long *__restrict__ hiflag)
+{ constexpr int ITEMS = os64_tile<IW>::ITEMS, TILE = os64_tile<IW>::TILE;
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  unsigned long long *tile = reinterpret_cast<unsigned long long *>(smem_raw);   // input tile, then the words in digit order
+  unsigned *wcount = reinterpret_cast<unsigned *>(smem_raw + (size_t) TILE*IW); // [SORT_WARPS][256]
+  unsigned *bexcl  = wcount + SORT_WARPS*256;                                   // [256]
+  unsigned *nhist  = bexcl + 256;                                               // [256] next digit
+  unsigned *wtot   = nhist + 256;                                               // [8]
+  unsigned long long *gbase = reinterpret_cast<unsigned long long *>(wtot + 8); // [256]
+  __shared__ unsigned tile_s;
+  __shared__ __align__(8) unsigned long long tbar;
+
+  int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  if (tid == 0)
+    { unsigned t = atomicAdd(ticket,1u);
+      tile_s = t;
+      //  an odd count of 8-byte words is rounded up to the 16 bytes a bulk copy moves (the caller's
+      //  buffers have room for that word; it is never ranked)
+      long long t0 = (long long) t * TILE, rm = n - t0;
+      unsigned nb = ((unsigned) (rm < TILE ? rm : TILE) * IW + 15u) & ~15u;
+      mbar_init(&tbar,1);
+      tma_load_1d(tile,reinterpret_cast<const unsigned char *>(in) + t0*IW,nb,&tbar);
+    }
+  for (int i = tid; i < SORT_WARPS*256; i += SORT_THREADS) wcount[i] = 0;
+  if (tid < 256) nhist[tid] = 0;
+  __syncthreads();
+  const unsigned tileid = tile_s;
+  long long tile0 = (long long) tileid * TILE;
+  long long rem = n - tile0;
+  int cnt = rem < TILE ? (int) rem : TILE;
+
+  unsigned long long r[ITEMS], hi_or = 0;
+  unsigned rank[ITEMS];
+  int base = w*(32*ITEMS);
+  unsigned *myc = wcount + w*256;
+  mbar_wait(&tbar,0);
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++)
+    { int idx = base + it*32 + lane;
+      bool valid = idx < cnt;
+      unsigned d = 0;
+      if (valid)
+        { if (IW == 16)
+            { rec128 v = ld_rec(reinterpret_cast<const rec128 *>(tile) + idx);
+              r[it] = v.lo;
+              hi_or |= v.hi;
+            }
+          else
+            r[it] = tile[idx];
+          d = (unsigned) (r[it] >> dsh) & 0xff;
+        }
+      unsigned peers = match_digit(d,valid);
+      int leader = valid ? __ffs(peers)-1 : lane;
+      unsigned b = 0;
+      if (valid && lane == leader)
+        { b = myc[d];
+          myc[d] = b + __popc(peers);
+        }
+      b = __shfl_sync(0xffffffffu,b,leader);
+      rank[it] = b + __popc(peers & lanemask_lt());
+      if (next_dsh >= 0 && valid) atomicAdd(&nhist[(unsigned) (r[it] >> next_dsh) & 0xff],1u);
+      __syncwarp();
+    }
+  if (IW == 16 && hi_or) atomicOr(hiflag,hi_or);
+  __syncthreads();
+
+  unsigned c = 0, inc = 0;
+  unsigned long long *mine = status + (unsigned long long) tileid*256 + tid;
+  if (tid < 256)
+    { unsigned sum = 0;
+#pragma unroll
+      for (int ww = 0; ww < SORT_WARPS; ww++)
+        { unsigned t = wcount[ww*256+tid];
+          wcount[ww*256+tid] = sum;
+          sum += t;
+        }
+      c = sum;
+      if (tileid == 0)
+        atomicExch(mine,ST_INC | c);
+      else
+        atomicExch(mine,ST_AGG | c);
+      inc = warp_incl_scan(c,lane);
+      if (lane == 31) wtot[w] = inc;
+    }
+  __syncthreads();
+  if (tid < 256)
+    { unsigned pre = 0;
+      for (int i = 0; i < w; i++) pre += wtot[i];
+      bexcl[tid] = pre + inc - c;
+    }
+  __syncthreads();
+
+#pragma unroll
+  for (int it = 0; it < ITEMS; it++)
+    { int idx = base + it*32 + lane;
+      if (idx < cnt)
+        { unsigned d = (unsigned) (r[it] >> dsh) & 0xff;
+          tile[bexcl[d] + myc[d] + rank[it]] = r[it];
+        }
+    }
+  if (tid < 256)
+    { volatile unsigned long long *stt = status;
+      unsigned long long excl = 0;
+      for (long long t = (long long) tileid - 1; t >= 0; )
+        { unsigned long long v[4];
+#pragma unroll
+          for (int q = 0; q < 4; q++)
+            v[q] = (t - q >= 0) ? stt[(unsigned long long) (t - q)*256 + tid] : ST_INC;
+          bool done = false;
+#pragma unroll
+          for (int q = 0; q < 4; q++)
+            { if (done || (v[q] >> 62) == 0) break;
+              excl += v[q] & ST_MASK;
+              t -= 1;
+              if (v[q] & ST_INC) done = true;
+            }
+          if (done) break;
+        }
+      if (tileid != 0) atomicExch(mine,ST_INC | (excl + c));
+      gbase[tid] = binbase[tid] + excl - bexcl[tid];
+      if (next_dsh >= 0 && nhist[tid]) atomicAdd(&nexthist[tid],(unsigned long long) nhist[tid]);
+    }
+  __syncthreads();
+
+  for (int p = tid; p < cnt; p += SORT_THREADS)
+    { unsigned long long v = tile[p];
+      unsigned long long o = gbase[(unsigned) (v >> dsh) & 0xff] + p;
+      if (OW == 8)
+        reinterpret_cast<unsigned long long *>(out)[o] = v;
+      else
+        { rec128 R; R.lo = v; R.hi = 0;
+          st_rec(reinterpret_cast<rec128 *>(out) + o,R);
+        }
+    }
+}
+
+template <int IW, int OW>
+static int onesweep64_pass(const void *in, void *out, long long n, int dsh, int next_dsh, const unsigned long long *binbase,
+                           unsigned long long *nexthist, unsigned long long *status, unsigned *ticket,
+                           unsigned long long *hiflag, cudaStream_t st)
+{ typedef os64_tile<IW> T;
+  static bool attr_set = false;
+  if (!attr_set)
+    { CUDA_TRY(cudaFuncSetAttribute(sort_onesweep64_kernel<IW,OW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) T::SMEM));
+      attr_set = true;
+    }
+  int ntiles = (int) ((n + T::TILE - 1) / T::TILE);
+  CUDA_TRY(cudaMemsetAsync(status,0,256ull*ntiles*8,st));
+  sort_onesweep64_kernel<IW,OW><<<ntiles,SORT_THREADS,T::SMEM,st>>>(in,out,n,dsh,next_dsh,binbase,nexthist,status,ticket,hiflag);
+  fgb_count_launch(1);
+  return FGB_OK;
+}
+
+//  Sorts n 16-byte records in d_a on bits [bit_lo,bit_hi) like fgb_sort128_bits_device, for records
+//  whose hi word is zero (bit_hi <= 64).  The two 8-byte ping-pong buffers are the two halves of d_b
+//  (16(n+1) bytes), the result lands in d_a.  *d_flag (device) gets the OR of every hi word the first
+//  pass dropped: non-zero means the records broke the contract and d_a is not sorted.
+extern "C" int fgb_sort_seeds64_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
+                                       void *d_tmp, long long tmp_bytes, unsigned long long *d_flag, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (n < 0 || bit_lo < 0 || bit_hi > 64 || bit_lo > bit_hi) return FGB_ERR_ARG;
+  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
+  CUDA_TRY(cudaMemsetAsync(d_flag,0,8,st));
+  if (n <= 1 || bit_lo == bit_hi) return FGB_OK;
+  if (tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
+  if (bit_hi - bit_lo <= 8)                   // one pass: nothing to narrow
+    { int inb = 0;
+      int rc = fgb_sort128_bits_device(d_a,d_b,n,bit_lo,bit_hi,d_tmp,tmp_bytes,&inb,stream);
+      if (rc) return rc;
+      if (inb) CUDA_TRY(cudaMemcpyAsync(d_a,d_b,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+      return FGB_OK;
+    }
+
+  int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE);       // the carve-up of fgb_sort128_bits_device
+  unsigned long long *status = (unsigned long long *) d_tmp;
+  unsigned long long *hist[2] = { status + 256ull*ntiles, status + 256ull*ntiles + 256 };
+  unsigned long long *binbase = status + 256ull*ntiles + 512;
+  unsigned *ticket = (unsigned *) (binbase + 256);
+  //  the second half starts 16-byte aligned; both halves may be read one word past their end
+  unsigned char *half[2] = { (unsigned char *) d_b, (unsigned char *) d_b + ((8*n + 15) & ~15ll) };
+
+  CUDA_TRY(cudaMemsetAsync(hist[0],0,256*8,st));
+  { int nb = ntiles < 1184 ? ntiles : 1184;
+    sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>((const rec128 *) d_a,n,bit_lo,hist[0]);
+    fgb_count_launch(1);
+  }
+  int cur = 0, rc = FGB_OK;
+  for (int p = 0, b = bit_lo; b < bit_hi && rc == FGB_OK; p++, b += 8)
+    { const int nd = (b+8 < bit_hi) ? b+8 : -1;
+      sort_bins_kernel<<<1,256,0,st>>>(hist[cur],binbase,hist[cur^1],ticket);
+      fgb_count_launch(1);
+      if (p == 0)
+        rc = onesweep64_pass<16,8>(d_a,half[0],n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
+      else if (nd >= 0)
+        rc = onesweep64_pass<8,8>(half[(p-1)&1],half[p&1],n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
+      else
+        rc = onesweep64_pass<8,16>(half[(p-1)&1],d_a,n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
+      cur ^= 1;
+    }
+  if (rc) return rc;
+  CUDA_TRY(cudaGetLastError());
+  return FGB_OK;
+}
+
+/***********************************************************************************************
  *  k-mer table sort (msd_sort's job in GIXmake.c:1436): by the 40-mer (bytes 6..15), equal
  *  k-mers by (strand|contig rank, post), i.e. by the whole 128-bit value.
  *
