@@ -35,6 +35,19 @@ int fgb_syncmer_emit_device(const void *d_seq, const long long *d_clen, const lo
                             const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
                             int ntiles, unsigned *d_tile_offset, void *d_records, unsigned plo,
                             unsigned phi, void *stream);
+int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
+int fgb_syncmer_bin_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
+                                 const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
+                                 int ntiles, unsigned long long *d_buck1024, unsigned *d_bin_start, long long nf,
+                                 int fsh, unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
+                                 unsigned plo, unsigned phi, void *stream);
+int fgb_syncmer_scatter_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
+                               const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
+                               int ntiles, const unsigned *d_bin_start, unsigned *d_cursor, long long nf, int fsh,
+                               long long n, void *d_records, unsigned *d_bad, unsigned plo, unsigned phi,
+                               void *stream);
+int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
+                                     const unsigned *fstart, long long nf, int fsh, int *result_in_b, void *stream);
 int fgb_kix_index_device(const void *d_tab, long long n, unsigned *d_pstart, unsigned char *d_adj, void *stream);
 int fgb_ktab_export_device(const void *d_tab, long long n, int pbytes, int cbytes,
                            const long long *d_part_first, int nparts, void *d_out, void *stream);
@@ -256,7 +269,7 @@ static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-
   for (cum = 1; cum < 2ll*g->ncontig; cum *= 256) x->cont_bytes += 1;
 }
 
-//  K1..K4: syncmer scan -> 128-bit records -> 10-pass byte radix sort on the 80-bit k-mer ->
+//  K1..K4: syncmer scan -> 128-bit records laid out by prefix bin -> bucket sort on the whole record ->
 //  2^24 prefix index.
 
 #define GIX_FWD_ONLY 0x80000000u     // flag bit carried in `phi` down to syncmer_kernel
@@ -294,70 +307,117 @@ extern "C" int fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned p
   return gix_build_range(g,plo,phi,out,stream);
 }
 
+//  The fine prefix bins a table's scan lays its records out by (fgb_kmer_sort_fine_binned_device):
+//  bin f = (prefix24 >> fsh) - (plo >> fsh) holds records [start[f], start[f+1]), f < nf.
+struct fine_bins
+{ int fsh = 0;
+  long long nf = 0;
+  std::vector<unsigned> start;
+};
+
 //  K1/K2: syncmer scan + record build of the contigs selected by `mask` (NULL: all) into a fresh
 //  device buffer of *n unsorted records (room for n+1).  *nrev = reverse entries left out (fwd-only).
+//  fb == NULL: the records are packed tile after tile.  Otherwise the count pass counts them per fine
+//  bin, at the resolution the k-mer sort would pick for an upper bound of n (two records per scanned
+//  position), and the emit pass writes each record straight into its bin; fb gets the bins.
 static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo, unsigned phi_flags,
-                    rec128 **d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024, cudaStream_t st)
+                    rec128 **d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
+                    fine_bins *fb, cudaStream_t st)
 { int T = fgb_sc_tile();
   std::vector<int> tc, ts;
+  long long npos = 0;
   for (int c = 0; c < g->ncontig; c++)
     if (g->clen[c] >= 12 && g->boff[c] >= 0 && (mask == NULL || mask[c]))
-      for (long long t0 = 0; t0 + 12 <= g->clen[c]; t0 += T)
-        { tc.push_back(c); ts.push_back((int) t0); }
+      { npos += g->clen[c] - 11;
+        for (long long t0 = 0; t0 + 12 <= g->clen[c]; t0 += T)
+          { tc.push_back(c); ts.push_back((int) t0); }
+      }
   int ntiles = (int) tc.size();
   int *d_tc = NULL, *d_ts = NULL; unsigned *d_cnt = NULL;
   u64 *d_buck = NULL, *d_total = NULL; void *d_tmp = NULL;
+  unsigned *d_fb = NULL, bad = 0;          // fine bins: starts [0,nf), cursors [nf,2nf), check flag [2nf]
+  long long nf = 0;
   rec128 *d_a = NULL;
   long long tmpb = fgb_dev_scan_tmp_bytes(ntiles);
   int rc = FGB_OK;
   u64 total = 0, rdropped = 0;
+  if (fb)
+    { const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
+      const unsigned bhi = phi > plo ? phi : plo + 1;          // an empty range still gets one (empty) bin
+      fb->fsh = fgb_kmer_bin_shift(2*npos,plo,bhi);
+      fb->nf = nf = (long long) ((((unsigned long long) (bhi - 1)) >> fb->fsh) - ((unsigned long long) plo >> fb->fsh)) + 1;
+      tmpb = fgb_dev_scan_tmp_bytes(nf);
+    }
 #define GS_TRY(call) do { if ((call) != cudaSuccess) { rc = FGB_ERR_CUDA; goto done; } } while (0)
   GS_TRY(fgb_dmalloc((void **) &d_tc,sizeof(int)*(ntiles+1),st));
   GS_TRY(fgb_dmalloc((void **) &d_ts,sizeof(int)*(ntiles+1),st));
-  GS_TRY(fgb_dmalloc((void **) &d_cnt,sizeof(unsigned)*(ntiles+1),st));
+  if (fb) GS_TRY(fgb_dmalloc((void **) &d_fb,sizeof(unsigned)*(2*nf+1),st));
+  else    GS_TRY(fgb_dmalloc((void **) &d_cnt,sizeof(unsigned)*(ntiles+1),st));
   GS_TRY(fgb_dmalloc((void **) &d_buck,8*1025,st));
   GS_TRY(fgb_dmalloc((void **) &d_total,8,st));
   GS_TRY(fgb_dmalloc((void **) &d_tmp,tmpb,st));
   GS_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   GS_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   { stage_timer t(&g_timings.scan_ms,st);
-    rc = fgb_syncmer_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,
-                                  d_buck,d_total,d_tmp,tmpb,plo,phi_flags,st);
+    if (fb)
+      rc = fgb_syncmer_bin_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_fb,nf,
+                                        fb->fsh,d_total,d_tmp,tmpb,plo,phi_flags,st);
+    else
+      rc = fgb_syncmer_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,
+                                    d_buck,d_total,d_tmp,tmpb,plo,phi_flags,st);
     if (rc) goto done;
     GS_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
     if (buck1024) GS_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
     GS_TRY(cudaMemcpyAsync(&rdropped,d_buck + 1024,8,cudaMemcpyDeviceToHost,st));
+    if (fb)
+      { fb->start.resize((size_t) nf + 1);
+        GS_TRY(cudaMemcpyAsync(fb->start.data(),d_fb,sizeof(unsigned)*nf,cudaMemcpyDeviceToHost,st));
+      }
     GS_TRY(cudaStreamSynchronize(st));
   }
   if (total >= 0xfffffff0ull) { rc = FGB_ERR_LIMIT; goto done; }
   GS_TRY(fgb_dmalloc((void **) &d_a,sizeof(rec128)*(total+1),st));
   { stage_timer t(&g_timings.scan_ms,st);
-    rc = fgb_syncmer_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,d_a,plo,phi_flags,st);
+    if (fb)
+      { rc = fgb_syncmer_scatter_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_fb,d_fb + nf,nf,
+                                        fb->fsh,(long long) total,d_a,d_fb + 2*nf,plo,phi_flags,st);
+        if (!rc && cudaMemcpyAsync(&bad,d_fb + 2*nf,4,cudaMemcpyDeviceToHost,st) != cudaSuccess) rc = FGB_ERR_CUDA;
+      }
+    else
+      rc = fgb_syncmer_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,d_a,plo,phi_flags,st);
   }
   if (rc == FGB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;   // tc/ts must outlive the copies
+  if (rc == FGB_OK && bad) rc = FGB_ERR_OVERFLOW;        // a bin came out over- or underfull: d_a is not laid out by bin
+  if (rc == FGB_OK && fb) fb->start[nf] = (unsigned) total;
 done:
 #undef GS_TRY
-  fgb_dfree(d_tc,st); fgb_dfree(d_ts,st); fgb_dfree(d_cnt,st); fgb_dfree(d_buck,st); fgb_dfree(d_total,st); fgb_dfree(d_tmp,st);
+  fgb_dfree(d_tc,st); fgb_dfree(d_ts,st); fgb_dfree(d_cnt,st); fgb_dfree(d_fb,st); fgb_dfree(d_buck,st);
+  fgb_dfree(d_total,st); fgb_dfree(d_tmp,st);
   if (rc) { fgb_dfree(d_a,st); return rc; }
   *d_recs = d_a; *n_out = (long long) total; *nrev = (long long) rdropped;
   return FGB_OK;
 }
 
 //  K3/K4: sorts the records in d_a (consumed: it ends up inside the handle or is released) whose
-//  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.
-static int gix_finish(fgb_gix *x, rec128 *d_a, long long n, unsigned plo, unsigned phi, cudaStream_t st, bool index = true)
+//  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.  fb: the fine bins the
+//  scan laid d_a out by; NULL: records in any order (the partition passes lay them out).
+static int gix_finish(fgb_gix *x, rec128 *d_a, long long n, unsigned plo, unsigned phi, const fine_bins *fb,
+                      cudaStream_t st, bool index = true)
 { rec128 *d_b = NULL; void *d_stmp = NULL;
   long long stmpb = fgb_sort128_tmp_bytes(n);
   int rc = FGB_OK, inb = 0;
   x->n = n;
   if (fgb_dmalloc((void **) &d_b,sizeof(rec128)*(n+1),st) != cudaSuccess ||
-      fgb_dmalloc((void **) &d_stmp,stmpb,st) != cudaSuccess ||
+      (!fb && fgb_dmalloc((void **) &d_stmp,stmpb,st) != cudaSuccess) ||
       (index && fgb_dmalloc((void **) &x->d_pstart,sizeof(unsigned)*((1<<24)+1+8),st) != cudaSuccess) ||
       (index && fgb_dmalloc((void **) &x->d_adj,(size_t) n + 32,st) != cudaSuccess))
     rc = FGB_ERR_CUDA;
   if (!rc)
     { stage_timer t(&g_timings.ksort_ms,st);
-      rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
+      if (fb)
+        rc = fgb_kmer_sort_fine_binned_device(d_a,d_b,n,plo,phi,fb->start.data(),fb->nf,fb->fsh,&inb,st);
+      else
+        rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
     }
   if (!rc)
     { x->d_tab = inb ? d_b : d_a;
@@ -382,8 +442,12 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
   x->ncontig = g->ncontig;
   x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
   rec128 *d_a = NULL; long long n = 0, nrev = 0;
-  int rc = gix_scan(g,NULL,plo,phi_flags,&d_a,&n,&nrev,x->buck1024,st);
-  if (!rc) { x->n_both = n + nrev; rc = gix_finish(x,d_a,n,plo,phi,st,index); }
+  //  the scan lays the records out by prefix bin; FGB_KSORT_PARTITION=1 packs them by tile and lays them
+  //  out with the Onesweep partition passes instead (both paths can be compared in one process)
+  const char *part_env = getenv("FGB_KSORT_PARTITION");
+  fine_bins fb, *pfb = (part_env != NULL && atoi(part_env) != 0) ? NULL : &fb;
+  int rc = gix_scan(g,NULL,plo,phi_flags,&d_a,&n,&nrev,x->buck1024,pfb,st);
+  if (!rc) { x->n_both = n + nrev; rc = gix_finish(x,d_a,n,plo,phi,pfb,st,index); }
   if (rc) { fgb_gix_free(x); return rc; }
   *out = x;
   return FGB_OK;
@@ -405,7 +469,7 @@ extern "C" void fgb_device_free(void *p) { fgb_dfree(p,0); }
 extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only,
                               void **d_recs, long long *n, void *stream)
 { rec128 *d = NULL; long long nrev = 0;
-  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),&d,n,&nrev,NULL,(cudaStream_t) stream);
+  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),&d,n,&nrev,NULL,NULL,(cudaStream_t) stream);
   if (rc) return rc;
   *d_recs = d;
   return FGB_OK;
@@ -449,7 +513,7 @@ extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned pl
   int rc = FGB_OK;
   if (fgb_dmalloc((void **) &d_a,sizeof(rec128)*(n+1),st) != cudaSuccess) rc = FGB_ERR_CUDA;
   if (!rc && n > 0 && cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc) rc = gix_finish(x,d_a,n,plo,phi,st); else fgb_dfree(d_a,st);
+  if (!rc) rc = gix_finish(x,d_a,n,plo,phi,NULL,st); else fgb_dfree(d_a,st);
   if (rc) { fgb_gix_free(x); return rc; }
   *out = x;
   return FGB_OK;

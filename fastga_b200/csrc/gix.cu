@@ -2,7 +2,8 @@
 // build, prefix index + LCP, and conversion from/to the on-disk .ktab entry format.
 //
 // Replaces (reference file:line):
-//   sample_thread / scan_thread      GIXmake.c:164-328, 406-611    -> syncmer_{count,emit}_kernel
+//   sample_thread / scan_thread      GIXmake.c:164-328, 406-611    -> syncmer_bin_count/scatter_kernel
+//                                                                     (syncmer_kernel<0/1>: by tile)
 //   setup_thread_plain               GIXmake.c:802-980             -> emit of 128-bit records
 //   msd_sort                         MSDsort.c:404                 -> sort128.cu (10 byte passes)
 //   compress_thread / k_sort writer  GIXmake.c:1211-1278,1300-1596 -> kix_index/ktab_export kernels
@@ -176,17 +177,21 @@ static __device__ __forceinline__ unsigned syncmer_mask(u64 E, const unsigned ch
   return sel;
 }
 
-template<int EMIT> __global__ void __launch_bounds__(SC_THREADS)
-syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
-               const long long *__restrict__ woff, const int *__restrict__ crank,
-               const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
-               unsigned *__restrict__ tile_count,       // EMIT=0: out counts; EMIT=1: in offsets
-               unsigned long long *__restrict__ buck1024,
-               rec128 *__restrict__ out, unsigned plo, unsigned phi_flags)
+//  EMIT = 0: count pass (sampler histogram; per-tile record counts, or with BINNED per-fine-bin record
+//  counts in bincur).  EMIT = 1: emit pass (records at the tile offsets in tile_count, or with BINNED
+//  scattered into their fine bins through the cursors in bincur).  A fine bin is
+//  (prefix24 >> fsh) - (plo >> fsh).
+template<int EMIT, bool BINNED> static __device__ __forceinline__ void
+syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+             const long long *__restrict__ woff, const int *__restrict__ crank,
+             const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+             unsigned *__restrict__ tile_count, unsigned long long *__restrict__ buck1024,
+             rec128 *__restrict__ out, unsigned plo, unsigned phi_flags,
+             unsigned *__restrict__ bincur, int fsh, unsigned nlim)
 { __shared__ u64 sw[SC_WORDS+1];
   __shared__ unsigned char tn[256], tc[256];
   __shared__ unsigned wsum[SC_THREADS/32];
-  __shared__ unsigned hist[1024];
+  __shared__ unsigned hist[EMIT == 0 ? 1024 : 1];
 
   //  bit 31 of phi_flags: forward-strand entries only (the table is only ever the adaptamer side
   //  of a merge, where reverse entries never seed, FastGA.c:921-928)
@@ -246,18 +251,54 @@ syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
   unsigned cnt = __popc(fmask) + __popc(rmask);
 
   int lane = tid & 31, wp = tid >> 5;
-  unsigned inc = cnt;
+  unsigned pre = 0, tot = 0, inc = cnt;
+  if (!BINNED)
+    {
 #pragma unroll
-  for (int o = 1; o < 32; o <<= 1)
-    { unsigned t = __shfl_up_sync(0xffffffffu,inc,o);
-      if (lane >= o) inc += t;
+      for (int o = 1; o < 32; o <<= 1)
+        { unsigned t = __shfl_up_sync(0xffffffffu,inc,o);
+          if (lane >= o) inc += t;
+        }
+      if (lane == 31) wsum[wp] = inc;
+      __syncthreads();
+      for (int i = 0; i < SC_THREADS/32; i++)
+        { if (i < wp) pre += wsum[i];
+          tot += wsum[i];
+        }
     }
-  if (lane == 31) wsum[wp] = inc;
-  __syncthreads();
-  unsigned pre = 0, tot = 0;
-  for (int i = 0; i < SC_THREADS/32; i++)
-    { if (i < wp) pre += wsum[i];
-      tot += wsum[i];
+  const unsigned cr = (unsigned) crank[c];
+
+  if (BINNED)
+    { //  every record on its own: the k-mers of neighbouring lanes almost never share a fine bin, so
+      //  aggregating a warp's increments (__match_any_sync) merges next to nothing, and a warp-uniform
+      //  loop keeps every lane waiting for the lane with the most records
+      const unsigned fbase = plo >> fsh;
+      unsigned fm = fmask, rm = rmask;
+      while (fm | rm)
+        { rec128 r;
+          r.lo = 0;
+          if (fm)
+            { int i = __ffs(fm)-1;
+              fm &= fm-1;
+              r.hi = rev2(sm_bases64(sw,sb+i));
+              if (EMIT)
+                r.lo = (rev2(sm_bases64(sw,sb+i+32)) & 0xffff000000000000ull) | ((u64) cr << 32) | (unsigned) (p+i);
+            }
+          else
+            { int i = __ffs(rm)-1;
+              rm &= rm-1;
+              u64 e0 = sm_bases64(sw,sb+i-28), e1 = sm_bases64(sw,sb+i+4) & 0xffffull;
+              r.hi = ~((e1 << 48) | (e0 >> 16));
+              r.lo = ((~e0 & 0xffffull) << 48) | ((u64) (cr | 0x8000u) << 32) | (unsigned) (p+i+12);
+            }
+          const unsigned b = (unsigned) (r.hi >> (40 + fsh)) - fbase;
+          if (EMIT == 0)
+            atomicAdd(&bincur[b],1u);                                  // count pass: the bin's count
+          else
+            { const unsigned s = atomicAdd(&bincur[b],1u);             // emit pass: a slot at the bin's cursor
+              if (s < nlim) st_rec(out + s,r);                         // an overrun is caught by kmer_scatter_check_kernel
+            }
+        }
     }
 
   if (EMIT == 0)
@@ -286,12 +327,12 @@ syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
         { rdropped = __reduce_add_sync(0xffffffffu,rdropped);
           if (lane == 0 && rdropped) atomicAdd(&buck1024[1024],(unsigned long long) rdropped);
         }
-      if (tid == 0) tile_count[blockIdx.x] = tot;
+      if (!BINNED && tid == 0) tile_count[blockIdx.x] = tot;
       return;
     }
+  if (BINNED) return;
 
   long long o = (long long) tile_count[blockIdx.x] + pre + inc - cnt;
-  unsigned cr = (unsigned) crank[c];
   unsigned m = fmask | rmask;
   while (m)
     { int i = __ffs(m)-1;
@@ -316,6 +357,43 @@ syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
           o += 1;
         }
     }
+}
+
+//  Records packed by tile, for callers that sort them with the partition passes (the sharded path)
+template<int EMIT> __global__ void __launch_bounds__(SC_THREADS)
+syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+               const long long *__restrict__ woff, const int *__restrict__ crank,
+               const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+               unsigned *__restrict__ tile_count,       // EMIT=0: out counts; EMIT=1: in offsets
+               unsigned long long *__restrict__ buck1024,
+               rec128 *__restrict__ out, unsigned plo, unsigned phi_flags)
+{ syncmer_body<EMIT,false>(seq,clen,woff,crank,tile_contig,tile_start,tile_count,buck1024,out,plo,phi_flags,NULL,0,0); }
+
+//  Records laid out by fine bin: counts per bin, then a scatter through per-bin cursors
+__global__ void __launch_bounds__(SC_THREADS)
+syncmer_bin_count_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+                         const long long *__restrict__ woff, const int *__restrict__ crank,
+                         const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+                         unsigned long long *__restrict__ buck1024, unsigned plo, unsigned phi_flags,
+                         unsigned *__restrict__ bin_count, int fsh)
+{ syncmer_body<0,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,buck1024,NULL,plo,phi_flags,bin_count,fsh,0); }
+
+__global__ void __launch_bounds__(SC_THREADS)
+syncmer_scatter_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+                       const long long *__restrict__ woff, const int *__restrict__ crank,
+                       const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+                       rec128 *__restrict__ out, unsigned n, unsigned plo, unsigned phi_flags,
+                       unsigned *__restrict__ bin_cursor, int fsh)
+{ syncmer_body<1,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,NULL,out,plo,phi_flags,bin_cursor,fsh,n); }
+
+//  After the scatter every fine-bin cursor has advanced to the start of the next bin.  Any other value
+//  means the count and emit passes disagreed about which records exist: *bad = 1.
+__global__ void kmer_scatter_check_kernel(const unsigned *__restrict__ cursor, const unsigned *__restrict__ start,
+                                          long long nf, unsigned n, unsigned *__restrict__ bad)
+{ long long f = (long long) blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= nf) return;
+  unsigned end = (f + 1 < nf) ? start[f+1] : n;
+  if (cursor[f] != end) *bad = 1;
 }
 
 /***********************************************************************************************
@@ -483,6 +561,54 @@ extern "C" int fgb_syncmer_emit_device(const void *d_seq, const long long *d_cle
                                                    d_tile_contig,d_tile_start,d_tile_offset,
                                                    NULL,(rec128 *) d_records,plo,phi);
   fgb_count_launch(1);
+  CUDA_TRY(cudaGetLastError());
+  return FGB_OK;
+}
+
+//  Pass 1 of the binned scan: 1024-bin sampler histogram, and the records per fine bin (nf bins of
+//  shift fsh) scanned in place to the bins' first slots; *d_total = number of records.
+extern "C" int fgb_syncmer_bin_count_device(const void *d_seq, const long long *d_clen,
+                                            const long long *d_woff, const int *d_crank,
+                                            const int *d_tile_contig, const int *d_tile_start, int ntiles,
+                                            unsigned long long *d_buck1024, unsigned *d_bin_start, long long nf,
+                                            int fsh, unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
+                                            unsigned plo, unsigned phi, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  int rc = init_tables();
+  if (rc) return rc;
+  CUDA_TRY(cudaMemsetAsync(d_buck1024,0,1025*8,st));
+  CUDA_TRY(cudaMemsetAsync(d_bin_start,0,sizeof(unsigned)*nf,st));
+  if (ntiles > 0)
+    { syncmer_bin_count_kernel<<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
+                                                           d_tile_contig,d_tile_start,d_buck1024,plo,phi,
+                                                           d_bin_start,fsh);
+      fgb_count_launch(1);
+    }
+  CUDA_TRY(cudaGetLastError());
+  return fgb_dev_exclusive_scan_u32(d_bin_start,nf,d_total,d_tmp,tmp_bytes,st);
+}
+
+//  Pass 2: every record straight into its fine bin of d_records (n records), through cursors that start
+//  as a copy of d_bin_start (d_cursor: nf words); then *d_bad = 1 unless every bin came out exactly full.
+extern "C" int fgb_syncmer_scatter_device(const void *d_seq, const long long *d_clen,
+                                          const long long *d_woff, const int *d_crank,
+                                          const int *d_tile_contig, const int *d_tile_start, int ntiles,
+                                          const unsigned *d_bin_start, unsigned *d_cursor, long long nf, int fsh,
+                                          long long n, void *d_records, unsigned *d_bad, unsigned plo,
+                                          unsigned phi, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  CUDA_TRY(cudaMemcpyAsync(d_cursor,d_bin_start,sizeof(unsigned)*nf,cudaMemcpyDeviceToDevice,st));
+  CUDA_TRY(cudaMemsetAsync(d_bad,0,sizeof(unsigned),st));
+  if (ntiles > 0)
+    { syncmer_scatter_kernel<<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
+                                                         d_tile_contig,d_tile_start,(rec128 *) d_records,
+                                                         (unsigned) n,plo,phi,d_cursor,fsh);
+      fgb_count_launch(1);
+    }
+  if (nf > 0)
+    { kmer_scatter_check_kernel<<<(unsigned) ((nf + 255) / 256),256,0,st>>>(d_cursor,d_bin_start,nf,(unsigned) n,d_bad);
+      fgb_count_launch(1);
+    }
   CUDA_TRY(cudaGetLastError());
   return FGB_OK;
 }

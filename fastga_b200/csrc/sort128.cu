@@ -546,14 +546,19 @@ extern "C" int fgb_sort_seeds64_device(void *d_a, void *d_b, long long n, int bi
  *  k-mers by (strand|contig rank, post), i.e. by the whole 128-bit value.
  *
  *  Ten full Onesweep passes move 10 x 32 bytes per record through HBM.  Instead:
- *    1. two Onesweep passes on the two MOST significant key bytes (byte 14 then 15) leave the
- *       records partitioned into 65536 prefix bins;
+ *    1. the records are laid out by prefix bin: bin p at [bins[p], bins[p+1]), in any order inside
+ *       the bin.  A table built from a genome gets that layout from the scan itself (the count pass
+ *       counts per bin, the emit pass scatters into the bins: fgb_kmer_sort_fine_binned_device);
+ *       records from elsewhere get it from two Onesweep partition passes on the two MOST
+ *       significant key bytes (fgb_kmer_sort_range_device);
  *    2. consecutive bins are packed into groups of at most BK_CAP records and BK_SPAN bins; one
  *       CTA per group pulls the group into shared memory with one TMA bulk copy, sorts it there
  *       (kmer_bucket_sort_kernel) and writes it back once;
  *    3. bins larger than BK_CAP (repeats) are compacted, sorted with the generic Onesweep sort and
  *       copied back.
- *  HBM traffic per record: 2 x 32 + 32 bytes instead of 10 x 32.
+ *  Every record is unique (contig, strand and post differ) and steps 2 and 3 order a bin by the whole
+ *  128-bit value, so the order records arrive in inside a bin does not change the table.
+ *  HBM traffic per record after the layout: 32 bytes (10 x 32 for a full LSD sort).
  **********************************************************************************************/
 
 #define BK_THREADS SORT_THREADS
@@ -592,7 +597,8 @@ extern "C" int fgb_kmer_bins_device(const void *d_tab, long long n, int binshift
 
 __global__ void __launch_bounds__(BK_THREADS,2)
 kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
-                        const uint2 *__restrict__ groups /* start, count */, int binshift)
+                        const uint4 *__restrict__ groups /* start, count, hi >> binshift of its first bin */,
+                        int binshift)
 { extern __shared__ __align__(16) unsigned char smem_raw[];
   rec128   *tile   = reinterpret_cast<rec128 *>(smem_raw);
   unsigned *cnt    = reinterpret_cast<unsigned *>(tile + BK_CAP);        // [BK_NSUB+1]; LSD path: wcount[BK_WARPS][256]
@@ -601,7 +607,7 @@ kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
   __shared__ __align__(8) unsigned long long tbar;
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint2 g = groups[blockIdx.x];
+  const uint4 g = groups[blockIdx.x];
   const int count = (int) g.y;
   if (tid == 0)
     { mbar_init(&tbar,1);
@@ -614,7 +620,7 @@ kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
   rec128   r[BK_ITEMS];
   unsigned sub[BK_ITEMS], off[BK_ITEMS];
   const int base = w*(32*BK_ITEMS);
-  const unsigned b0 = (unsigned) (tile[0].hi >> binshift);
+  const unsigned b0 = g.z;                     // not tile[0]'s bin: a bin's records come in any order
   const int subshift = binshift - BK_SUBBITS;
 #pragma unroll
   for (int it = 0; it < BK_ITEMS; it++)
@@ -751,39 +757,29 @@ __global__ void kmer_copy_segments_kernel(const rec128 *__restrict__ src, rec128
 
 static const size_t BUCKET_SMEM = BK_CAP*sizeof(rec128) + (BK_NSUB + 32 + 256 + BK_WARPS)*sizeof(unsigned);
 
-//  d_a: n records in emit order; d_b: scratch of the same size.  Sorted table lands in d_a or d_b
-//  (*result_in_b).  d_tmp as for fgb_sort128_device.  Synchronises the stream once (the bin
-//  boundaries come to the host to pack the groups).
-
-//  [plo,phi): the range of 12-base prefixes the records come from (the whole space, or one
-//  rank's share of a cooperatively built table).  The 65536 bins always tile THAT range, so a share
-//  is binned as finely as a whole table of the same size (bins of 16 + log2(2^24/range) top bits;
-//  one more partition pass when that exceeds two bytes).
-
-extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                                          void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  *result_in_b = 0;
-  if (n <= 1) return FGB_OK;
-  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
-  if (phi <= plo || phi > (1u << 24)) return FGB_ERR_ARG;
-  //  as many bins as keep the average bin near 1.5 K records (a CTA sorts <= BK_CAP in shared memory):
-  //  65536 up to ~100 M records, one more power of two per doubling beyond (a 1 Gbp genome: 2^19)
-  long long maxbins = 65536, target = 1536;
+//  The bins of n records whose 12-base prefixes lie in [plo,phi) (the whole space, or one rank's share
+//  of a cooperatively built table): bin = (prefix24 >> sh) - (plo >> sh).  The bins always tile THAT
+//  range, so a share is binned as finely as a whole table of the same size.  As many bins as keep the
+//  average bin near 1.5 K records (a CTA sorts <= BK_CAP in shared memory): 65536 up to ~100 M records,
+//  one more power of two per doubling beyond (a 1 Gbp genome: 2^19).  sh never grows with n, so the
+//  bins chosen for an upper bound of n refine the bins chosen for n.
+extern "C" int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi)
+{ long long maxbins = 65536, target = 1536;
   if (getenv("FGB_KSORT_BIN_TARGET") != NULL) target = atoll(getenv("FGB_KSORT_BIN_TARGET"));   // tests: force more bins
   if (target < 1) target = 1;
   while (maxbins < (1ll << 24) && n / maxbins > target) maxbins <<= 1;
-  int sh = 0;                                            // bins = ((prefix24 - plo') >> sh), plo' = plo rounded down
+  int sh = 0;
   while ((long long) ((((unsigned long long) (phi - 1) >> sh) - ((unsigned long long) plo >> sh))) >= maxbins) sh += 1;
-  const int binshift = 40 + sh;                          // prefix24 = hi >> 40
-  const unsigned long long base = (unsigned long long) plo >> sh;
-  const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
-  int inb = 0;
-  //  partition passes: 8-bit digits over the bins' bits (the top 24 - sh bits of the k-mer)
-  int rc = fgb_sort128_bits_device(d_a,d_b,n,64 + binshift,128,d_tmp,tmp_bytes,&inb,st);
-  if (rc) return rc;
-  rec128 *src = (rec128 *) (inb ? d_b : d_a), *dst = (rec128 *) (inb ? d_a : d_b);
+  return sh;
+}
 
+//  Sorts the records of src laid out by bin (bin p at [bins[p], bins[p+1]), any order inside a bin;
+//  bins on the host, nbins+1 entries) into dst.  Synchronises the stream.
+static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins, long long nbins, int sh,
+                            unsigned plo, cudaStream_t st)
+{ const int binshift = 40 + sh;                          // prefix24 = hi >> 40
+  const unsigned base = plo >> sh;
+  int rc = FGB_OK;
   static bool attr_set = false;
   if (!attr_set)
     { CUDA_TRY(cudaFuncSetAttribute(kmer_bucket_sort_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -791,17 +787,7 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
       attr_set = true;
     }
 
-  unsigned *d_bins = NULL;
-  CUDA_TRY(fgb_dmalloc((void **) &d_bins,sizeof(unsigned)*(size_t) (nbins+1),st));
-  { int nb = (int) ((n + 1 + 255) / 256);
-    kmer_bins_kernel<<<nb,256,0,st>>>(src,n,binshift,base,d_bins,nbins);
-    fgb_count_launch(1);
-  }
-  std::vector<unsigned> bins((size_t) nbins + 1);
-  CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*(size_t) (nbins+1),cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-
-  std::vector<uint2> groups;
+  std::vector<uint4> groups;
   std::vector<unsigned> ofrom, opre;                    // oversized bins: start, prefix of lengths
   unsigned ototal = 0;
   { unsigned gs = bins[0], gc = 0; long long gp = 0;           // group start record, size, first bin
@@ -809,22 +795,22 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
       { unsigned len = bins[p+1] - bins[p];
         if (len == 0) continue;
         if (len > BK_CAP)
-          { if (gc) { groups.push_back(make_uint2(gs,gc)); gc = 0; }
+          { if (gc) { groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0)); gc = 0; }
             ofrom.push_back(bins[p]); opre.push_back(ototal); ototal += len;
             continue;
           }
         if (gc != 0 && (gc + len > BK_CAP || p - gp >= BK_SPAN))
-          { groups.push_back(make_uint2(gs,gc)); gc = 0; }
+          { groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0)); gc = 0; }
         if (gc == 0) { gs = bins[p]; gp = p; }
         gc += len;
       }
-    if (gc) groups.push_back(make_uint2(gs,gc));
+    if (gc) groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0));
   }
 
-  uint2 *d_groups = NULL;
+  uint4 *d_groups = NULL;
   if (!groups.empty())
-    { CUDA_TRY(fgb_dmalloc((void **) &d_groups,sizeof(uint2)*groups.size(),st));
-      CUDA_TRY(cudaMemcpyAsync(d_groups,groups.data(),sizeof(uint2)*groups.size(),cudaMemcpyHostToDevice,st));
+    { CUDA_TRY(fgb_dmalloc((void **) &d_groups,sizeof(uint4)*groups.size(),st));
+      CUDA_TRY(cudaMemcpyAsync(d_groups,groups.data(),sizeof(uint4)*groups.size(),cudaMemcpyHostToDevice,st));
       kmer_bucket_sort_kernel<<<(unsigned) groups.size(),BK_THREADS,BUCKET_SMEM,st>>>(src,dst,d_groups,binshift);
       fgb_count_launch(1);
       CUDA_TRY(cudaGetLastError());
@@ -854,8 +840,70 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
       fgb_dfree(d_c1,st); fgb_dfree(d_c2,st); fgb_dfree(d_ctmp,st); fgb_dfree(d_seg,st);
     }
   CUDA_TRY(cudaStreamSynchronize(st));
-  fgb_dfree(d_bins,st); if (d_groups) fgb_dfree(d_groups,st);
+  if (d_groups) fgb_dfree(d_groups,st);
+  return FGB_OK;
+}
+
+//  d_a: n records in any order; d_b: scratch of the same size.  Sorted table lands in d_a or d_b
+//  (*result_in_b).  d_tmp as for fgb_sort128_device.  Partition passes (8-bit digits over the bins'
+//  bits, the top 24 - sh bits of the k-mer: one more pass when that exceeds two bytes) lay the records
+//  out by bin; synchronises the stream once more than kmer_sort_binned (the bin boundaries come to the
+//  host to pack the groups).
+extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
+                                          void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  *result_in_b = 0;
+  if (n <= 1) return FGB_OK;
+  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
+  if (phi <= plo || phi > (1u << 24)) return FGB_ERR_ARG;
+  const int sh = fgb_kmer_bin_shift(n,plo,phi);
+  const int binshift = 40 + sh;
+  const unsigned long long base = (unsigned long long) plo >> sh;
+  const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
+  int inb = 0;
+  int rc = fgb_sort128_bits_device(d_a,d_b,n,64 + binshift,128,d_tmp,tmp_bytes,&inb,st);
+  if (rc) return rc;
+  rec128 *src = (rec128 *) (inb ? d_b : d_a), *dst = (rec128 *) (inb ? d_a : d_b);
+
+  unsigned *d_bins = NULL;
+  CUDA_TRY(fgb_dmalloc((void **) &d_bins,sizeof(unsigned)*(size_t) (nbins+1),st));
+  { int nb = (int) ((n + 1 + 255) / 256);
+    kmer_bins_kernel<<<nb,256,0,st>>>(src,n,binshift,base,d_bins,nbins);
+    fgb_count_launch(1);
+  }
+  std::vector<unsigned> bins((size_t) nbins + 1);
+  CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*(size_t) (nbins+1),cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  fgb_dfree(d_bins,st);
+  rc = kmer_sort_binned(src,dst,bins.data(),nbins,sh,plo,st);
+  if (rc) return rc;
   *result_in_b = inb ^ 1;
+  return FGB_OK;
+}
+
+//  d_a: n records the syncmer scan scattered by FINE bin, (prefix24 >> fsh) - (plo >> fsh) at
+//  [fstart[f], fstart[f+1]) (fstart on the host, nf+1 entries), with fsh chosen for an upper bound of n.
+//  A bin of the rule for n is a run of whole fine bins, so d_a is already laid out by bin and goes
+//  straight to the bucket sort.  Sorted table lands in d_b (*result_in_b = 1), or stays in d_a when n <= 1.
+extern "C" int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
+                                                const unsigned *fstart, long long nf, int fsh, int *result_in_b,
+                                                void *stream)
+{ *result_in_b = 0;
+  if (n <= 1) return FGB_OK;
+  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
+  if (phi <= plo || phi > (1u << 24)) return FGB_ERR_ARG;
+  const int sh = fgb_kmer_bin_shift(n,plo,phi);
+  if (sh < fsh || (long long) fstart[nf] != n) return FGB_ERR_ARG;
+  const unsigned long long base = (unsigned long long) plo >> sh, fbase = (unsigned long long) plo >> fsh;
+  const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
+  std::vector<unsigned> bins((size_t) nbins + 1);
+  for (long long p = 0; p <= nbins; p++)
+    { long long f = (long long) ((base + p) << (sh - fsh)) - (long long) fbase;     // first fine bin of bin p
+      bins[p] = fstart[f < 0 ? 0 : (f > nf ? nf : f)];
+    }
+  int rc = kmer_sort_binned((const rec128 *) d_a,(rec128 *) d_b,bins.data(),nbins,sh,plo,(cudaStream_t) stream);
+  if (rc) return rc;
+  *result_in_b = 1;
   return FGB_OK;
 }
 
