@@ -2237,18 +2237,24 @@ extend_kernel(ext_params P)
 
 struct la_job { int actg, bctg, comp, low, hgh, anti, lbord, hbord; };
 
+//  W = EX_W: wave state in shared memory.  W = EX_WBIG: the retry of the calls whose band outgrew that
+//  (or whose arenas overflowed), wave state in HBM (P.bigstate); idx then lists the calls to run.
+template<int W>
 __global__ void __launch_bounds__(EX_WARPS*32,EX_MINBLK)
-la_batch_kernel(ext_params P, const la_job *__restrict__ jobs, int njobs, int *__restrict__ status)
+la_batch_kernel(ext_params P, const la_job *__restrict__ jobs, const unsigned *__restrict__ idx, int njobs,
+                int *__restrict__ status)
 { unsigned char *const smem = ex_smem;
   const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
   const long long gw = (long long) blockIdx.x * EX_WARPS + wp;
-  unsigned char *sb = smem + (size_t) wp * STATE_BYTES;
+  unsigned char *sb = (W == EX_W) ? (smem + (size_t) wp * STATE_BYTES)
+                                  : (P.bigstate + (size_t) gw * WSTATE_BYTES(EX_WBIG));
   Ctx c;
   c.T  = (u64 *) sb;
-  c.V  = (int *) (sb + EX_W*8);
-  c.HA = c.V + EX_W; c.HM = c.HA + EX_W; c.NA = c.HM + EX_W;
-  c.carry = c.NA + EX_W;
-  c.pwin = (Peb *) (sb + WSTATE_BYTES(EX_W)); c.pwin_n = 64;
+  c.V  = (int *) (sb + W*8);
+  c.HA = c.V + W; c.HM = c.HA + W; c.NA = c.HM + W;
+  c.carry = c.NA + W;
+  c.pwin = (W == EX_W) ? (Peb *) (sb + WSTATE_BYTES(EX_W)) : (Peb *) (smem + (size_t) wp * BIG_SMEM_PER_WARP);
+  c.pwin_n = 64;
   c.ttab = P.table; c.sc15 = TRIM_LEN * P.dscore;
   c.box = NULL; c.box_off = 0;
   c.cells = P.cells + gw * P.cells_per_warp;
@@ -2264,13 +2270,14 @@ la_batch_kernel(ext_params P, const la_job *__restrict__ jobs, int njobs, int *_
       if (lane == 0) w = atomicAdd(P.queue,1u);
       w = __shfl_sync(FULL,w,0);
       if (w >= (unsigned) njobs) break;
+      if (idx != NULL) w = idx[w];
       const la_job J = jobs[w];
       c.A = (const unsigned *) ((J.comp ? P.arseq : P.aseq) + P.awoff[J.actg]);
       c.B = (const unsigned *) (P.bseq + P.bwoff[J.bctg]);
       c.alen = (int) P.aclen[J.actg]; c.blen = (int) P.bclen[J.bctg];
       c.anw = (c.alen + 31) >> 5; c.bnw = (c.blen + 31) >> 5;
       LAres R;
-      int st = local_alignment<EX_W>(c,J.comp,J.low,J.hgh,J.anti,R,J.lbord,J.hbord);
+      int st = local_alignment<W>(c,J.comp,J.low,J.hgh,J.anti,R,J.lbord,J.hbord);
       if (st == ST_OK) emit_record(P,c,R,J.comp,w,0,0u);
       if (lane == 0) status[w] = st;
       __syncwarp();
@@ -2910,7 +2917,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
 //  jobs: n x 8 ints (A contig, B contig, comp, low, hgh, anti, lbord, hbord) -- the arguments of
 //  Local_Alignment with aseq/bseq = those contigs (A reverse-complemented and ACOMP_FLAG set when comp,
 //  as align_contigs calls it, FastGA.c:3184-3260).  paths: n x 7 ints (abpos bbpos aepos bepos diffs tlen
-//  status), status 0 or the ST_* code of a call that did not fit the device arenas; toff: n offsets into
+//  status), status 0 (a call that did not fit the shared-memory wave state or the arenas is re-run on the
+//  wide-band kernel; one that never fits fails the whole call with FGB_ERR_OVERFLOW); toff: n offsets into
 //  `traces` (uint8 pairs, what Compress_TraceTo8 leaves).  traces_cap bytes are available; *traces_used
 //  returns the bytes needed (call again with a larger buffer if it exceeds the capacity).
 extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, long long n, const int *jobs,
@@ -2942,13 +2950,14 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   const int stage_bytes = 1 << 16;
   const size_t smem = (size_t) EX_WARPS * STATE_BYTES;
   short *d_tables = NULL; la_job *d_jobs = NULL; int *d_status = NULL; unsigned *d_misc = NULL;
-  Peb *d_cells = NULL; unsigned char *d_stage = NULL, *d_out = NULL;
+  Peb *d_cells = NULL; unsigned char *d_stage = NULL, *d_out = NULL, *d_big = NULL; unsigned *d_idx = NULL;
+  long long cells_big = cells_per_warp; int stage_big = stage_bytes;
   std::vector<unsigned char> h;
   std::vector<int> hs(n);
   u64 out_cap = (u64) n * 256 + (u64) traces_cap + (1ull << 20), out_used = 0;
   int rc = FGB_OK;
 #define LA_TRY(call) do { if ((call) != cudaSuccess) { rc = FGB_ERR_CUDA; goto done; } } while (0)
-  LA_TRY(cudaFuncSetAttribute(la_batch_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
+  LA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
   LA_TRY(fgb_dmalloc((void **) &d_tables,65536*sizeof(short),st));
   LA_TRY(fgb_dmalloc((void **) &d_jobs,sizeof(la_job)*(size_t) n,st));
   LA_TRY(fgb_dmalloc((void **) &d_status,sizeof(int)*(size_t) n,st));
@@ -2964,13 +2973,49 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   P.stage = d_stage; P.stage_bytes = stage_bytes;
   P.out = d_out; P.out_cap = out_cap; P.out_used = (u64 *) (d_misc + 4);
   P.queue = d_misc + 1;
-  la_batch_kernel<<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P,d_jobs,(int) n,d_status);
+  la_batch_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P,d_jobs,NULL,(int) n,d_status);
   fgb_count_launch(1);
   LA_TRY(cudaGetLastError());
   LA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
   LA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
   LA_TRY(cudaStreamSynchronize(st));
   if (out_used > out_cap) { rc = FGB_ERR_OVERFLOW; goto done; }
+  //  calls that did not fit (a band wider than EX_W diagonals, a full arena): again on the wide-band
+  //  kernel with the wave state in HBM, growing the arenas each round, as fgb_extend re-runs its triples.
+  //  A failed call emitted nothing, so its record comes from the round that completes it.
+  for (int attempt = 1; ; attempt++)
+    { std::vector<unsigned> redo;
+      for (long long i = 0; i < n; i++)
+        if (hs[i] != ST_OK) redo.push_back((unsigned) i);
+      if (redo.empty()) break;
+      if (attempt > 4) { rc = FGB_ERR_OVERFLOW; goto done; }
+      if (attempt > 1) { cells_big *= 8; stage_big *= 4; }
+      const size_t smem_big = (size_t) EX_WARPS * BIG_SMEM_PER_WARP;
+      long long nb2 = ((long long) redo.size() + EX_WARPS - 1) / EX_WARPS;
+      if (nb2 > nsm) nb2 = nsm;
+      long long maxb = (24ll << 30) / ((long long) sizeof(Peb) * cells_big * EX_WARPS);
+      if (nb2 > maxb) nb2 = maxb > 1 ? maxb : 1;
+      const long long nw2 = nb2 * EX_WARPS;
+      fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_big,st); fgb_dfree(d_idx,st);
+      d_cells = NULL; d_stage = NULL; d_big = NULL; d_idx = NULL;
+      LA_TRY(fgb_dmalloc((void **) &d_cells,sizeof(Peb)*cells_big*nw2,st));
+      LA_TRY(fgb_dmalloc((void **) &d_stage,2ll*stage_big*nw2,st));
+      LA_TRY(fgb_dmalloc((void **) &d_big,(size_t) nw2 * WSTATE_BYTES(EX_WBIG),st));
+      LA_TRY(fgb_dmalloc((void **) &d_idx,sizeof(unsigned)*redo.size(),st));
+      LA_TRY(cudaMemcpyAsync(d_idx,redo.data(),sizeof(unsigned)*redo.size(),cudaMemcpyHostToDevice,st));
+      LA_TRY(cudaMemsetAsync(d_misc + 1,0,4,st));                 // queue
+      LA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
+      P.cells = d_cells; P.cells_per_warp = cells_big;
+      P.stage = d_stage; P.stage_bytes = stage_big;
+      P.bigstate = d_big;
+      la_batch_kernel<EX_WBIG><<<(unsigned) nb2,EX_WARPS*32,smem_big,st>>>(P,d_jobs,d_idx,(int) redo.size(),d_status);
+      fgb_count_launch(1);
+      LA_TRY(cudaGetLastError());
+      LA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
+      LA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
+      LA_TRY(cudaStreamSynchronize(st));
+      if (out_used > out_cap) { rc = FGB_ERR_OVERFLOW; goto done; }
+    }
   h.resize((size_t) out_used + 64);
   LA_TRY(cudaMemcpy(h.data(),d_out,out_used,cudaMemcpyDeviceToHost));
   { long long used = 0;
@@ -2995,7 +3040,7 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
 done:
 #undef LA_TRY
   fgb_dfree(d_tables,st); fgb_dfree(d_jobs,st); fgb_dfree(d_status,st); fgb_dfree(d_misc,st);
-  fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_out,st);
+  fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_out,st); fgb_dfree(d_big,st); fgb_dfree(d_idx,st);
   return rc;
 }
 

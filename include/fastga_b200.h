@@ -146,9 +146,10 @@ int  fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B,
 /* the align.h seam proper: Local_Alignment (align.c:1423; align.h:262-298) for a batch of call tuples.
  * jobs: n x 8 ints (A contig, B contig, comp, low, hgh, anti, lbord, hbord) = the arguments
  * align_contigs passes with aseq/bseq = those contigs (comp: A reverse-complemented + ACOMP_FLAG,
- * FastGA.c:3184-3260).  paths: n x 7 ints (abpos bbpos aepos bepos diffs tlen status; status != 0: the
- * call did not fit the device arenas); traces: uint8 (diff, B-advance) pairs at toff[i], as
- * Compress_TraceTo8 leaves them.  FGB_ERR_OVERFLOW with *traces_used set: call again with more room. */
+ * FastGA.c:3184-3260).  paths: n x 7 ints (abpos bbpos aepos bepos diffs tlen status; status is 0: a
+ * call whose band or arenas outgrow the shared-memory kernel is re-run on the wide-band kernel);
+ * traces: uint8 (diff, B-advance) pairs at toff[i], as Compress_TraceTo8 leaves them.
+ * FGB_ERR_OVERFLOW with *traces_used set: call again with more room. */
 int  fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, long long n, const int *jobs,
                           const short *tables, int ave_path, int tspace,
                           int *paths, long long *toff, unsigned char *traces, long long traces_cap,

@@ -159,9 +159,10 @@ def reference(key, inputs, compute):
     return g["result"]
 
 
-def ref_alignments(wd, a, b, threads=8):
-    """FastGA -v -k -T<n> -1:ref a [b] in workdir: -v counters + count and md5 of the canonical records"""
-    st = parse_fastga_log(ref_fastga(wd, a, b, threads=threads))
+def ref_alignments(wd, a, b, threads=8, extra=()):
+    """FastGA -v -k -T<n> -1:ref <extra> a [b] in workdir: -v counters + count and md5 of the canonical
+    records"""
+    st = parse_fastga_log(ref_fastga(wd, a, b, threads=threads, extra=extra))
     recs = oneview_records(os.path.join(wd, "ref.1aln"))
     st.update(records=len(recs), aln_md5=md5_lines(recs))
     return st
@@ -183,8 +184,8 @@ def path_key(abpos, bbpos, aepos, bepos, diffs, tlen, trace):
     return hashlib.md5(h + np.asarray(trace).astype(np.uint8).tobytes()).hexdigest()[:12]
 
 
-def ref_local_alignments(calls, freq):
-    """path_key of the reference's Local_Alignment (libfastga_ref.so, New_Align_Spec(0.7, 100, freq))
+def ref_local_alignments(calls, freq, ave_corr=0.7):
+    """path_key of the reference's Local_Alignment (libfastga_ref.so, New_Align_Spec(ave_corr, 100, freq))
     for every call (framed a, framed b, comp, low, hgh, anti, lbord, hbord)"""
     ref = C.CDLL(REF_SO)
     ref.New_Work_Data.restype = C.c_void_p
@@ -192,7 +193,7 @@ def ref_local_alignments(calls, freq):
     ref.New_Align_Spec.argtypes = [C.c_double, C.c_int, C.POINTER(C.c_float), C.c_int]
     ref.Local_Alignment.argtypes = [C.POINTER(Alignment), C.c_void_p, C.c_void_p] + [C.c_int] * 5
     work = ref.New_Work_Data()
-    spec = ref.New_Align_Spec(0.7, 100, (C.c_float * 4)(*[float(v) for v in freq]), 0)
+    spec = ref.New_Align_Spec(ave_corr, 100, (C.c_float * 4)(*[float(v) for v in freq]), 0)
     out = []
     for a, b, comp, low, hgh, anti, lb, hb in calls:
         p = Path()
@@ -414,10 +415,11 @@ def oracle_pipeline_self(g, **kw):
     seeds, sumlen = self_merge(t, s, kw.get("freq", 10))
     layout = seed_layout(g, g)
     recs = seed_records(seeds, layout)
+    skw = {k: v for k, v in kw.items() if k in ("chain_break", "chain_min", "align_min", "align_rate")}
     o = orc()
     o.orc_set_self(1)
     try:
-        ov, tp, nhit = search(recs, layout, g, g, pa, pa, g.freq)
+        ov, tp, nhit = search(recs, layout, g, g, pa, pa, g.freq, **skw)
     finally:
         o.orc_set_self(0)
     O = pack_overlaps(ov, tp, ra, ra, layout[2], layout[3])

@@ -1,49 +1,20 @@
 """-m gpu: the align.h seam -- fgb_local_alignments (batched Local_Alignment) against the UNMODIFIED
 reference's Local_Alignment (oracle/_ref/libfastga_ref.so; its results stored in
 tests/golden/reference_runs.json) on random call tuples, borders included."""
-import numpy as np
 import pytest
 
 import oracle_lib as ol
-from fastga_b200 import formats, lib, synth
+from fastga_b200 import formats, lib
+from param_cases import seam_calls, seam_jobs
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.mark.parametrize("borders", [False, True])
 def test_batched_local_alignment_matches_reference(borders):
-    rng = np.random.default_rng(41 + int(borders))
-    ncont = 6
-    A = [rng.integers(0, 4, int(rng.integers(3000, 40000)), dtype=np.uint8) for _ in range(ncont)]
-    B, pad = [], []
-    for a in A:
-        rate = float(rng.choice([0.02, 0.05, 0.1, 0.15]))
-        b = synth.diverged_copy(rng, a, rate, sv_every=0, inversions=False)      # small mutations only
-        pad.append(int(rng.integers(0, 300)))
-        B.append(np.concatenate([rng.integers(0, 4, pad[-1], dtype=np.uint8), b]))
+    A, B, jobs = seam_jobs(41 + int(borders), borders)
     gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
-    jobs = []
-    for _ in range(300):
-        i = int(rng.integers(0, ncont))
-        comp = int(rng.random() < 0.4)
-        la, lb = len(A[i]), len(B[i])
-        x = int(rng.integers(100, la - 100))
-        y = int(np.clip(x + (lb - la) + int(rng.integers(-60, 60)), 50, lb - 50))
-        if comp:                       # the strand-C call sees reverse-complemented A: any diagonal will do
-            y = int(rng.integers(50, lb - 50))
-        d, anti = x - y, x + y
-        low, hgh = d - int(rng.integers(0, 70)), d + int(rng.integers(0, 70))
-        lbd = hbd = -1
-        if borders:
-            lbd = int(rng.integers(0, 40)) if rng.random() < 0.7 else -1
-            hbd = int(rng.integers(0, 40)) if rng.random() < 0.7 else -1
-        jobs.append((i, i, comp, low, hgh, anti, lbd, hbd))
-    jobs = np.array(jobs, dtype=np.int32)
-    fA = [ol._framed(a) for a in A]
-    fAC = [ol._framed(3 - a[::-1]) for a in A]
-    fB = [ol._framed(b) for b in B]
-    calls = [((fAC[i] if comp else fA[i]), fB[j], comp, low, hgh, anti, lbd, hbd)
-             for (i, j, comp, low, hgh, anti, lbd, hbd) in jobs.tolist()]
+    calls = seam_calls(A, B, jobs)
     want = ol.reference("local_alignment/batch%s" % ("_borders" if borders else ""), ol.digest(calls, gA.freq),
                         lambda: ol.ref_local_alignments(calls, gA.freq))
     dA, dB = lib.DeviceGenome(gA, want_revcomp=True), lib.DeviceGenome(gB)

@@ -118,15 +118,28 @@ def _la_calls(seed, borders):
     return calls
 
 
-def _la_compare(seed, borders):
+def _la_compare(seed, borders, ave_corr=0.7, freq=None):
+    """the oracle's Local_Alignment against the reference's on _la_calls(seed, borders); at the default
+    spec (ave_corr .7, uniform freq) under the original keys, else under keys that name both"""
     calls = _la_calls(seed, borders)
-    freq = np.array([.25] * 4, np.float32)
-    want = ol.reference("local_alignment/%d%s" % (seed, "_borders" if borders else ""), ol.digest(calls),
-                        lambda: ol.ref_local_alignments(calls, freq))
+    name = "local_alignment/%d%s" % (seed, "_borders" if borders else "")
+    if freq is None and ave_corr == 0.7:
+        freq = np.array([.25] * 4, np.float32)
+        want = ol.reference(name, ol.digest(calls), lambda: ol.ref_local_alignments(calls, freq))
+    else:
+        freq = np.array([.25] * 4, np.float32) if freq is None else np.asarray(freq, np.float32)
+        name += "_i%.3g_at%.3g" % (ave_corr, float(freq[0]) + float(freq[3]))
+        want = ol.reference(name, ol.digest(calls, ave_corr, freq),
+                            lambda: ol.ref_local_alignments(calls, freq, ave_corr))
+    _la_check_oracle(calls, want, freq, ave_corr)
+
+
+def _la_check_oracle(calls, want, freq, ave_corr):
+    """every call through the oracle's Local_Alignment gives the reference's path_key want[call]"""
     orc = ol.orc()
     orc.orc_local_alignment.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int] + \
         [C.c_int] * 6 + [C.POINTER(OPath)]
-    ospec, _tabs, _ = ol.make_spec(freq, 0.7)
+    ospec, _tabs, _ = ol.make_spec(freq, ave_corr)
     owork = C.c_void_p(orc.orc_new_work())
     for it, (ab, bb, acomp, low, hgh, anti, lb, hb) in enumerate(calls):
         op = OPath()
