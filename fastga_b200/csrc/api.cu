@@ -156,6 +156,19 @@ extern "C" void fgb_release_cache()
   g_free.clear();
 }
 
+//  Blocks of the cache handed to the caller (the sharded path's exchange buffers).
+extern "C" int fgb_device_alloc(long long bytes, void **out, void *stream)
+{ CUDA_TRY(fgb_dmalloc(out,(size_t) (bytes > 0 ? bytes : 16),(cudaStream_t) stream)); return FGB_OK; }
+extern "C" void fgb_device_free(void *p) { fgb_dfree(p,0); }
+
+//  Bytes of the blocks handed out and not yet given back (size classes, as the cache counts them).
+extern "C" long long fgb_device_live_bytes()
+{ std::lock_guard<std::mutex> g(g_mem_lock);
+  long long s = 0;
+  for (auto &kv : g_live) s += (long long) kv.second;
+  return s;
+}
+
 extern "C" void fgb_timings_reset() { memset(&g_timings,0,sizeof(g_timings)); }
 extern "C" void fgb_timings_get(fgb_timings *out) { *out = g_timings; }
 
@@ -174,7 +187,7 @@ extern "C" int fgb_genome_create(const unsigned char *bps, long long bps_bytes, 
                                  fgb_genome **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (ncontig <= 0 || ncontig > 0x7fff) return FGB_ERR_LIMIT;   // contig rank is a 15-bit field
-  fgb_genome *g = new fgb_genome();
+  std::unique_ptr<fgb_genome> g(new fgb_genome());
   g->ncontig = ncontig;
   g->clen.assign(clen,clen+ncontig);
   g->boff.assign(boff,boff+ncontig);
@@ -182,7 +195,7 @@ extern "C" int fgb_genome_create(const unsigned char *bps, long long bps_bytes, 
   g->seqtot = 0; g->maxlen = 0;
   long long w = 2;                             // 16 zero bytes ahead of the first contig too
   for (int c = 0; c < ncontig; c++)
-    { if (clen[c] >= 0x7fffffffll) { delete g; return FGB_ERR_LIMIT; }
+    { if (clen[c] >= 0x7fffffffll) return FGB_ERR_LIMIT;
       g->woff[c] = w;
       w += ((clen[c] + 31) >> 5) + 2;          // zero pad so 64-bit window reads stay inside
       w = (w + 1) & ~1ll;                      // 16-byte alignment of every contig
@@ -198,16 +211,16 @@ extern "C" int fgb_genome_create(const unsigned char *bps, long long bps_bytes, 
   qsort(g->perm.data(),ncontig,sizeof(int),LSORT);     // same libc call as GIXmake.c:1959
   for (int c = 0; c < ncontig; c++) g->crank[g->perm[c]] = c;
 
-  unsigned char *d_bps = NULL;
-  long long *d_boff = NULL;
-  CUDA_TRY(fgb_dmalloc((void **) &d_bps,bps_bytes + 16,st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_boff,sizeof(long long)*ncontig,st));
-  CUDA_TRY(fgb_dmalloc((void **) &g->d_clen,sizeof(long long)*ncontig,st));
-  CUDA_TRY(fgb_dmalloc((void **) &g->d_woff,sizeof(long long)*(ncontig+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &g->d_crank,sizeof(int)*ncontig,st));
-  CUDA_TRY(fgb_dmalloc((void **) &g->d_perm,sizeof(int)*ncontig,st));
-  CUDA_TRY(fgb_dmalloc((void **) &g->d_seq,sizeof(u64)*(w + 1024),st));      // slack: the extension stages 1 KB tiles that may start near a contig end
-  if (want_revcomp) CUDA_TRY(fgb_dmalloc((void **) &g->d_rseq,sizeof(u64)*(w + 1024),st));
+  dblock<unsigned char> d_bps;
+  dblock<long long> d_boff;
+  CUDA_TRY(d_bps.alloc(bps_bytes + 16,st));
+  CUDA_TRY(d_boff.alloc(ncontig,st));
+  CUDA_TRY(g->d_clen.alloc(ncontig,st));
+  CUDA_TRY(g->d_woff.alloc(ncontig+1,st));
+  CUDA_TRY(g->d_crank.alloc(ncontig,st));
+  CUDA_TRY(g->d_perm.alloc(ncontig,st));
+  CUDA_TRY(g->d_seq.alloc(w + 1024,st));      // slack: the extension stages 1 KB tiles that may start near a contig end
+  if (want_revcomp) CUDA_TRY(g->d_rseq.alloc(w + 1024,st));
   { stage_timer t(&g_timings.h2d_ms,st);
     CUDA_TRY(cudaMemcpyAsync(d_bps,bps,bps_bytes,cudaMemcpyHostToDevice,st));
     CUDA_TRY(cudaMemcpyAsync(d_boff,boff,sizeof(long long)*ncontig,cudaMemcpyHostToDevice,st));
@@ -222,19 +235,12 @@ extern "C" int fgb_genome_create(const unsigned char *bps, long long bps_bytes, 
     rc = fgb_stage_genome_device(d_bps,d_boff,g->d_clen,g->d_woff,ncontig,w,g->d_seq,g->d_rseq,st);
   }
   CUDA_TRY(cudaStreamSynchronize(st));
-  fgb_dfree(d_bps,st); fgb_dfree(d_boff,st);
-  if (rc) { delete g; return rc; }
-  *out = g;
+  if (rc) return rc;
+  *out = g.release();
   return FGB_OK;
 }
 
-extern "C" void fgb_genome_free(fgb_genome *g)
-{ cudaStream_t st = 0;
-  if (!g) return;
-  fgb_dfree(g->d_clen,st); fgb_dfree(g->d_woff,st); fgb_dfree(g->d_crank,st); fgb_dfree(g->d_perm,st);
-  fgb_dfree(g->d_seq,st); fgb_dfree(g->d_rseq,st);
-  delete g;
-}
+extern "C" void fgb_genome_free(fgb_genome *g) { delete g; }
 
 extern "C" int fgb_genome_perm(const fgb_genome *g, int *perm_out)
 { memcpy(perm_out,g->perm.data(),sizeof(int)*g->ncontig); return FGB_OK; }
@@ -254,12 +260,7 @@ extern "C" long long fgb_genome_words(const fgb_genome *g) { return g->total_wor
  *  GIX
  **********************************************************************************************/
 
-extern "C" void fgb_gix_free(fgb_gix *x)
-{ cudaStream_t st = 0;
-  if (!x) return;
-  fgb_dfree(x->d_tab,st); fgb_dfree(x->d_pstart,st); fgb_dfree(x->d_adj,st);
-  delete x;
-}
+extern "C" void fgb_gix_free(fgb_gix *x) { delete x; }
 
 static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-1901
 { long long cum;
@@ -276,20 +277,6 @@ static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-
 #define GIX_NO_INDEX 0x40000000u     // table only: no prefix index, no LCP bytes (the T1 side of a merge reads neither)
 
 static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi, fgb_gix **out, void *stream);
-
-//  a table handle (and, with it, its device blocks) is released on every way out of the call that
-//  builds it unless it was handed to the caller; likewise loose device blocks
-struct gix_scope
-{ fgb_gix *x;
-  explicit gix_scope(fgb_gix *p) : x(p) {}
-  fgb_gix *release() { fgb_gix *p = x; x = NULL; return p; }
-  ~gix_scope() { if (x != NULL) fgb_gix_free(x); }
-};
-struct blk_scope
-{ std::vector<void **> slots;
-  template<class T> void own(T *&p) { slots.push_back((void **) &p); }
-  ~blk_scope() { for (void **s : slots) if (*s != NULL) { fgb_dfree(*s,0); *s = NULL; } }
-};
 
 extern "C" int fgb_gix_build(const fgb_genome *g, fgb_gix **out, void *stream)
 { return gix_build_range(g,0u,1u << 24,out,stream); }
@@ -321,7 +308,7 @@ struct fine_bins
 //  bin, at the resolution the k-mer sort would pick for an upper bound of n (two records per scanned
 //  position), and the emit pass writes each record straight into its bin; fb gets the bins.
 static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo, unsigned phi_flags,
-                    rec128 **d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
+                    dblock<rec128> &d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
                     fine_bins *fb, cudaStream_t st)
 { int T = fgb_sc_tile();
   std::vector<int> tc, ts;
@@ -333,13 +320,13 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
           { tc.push_back(c); ts.push_back((int) t0); }
       }
   int ntiles = (int) tc.size();
-  int *d_tc = NULL, *d_ts = NULL; unsigned *d_cnt = NULL;
-  u64 *d_buck = NULL, *d_total = NULL; void *d_tmp = NULL;
-  unsigned *d_fb = NULL, bad = 0;          // fine bins: starts [0,nf), cursors [nf,2nf), check flag [2nf]
+  dblock<int> d_tc, d_ts; dblock<unsigned> d_cnt;
+  dblock<u64> d_buck, d_total; dblock<unsigned char> d_tmp;
+  dblock<unsigned> d_fb;                   // fine bins: starts [0,nf), cursors [nf,2nf), check flag [2nf]
+  unsigned bad = 0;
   long long nf = 0;
-  rec128 *d_a = NULL;
   long long tmpb = fgb_dev_scan_tmp_bytes(ntiles);
-  int rc = FGB_OK;
+  int rc;
   u64 total = 0, rdropped = 0;
   if (fb)
     { const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
@@ -348,16 +335,15 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
       fb->nf = nf = (long long) ((((unsigned long long) (bhi - 1)) >> fb->fsh) - ((unsigned long long) plo >> fb->fsh)) + 1;
       tmpb = fgb_dev_scan_tmp_bytes(nf);
     }
-#define GS_TRY(call) do { if ((call) != cudaSuccess) { rc = FGB_ERR_CUDA; goto done; } } while (0)
-  GS_TRY(fgb_dmalloc((void **) &d_tc,sizeof(int)*(ntiles+1),st));
-  GS_TRY(fgb_dmalloc((void **) &d_ts,sizeof(int)*(ntiles+1),st));
-  if (fb) GS_TRY(fgb_dmalloc((void **) &d_fb,sizeof(unsigned)*(2*nf+1),st));
-  else    GS_TRY(fgb_dmalloc((void **) &d_cnt,sizeof(unsigned)*(ntiles+1),st));
-  GS_TRY(fgb_dmalloc((void **) &d_buck,8*1025,st));
-  GS_TRY(fgb_dmalloc((void **) &d_total,8,st));
-  GS_TRY(fgb_dmalloc((void **) &d_tmp,tmpb,st));
-  GS_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
-  GS_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(d_tc.alloc(ntiles+1,st));
+  CUDA_TRY(d_ts.alloc(ntiles+1,st));
+  if (fb) CUDA_TRY(d_fb.alloc(2*nf+1,st));
+  else    CUDA_TRY(d_cnt.alloc(ntiles+1,st));
+  CUDA_TRY(d_buck.alloc(1025,st));
+  CUDA_TRY(d_total.alloc(1,st));
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
+  CUDA_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   { stage_timer t(&g_timings.scan_ms,st);
     if (fb)
       rc = fgb_syncmer_bin_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_fb,nf,
@@ -365,71 +351,67 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
     else
       rc = fgb_syncmer_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,
                                     d_buck,d_total,d_tmp,tmpb,plo,phi_flags,st);
-    if (rc) goto done;
-    GS_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
-    if (buck1024) GS_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
-    GS_TRY(cudaMemcpyAsync(&rdropped,d_buck + 1024,8,cudaMemcpyDeviceToHost,st));
+    if (rc) return rc;
+    CUDA_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
+    if (buck1024) CUDA_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
+    CUDA_TRY(cudaMemcpyAsync(&rdropped,d_buck + 1024,8,cudaMemcpyDeviceToHost,st));
     if (fb)
       { fb->start.resize((size_t) nf + 1);
-        GS_TRY(cudaMemcpyAsync(fb->start.data(),d_fb,sizeof(unsigned)*nf,cudaMemcpyDeviceToHost,st));
+        CUDA_TRY(cudaMemcpyAsync(fb->start.data(),d_fb,sizeof(unsigned)*nf,cudaMemcpyDeviceToHost,st));
       }
-    GS_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaStreamSynchronize(st));
   }
-  if (total >= 0xfffffff0ull) { rc = FGB_ERR_LIMIT; goto done; }
-  GS_TRY(fgb_dmalloc((void **) &d_a,sizeof(rec128)*(total+1),st));
+  if (total >= 0xfffffff0ull) return FGB_ERR_LIMIT;
+  dblock<rec128> d_a;
+  CUDA_TRY(d_a.alloc(total+1,st));
   { stage_timer t(&g_timings.scan_ms,st);
     if (fb)
       { rc = fgb_syncmer_scatter_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_fb,d_fb + nf,nf,
                                         fb->fsh,(long long) total,d_a,d_fb + 2*nf,plo,phi_flags,st);
-        if (!rc && cudaMemcpyAsync(&bad,d_fb + 2*nf,4,cudaMemcpyDeviceToHost,st) != cudaSuccess) rc = FGB_ERR_CUDA;
+        if (rc) return rc;
+        CUDA_TRY(cudaMemcpyAsync(&bad,d_fb + 2*nf,4,cudaMemcpyDeviceToHost,st));
       }
     else
       rc = fgb_syncmer_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,d_a,plo,phi_flags,st);
   }
-  if (rc == FGB_OK && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;   // tc/ts must outlive the copies
-  if (rc == FGB_OK && bad) rc = FGB_ERR_OVERFLOW;        // a bin came out over- or underfull: d_a is not laid out by bin
-  if (rc == FGB_OK && fb) fb->start[nf] = (unsigned) total;
-done:
-#undef GS_TRY
-  fgb_dfree(d_tc,st); fgb_dfree(d_ts,st); fgb_dfree(d_cnt,st); fgb_dfree(d_fb,st); fgb_dfree(d_buck,st);
-  fgb_dfree(d_total,st); fgb_dfree(d_tmp,st);
-  if (rc) { fgb_dfree(d_a,st); return rc; }
-  *d_recs = d_a; *n_out = (long long) total; *nrev = (long long) rdropped;
+  if (rc) return rc;
+  CUDA_TRY(cudaStreamSynchronize(st));                   // tc/ts must outlive the copies
+  if (bad) return FGB_ERR_OVERFLOW;                      // a bin came out over- or underfull: d_a is not laid out by bin
+  if (fb) fb->start[nf] = (unsigned) total;
+  d_recs = std::move(d_a); *n_out = (long long) total; *nrev = (long long) rdropped;
   return FGB_OK;
 }
 
 //  K3/K4: sorts the records in d_a (consumed: it ends up inside the handle or is released) whose
 //  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.  fb: the fine bins the
 //  scan laid d_a out by; NULL: records in any order (the partition passes lay them out).
-static int gix_finish(fgb_gix *x, rec128 *d_a, long long n, unsigned plo, unsigned phi, const fine_bins *fb,
+static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const fine_bins *fb,
                       cudaStream_t st, bool index = true)
-{ rec128 *d_b = NULL; void *d_stmp = NULL;
+{ dblock<rec128> d_b; dblock<unsigned char> d_stmp;
   long long stmpb = fgb_sort128_tmp_bytes(n);
-  int rc = FGB_OK, inb = 0;
+  int rc, inb = 0;
   x->n = n;
-  if (fgb_dmalloc((void **) &d_b,sizeof(rec128)*(n+1),st) != cudaSuccess ||
-      (!fb && fgb_dmalloc((void **) &d_stmp,stmpb,st) != cudaSuccess) ||
-      (index && fgb_dmalloc((void **) &x->d_pstart,sizeof(unsigned)*((1<<24)+1+8),st) != cudaSuccess) ||
-      (index && fgb_dmalloc((void **) &x->d_adj,(size_t) n + 32,st) != cudaSuccess))
-    rc = FGB_ERR_CUDA;
-  if (!rc)
-    { stage_timer t(&g_timings.ksort_ms,st);
-      if (fb)
-        rc = fgb_kmer_sort_fine_binned_device(d_a,d_b,n,plo,phi,fb->start.data(),fb->nf,fb->fsh,&inb,st);
-      else
-        rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
+  CUDA_TRY(d_b.alloc(n+1,st));
+  if (!fb) CUDA_TRY(d_stmp.alloc(stmpb,st));
+  if (index)
+    { CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
+      CUDA_TRY(x->d_adj.alloc((size_t) n + 32,st));
     }
-  if (!rc)
-    { x->d_tab = inb ? d_b : d_a;
-      if (inb) d_b = NULL; else d_a = NULL;
-      if (index)
-        { stage_timer t(&g_timings.index_ms,st);
-          rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
-        }
+  { stage_timer t(&g_timings.ksort_ms,st);
+    if (fb)
+      rc = fgb_kmer_sort_fine_binned_device(d_a,d_b,n,plo,phi,fb->start.data(),fb->nf,fb->fsh,&inb,st);
+    else
+      rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
+  }
+  if (rc) return rc;
+  x->d_tab = std::move(inb ? d_b : d_a);                  // the other side goes back as the call returns
+  if (index)
+    { stage_timer t(&g_timings.index_ms,st);
+      rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
     }
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  fgb_dfree(d_a,st); fgb_dfree(d_b,st); fgb_dfree(d_stmp,st);
-  return rc;
+  if (rc) return rc;
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return FGB_OK;
 }
 
 static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags, fgb_gix **out, void *stream)
@@ -437,19 +419,20 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
   const bool index = !(phi_flags & GIX_NO_INDEX);
   phi_flags &= ~GIX_NO_INDEX;
   const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
-  fgb_gix *x = new fgb_gix();
-  gix_bytes(g,x);
+  std::unique_ptr<fgb_gix> x(new fgb_gix());
+  gix_bytes(g,x.get());
   x->ncontig = g->ncontig;
   x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
-  rec128 *d_a = NULL; long long n = 0, nrev = 0;
+  dblock<rec128> d_a; long long n = 0, nrev = 0;
   //  the scan lays the records out by prefix bin; FGB_KSORT_PARTITION=1 packs them by tile and lays them
   //  out with the Onesweep partition passes instead (both paths can be compared in one process)
   const char *part_env = getenv("FGB_KSORT_PARTITION");
   fine_bins fb, *pfb = (part_env != NULL && atoi(part_env) != 0) ? NULL : &fb;
-  int rc = gix_scan(g,NULL,plo,phi_flags,&d_a,&n,&nrev,x->buck1024,pfb,st);
-  if (!rc) { x->n_both = n + nrev; rc = gix_finish(x,d_a,n,plo,phi,pfb,st,index); }
-  if (rc) { fgb_gix_free(x); return rc; }
-  *out = x;
+  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,pfb,st);
+  if (rc) return rc;
+  x->n_both = n + nrev;
+  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,pfb,st,index))) return rc;
+  *out = x.release();
   return FGB_OK;
 }
 
@@ -460,18 +443,14 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
  *  their A-contig.  Nothing is replicated; the two exchanges are all-to-alls of 16-byte records.
  **********************************************************************************************/
 
-extern "C" int fgb_device_alloc(long long bytes, void **out, void *stream)
-{ CUDA_TRY(fgb_dmalloc(out,(size_t) (bytes > 0 ? bytes : 16),(cudaStream_t) stream)); return FGB_OK; }
-extern "C" void fgb_device_free(void *p) { fgb_dfree(p,0); }
-
 //  unsorted k-mer records of the contigs with mask[c] != 0 (device buffer handed to the caller:
 //  fgb_device_free); fwd_only: forward-strand entries only (the adaptamer side)
 extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only,
                               void **d_recs, long long *n, void *stream)
-{ rec128 *d = NULL; long long nrev = 0;
-  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),&d,n,&nrev,NULL,NULL,(cudaStream_t) stream);
+{ dblock<rec128> d; long long nrev = 0;
+  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),d,n,&nrev,NULL,NULL,(cudaStream_t) stream);
   if (rc) return rc;
-  *d_recs = d;
+  *d_recs = d.release();
   return FGB_OK;
 }
 
@@ -483,19 +462,17 @@ extern "C" int fgb_records_group_by_top_byte(void *d_recs, long long n, void *d_
 { cudaStream_t st = (cudaStream_t) stream;
   for (int b = 0; b <= 256; b++) bounds257[b] = 0;
   if (n <= 0) return FGB_OK;
-  void *d_tmp = NULL; unsigned *d_bins = NULL;
+  dblock<unsigned char> d_tmp; dblock<unsigned> d_bins;
   long long tmpb = fgb_sort128_tmp_bytes(n);
-  int rc = FGB_OK, inb = 0;
+  int rc, inb = 0;
   std::vector<unsigned> bins(65537);
-  if (fgb_dmalloc(&d_tmp,tmpb,st) != cudaSuccess || fgb_dmalloc((void **) &d_bins,sizeof(unsigned)*65537,st) != cudaSuccess)
-    rc = FGB_ERR_CUDA;
-  if (!rc) rc = fgb_sort128_device(d_recs,d_out,n,15,16,d_tmp,tmpb,&inb,st);
-  if (!rc && !inb && cudaMemcpyAsync(d_out,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc) rc = fgb_kmer_bins_device(d_out,n,56,d_bins,st);
-  if (!rc && (cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*65537,cudaMemcpyDeviceToHost,st) != cudaSuccess ||
-              cudaStreamSynchronize(st) != cudaSuccess)) rc = FGB_ERR_CUDA;
-  fgb_dfree(d_tmp,st); fgb_dfree(d_bins,st);
-  if (rc) return rc;
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
+  CUDA_TRY(d_bins.alloc(65537,st));
+  if ((rc = fgb_sort128_device(d_recs,d_out,n,15,16,d_tmp,tmpb,&inb,st))) return rc;
+  if (!inb) CUDA_TRY(cudaMemcpyAsync(d_out,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+  if ((rc = fgb_kmer_bins_device(d_out,n,56,d_bins,st))) return rc;
+  CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*65537,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   for (int b = 0; b <= 256; b++) bounds257[b] = bins[b];
   return FGB_OK;
 }
@@ -506,16 +483,15 @@ extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned pl
                                     int post_bytes, int cont_bytes, int ncontig, fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (n < 0 || n >= 0xfffffff0ll || plo >= phi || phi > (1u << 24)) return FGB_ERR_ARG;
-  fgb_gix *x = new fgb_gix();
+  std::unique_ptr<fgb_gix> x(new fgb_gix());
   x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
   x->fwd_only = fwd_only ? 1 : 0;
-  rec128 *d_a = NULL;
-  int rc = FGB_OK;
-  if (fgb_dmalloc((void **) &d_a,sizeof(rec128)*(n+1),st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc && n > 0 && cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc) rc = gix_finish(x,d_a,n,plo,phi,NULL,st); else fgb_dfree(d_a,st);
-  if (rc) { fgb_gix_free(x); return rc; }
-  *out = x;
+  dblock<rec128> d_a;
+  CUDA_TRY(d_a.alloc(n+1,st));
+  if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+  int rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,NULL,st);
+  if (rc) return rc;
+  *out = x.release();
   return FGB_OK;
 }
 
@@ -533,12 +509,11 @@ extern "C" int fgb_gix_from_device(const void *d_tab, long long n, int post_byte
                                    int ncontig, fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
-  fgb_gix *x = new fgb_gix();
-  gix_scope own(x);
+  std::unique_ptr<fgb_gix> x(new fgb_gix());
   x->n = n; x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_tab,sizeof(rec128)*(n+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_pstart,sizeof(unsigned)*((1<<24)+1+8),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_adj,(size_t) x->n + 32,st));
+  CUDA_TRY(x->d_tab.alloc(n+1,st));
+  CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
+  CUDA_TRY(x->d_adj.alloc((size_t) x->n + 32,st));
   CUDA_TRY(cudaMemcpyAsync(x->d_tab,d_tab,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
   int rc;
   { stage_timer t(&g_timings.index_ms,st);
@@ -546,7 +521,7 @@ extern "C" int fgb_gix_from_device(const void *d_tab, long long n, int post_byte
   }
   CUDA_TRY(cudaStreamSynchronize(st));
   if (rc) return rc;
-  *out = own.release();
+  *out = x.release();
   return FGB_OK;
 }
 extern "C" int fgb_gix_post_bytes(const fgb_gix *x) { return x->post_bytes; }
@@ -565,17 +540,16 @@ extern "C" int fgb_gix_upload(const void *tab, long long n, int post_bytes, int 
                               int ncontig, fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
-  fgb_gix *x = new fgb_gix();
-  gix_scope own(x);
+  std::unique_ptr<fgb_gix> x(new fgb_gix());
   x->n = n; x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_tab,sizeof(rec128)*(n+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_pstart,sizeof(unsigned)*((1<<24)+1+8),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_adj,(size_t) x->n + 32,st));
+  CUDA_TRY(x->d_tab.alloc(n+1,st));
+  CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
+  CUDA_TRY(x->d_adj.alloc((size_t) x->n + 32,st));
   CUDA_TRY(cudaMemcpyAsync(x->d_tab,tab,sizeof(rec128)*n,cudaMemcpyHostToDevice,st));
   int rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
   CUDA_TRY(cudaStreamSynchronize(st));
   if (rc) return rc;
-  *out = own.release();
+  *out = x.release();
   return FGB_OK;
 }
 
@@ -586,24 +560,22 @@ extern "C" int fgb_gix_import_ktab(const unsigned char *entries, long long n, in
                                    fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (n >= 0xfffffff0ll || post_bytes > 4 || cont_bytes > 2) return FGB_ERR_LIMIT;
-  fgb_gix *x = new fgb_gix();
-  gix_scope own(x);
+  std::unique_ptr<fgb_gix> x(new fgb_gix());
   x->n = n; x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
   long long E = 9 + post_bytes + cont_bytes;
-  unsigned char *d_ent = NULL; long long *d_index = NULL;
-  blk_scope B; B.own(d_ent); B.own(d_index);
-  CUDA_TRY(fgb_dmalloc((void **) &d_ent,E*n + 16,st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_index,8ll<<24,st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_tab,sizeof(rec128)*(n+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_pstart,sizeof(unsigned)*((1<<24)+1+8),st));
-  CUDA_TRY(fgb_dmalloc((void **) &x->d_adj,(size_t) x->n + 32,st));
+  dblock<unsigned char> d_ent; dblock<long long> d_index;
+  CUDA_TRY(d_ent.alloc(E*n + 16,st));
+  CUDA_TRY(d_index.alloc(1ll << 24,st));
+  CUDA_TRY(x->d_tab.alloc(n+1,st));
+  CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
+  CUDA_TRY(x->d_adj.alloc((size_t) x->n + 32,st));
   CUDA_TRY(cudaMemcpyAsync(d_ent,entries,E*n,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_index,index,8ll<<24,cudaMemcpyHostToDevice,st));
   int rc = fgb_ktab_import_device(d_ent,n,post_bytes,cont_bytes,d_index,x->d_tab,st);
   if (!rc) rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
   CUDA_TRY(cudaStreamSynchronize(st));
   if (rc) return rc;
-  *out = own.release();
+  *out = x.release();
   return FGB_OK;
 }
 
@@ -613,10 +585,9 @@ extern "C" int fgb_gix_export_ktab(const fgb_gix *x, const long long *part_first
                                    unsigned char *out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   long long E = 9 + x->post_bytes + x->cont_bytes;
-  unsigned char *d_out = NULL; long long *d_pf = NULL;
-  blk_scope B; B.own(d_out); B.own(d_pf);
-  CUDA_TRY(fgb_dmalloc((void **) &d_out,E*x->n + 16,st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_pf,8*(nparts+1),st));
+  dblock<unsigned char> d_out; dblock<long long> d_pf;
+  CUDA_TRY(d_out.alloc(E*x->n + 16,st));
+  CUDA_TRY(d_pf.alloc(nparts+1,st));
   CUDA_TRY(cudaMemcpyAsync(d_pf,part_first,8*nparts,cudaMemcpyHostToDevice,st));
   int rc = fgb_ktab_export_device(x->d_tab,x->n,x->post_bytes,x->cont_bytes,d_pf,nparts,d_out,st);
   if (!rc) CUDA_TRY(cudaMemcpyAsync(out,d_out,E*x->n,cudaMemcpyDeviceToHost,st));
@@ -630,12 +601,7 @@ extern "C" int fgb_gix_export_ktab(const fgb_gix *x, const long long *part_first
 
 static int bitlen(long long v) { int b = 0; while (v > 0) { b += 1; v >>= 1; } return b; }
 
-extern "C" void fgb_seeds_free(fgb_seeds *s)
-{ cudaStream_t st = 0;
-  if (!s) return;
-  fgb_dfree(s->d_rec,st);
-  delete s;
-}
+extern "C" void fgb_seeds_free(fgb_seeds *s) { delete s; }
 
 static int seeds_find_impl(const fgb_gix *x1, const fgb_gix *x2, long long amxpos,
                            long long bmxpos, int freq, bool self, fgb_seeds **out, void *stream);
@@ -661,87 +627,75 @@ static int seed_layout_of(const fgb_gix *x1, const fgb_gix *x2, long long amxpos
 
 //  K5: the unsorted seed records of x1 against x2 in a fresh device buffer (room for n+1)
 static int seeds_merge_impl(const fgb_gix *x1, const fgb_gix *x2, long long amxpos, long long bmxpos, int freq,
-                            bool self, const seed_bits &L, rec128 **d_out, long long *nseeds_out,
+                            bool self, const seed_bits &L, dblock<rec128> &d_out, long long *nseeds_out,
                             long long *sumlen_out, long long *n1m_out, cudaStream_t st)
 { if (self && x1->fwd_only) return FGB_ERR_ARG;                // SELF mode needs both strands
-  //  every device block of this call is released on every exit path
-  u64 *d_counters = NULL; rec128 *d_fwd = NULL, *d_a = NULL;
-  int rc = FGB_OK;
+  dblock<u64> d_counters; dblock<rec128> d_fwd, d_a;
+  int rc;
   u64 nseeds = 0, sumlen = 0;
   //  the adaptamer side must be a forward-strand table (reverse entries never seed): a both-strand
   //  table (imported .ktab, fgb_gix_build) is compacted once; the fused path builds it forward-only
   const rec128 *t1 = x1->d_tab; long long n1 = x1->n;
-#define SF_TRY(call) do { if ((call) != cudaSuccess) { rc = FGB_ERR_CUDA; goto done; } } while (0)
-  SF_TRY(fgb_dmalloc((void **) &d_counters,16,st));
+  CUDA_TRY(d_counters.alloc(2,st));
   if (!self && !x1->fwd_only && n1 > 0)
-    { SF_TRY(fgb_dmalloc((void **) &d_fwd,sizeof(rec128)*(n1+1),st));
-      if ((rc = fgb_forward_view_device(x1->d_tab,n1,d_fwd,&n1,st))) goto done;
+    { CUDA_TRY(d_fwd.alloc(n1+1,st));
+      if ((rc = fgb_forward_view_device(x1->d_tab,n1,d_fwd,&n1,st))) return rc;
       t1 = d_fwd;
     }
-  { long long cap = (self ? 2*x1->n : 2*n1 + (n1 >> 1)) + 1024;
-    for (int attempt = 0; ; attempt++)
-      { SF_TRY(fgb_dmalloc((void **) &d_a,sizeof(rec128)*(cap+1),st));
-        if (self)
-          rc = fgb_self_merge_device(x1->d_tab,x1->n,x1->d_pstart,freq,L.anti,L.band,L.jc,L.ic,amxpos,
-                                     d_a,cap,d_counters,&nseeds,&sumlen,st);
-        else
-          rc = fgb_merge_device(t1,n1,x2->d_tab,x2->n,x2->d_pstart,x2->d_adj,freq,L.anti,L.band,L.jc,L.ic,
-                                amxpos,bmxpos,d_a,cap,d_counters,&nseeds,&sumlen,st);
-        if (rc == FGB_OK) break;
-        fgb_dfree(d_a,st); d_a = NULL;
-        if (rc != FGB_ERR_OVERFLOW || attempt > 0) goto done;
-        cap = (long long) nseeds + 1024;
-        g_timings.merge_ms = 0; g_timings.merge_launches = 0;   // only the successful launch is reported
-      }
-  }
-  if (nseeds >= 0xfffffff0ull) rc = FGB_ERR_LIMIT;
-done:
-#undef SF_TRY
-  fgb_dfree(d_counters,st); fgb_dfree(d_fwd,st);
-  if (rc) { fgb_dfree(d_a,st); return rc; }
-  *d_out = d_a; *nseeds_out = (long long) nseeds; *sumlen_out = (long long) sumlen; *n1m_out = n1;
+  long long cap = (self ? 2*x1->n : 2*n1 + (n1 >> 1)) + 1024;
+  for (int attempt = 0; ; attempt++)
+    { CUDA_TRY(d_a.alloc(cap+1,st));
+      if (self)
+        rc = fgb_self_merge_device(x1->d_tab,x1->n,x1->d_pstart,freq,L.anti,L.band,L.jc,L.ic,amxpos,
+                                   d_a,cap,d_counters,&nseeds,&sumlen,st);
+      else
+        rc = fgb_merge_device(t1,n1,x2->d_tab,x2->n,x2->d_pstart,x2->d_adj,freq,L.anti,L.band,L.jc,L.ic,
+                              amxpos,bmxpos,d_a,cap,d_counters,&nseeds,&sumlen,st);
+      if (rc == FGB_OK) break;
+      d_a.reset();                                              // before the larger buffer is allocated
+      if (rc != FGB_ERR_OVERFLOW || attempt > 0) return rc;
+      cap = (long long) nseeds + 1024;
+      g_timings.merge_ms = 0; g_timings.merge_launches = 0;   // only the successful launch is reported
+    }
+  if (nseeds >= 0xfffffff0ull) return FGB_ERR_LIMIT;
+  d_out = std::move(d_a); *nseeds_out = (long long) nseeds; *sumlen_out = (long long) sumlen; *n1m_out = n1;
   return FGB_OK;
 }
 
 //  K6: sorts n seed records in d_a (consumed) into a handle
-static int seeds_sort_impl(rec128 *d_a, long long n, const seed_bits &L, long long amxpos, long long bmxpos,
+static int seeds_sort_impl(dblock<rec128> d_a, long long n, const seed_bits &L, long long amxpos, long long bmxpos,
                            bool self, long long sumlen, long long n1m, fgb_seeds **out, cudaStream_t st)
-{ rec128 *d_b = NULL; void *d_tmp = NULL;
-  fgb_seeds *s = new fgb_seeds();
+{ dblock<rec128> d_b; dblock<unsigned char> d_tmp;
+  std::unique_ptr<fgb_seeds> s(new fgb_seeds());
   s->self_mode = self ? 1 : 0;
   s->anti_bits = L.anti; s->band_bits = L.band; s->jc_bits = L.jc; s->ic_bits = L.ic;
   s->amxpos = amxpos; s->bmxpos = bmxpos;
   s->n = n; s->sumlen = sumlen; s->n1_merged = n1m;
   long long tmpb = fgb_sort128_tmp_bytes(n);
-  int rc = FGB_OK, inb = 0;
+  int rc, inb = 0;
   //  a key of <= 64 bits leaves hi = 0 in every record: the passes run on the lo words alone.
   //  FGB_SEED_SORT_WIDE=1 forces the 128-bit passes (both paths can be compared in one process).
   const char *wide_env = getenv("FGB_SEED_SORT_WIDE");
   const bool narrow = L.key <= 64 && !(wide_env != NULL && atoi(wide_env) != 0);
   u64 hiflag = 0, *d_hiflag = NULL;
-  if (fgb_dmalloc((void **) &d_b,sizeof(rec128)*(n+1),st) != cudaSuccess ||
-      fgb_dmalloc((void **) &d_tmp,tmpb + 8,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc)
-    { stage_timer t(&g_timings.ssort_ms,st);
-      //  from bit 6: the lcp field (bits 0..5) cannot break a tie -- two seeds that agree on strand,
-      //  contigs, band, anti-diagonal and diagonal remainder are the same pair of positions
-      if (narrow)
-        { d_hiflag = (u64 *) ((char *) d_tmp + tmpb);
-          rc = fgb_sort_seeds64_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,d_hiflag,st);
-        }
-      else
-        rc = fgb_sort128_bits_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,&inb,st);
-    }
-  if (!rc && d_hiflag && cudaMemcpyAsync(&hiflag,d_hiflag,8,cudaMemcpyDeviceToHost,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc && hiflag) rc = FGB_ERR_ARG;                 // a record with hi != 0: the 64-bit passes mis-ordered it
-  if (!rc)
-    { s->d_rec = inb ? d_b : d_a;
-      if (inb) d_b = NULL; else d_a = NULL;                     // ownership moved to the handle
-    }
-  fgb_dfree(d_a,st); fgb_dfree(d_b,st); fgb_dfree(d_tmp,st);
-  if (rc) { delete s; return rc; }
-  *out = s;
+  CUDA_TRY(d_b.alloc(n+1,st));
+  CUDA_TRY(d_tmp.alloc(tmpb + 8,st));
+  { stage_timer t(&g_timings.ssort_ms,st);
+    //  from bit 6: the lcp field (bits 0..5) cannot break a tie -- two seeds that agree on strand,
+    //  contigs, band, anti-diagonal and diagonal remainder are the same pair of positions
+    if (narrow)
+      { d_hiflag = (u64 *) (d_tmp + tmpb);
+        rc = fgb_sort_seeds64_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,d_hiflag,st);
+      }
+    else
+      rc = fgb_sort128_bits_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,&inb,st);
+  }
+  if (rc) return rc;
+  if (d_hiflag) CUDA_TRY(cudaMemcpyAsync(&hiflag,d_hiflag,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (hiflag) return FGB_ERR_ARG;                      // a record with hi != 0: the 64-bit passes mis-ordered it
+  s->d_rec = std::move(inb ? d_b : d_a);
+  *out = s.release();
   return FGB_OK;
 }
 
@@ -751,9 +705,9 @@ static int seeds_find_impl(const fgb_gix *x1, const fgb_gix *x2, long long amxpo
   seed_bits L;
   int rc = seed_layout_of(x1,x2,amxpos,bmxpos,&L);
   if (rc) return rc;
-  rec128 *d_a = NULL; long long n = 0, sumlen = 0, n1m = 0;
-  if ((rc = seeds_merge_impl(x1,x2,amxpos,bmxpos,freq,self,L,&d_a,&n,&sumlen,&n1m,st))) return rc;
-  return seeds_sort_impl(d_a,n,L,amxpos,bmxpos,self,sumlen,n1m,out,st);
+  dblock<rec128> d_a; long long n = 0, sumlen = 0, n1m = 0;
+  if ((rc = seeds_merge_impl(x1,x2,amxpos,bmxpos,freq,self,L,d_a,&n,&sumlen,&n1m,st))) return rc;
+  return seeds_sort_impl(std::move(d_a),n,L,amxpos,bmxpos,self,sumlen,n1m,out,st);
 }
 
 //  ---- sharded path: seeds leave the merge unsorted, travel to their A-contig's owner, are sorted there ----
@@ -765,78 +719,53 @@ extern "C" int fgb_seeds_merge(const fgb_gix *x1, const fgb_gix *x2, long long a
 { seed_bits L;
   int rc = seed_layout_of(x1,x2,amxpos,bmxpos,&L);
   if (rc) return rc;
-  rec128 *d_a = NULL; long long sumlen = 0, n1m = 0;
-  if ((rc = seeds_merge_impl(x1,x2,amxpos,bmxpos,freq,false,L,&d_a,n,&sumlen,&n1m,(cudaStream_t) stream))) return rc;
-  *d_seeds = d_a;
+  dblock<rec128> d_a; long long sumlen = 0, n1m = 0;
+  if ((rc = seeds_merge_impl(x1,x2,amxpos,bmxpos,freq,false,L,d_a,n,&sumlen,&n1m,(cudaStream_t) stream))) return rc;
+  *d_seeds = d_a.release();
   bits[0] = L.anti; bits[1] = L.band; bits[2] = L.jc; bits[3] = L.ic;
   if (info) { info[0] = sumlen; info[1] = n1m; }
   return FGB_OK;
 }
 
-//  seeds grouped by the rank that owns their A-contig: owner[r] for contig RANK r (the icont field);
-//  d_out[bounds[w] .. bounds[w+1]) are the seeds of owner w.  Count + scatter, order inside a group free.
-extern "C" int fgb_seeds_group_by_owner(const void *d_seeds, long long n, const int *bits, const int *owner,
-                                        int nrank_contigs, int world, void *d_out, long long *bounds,
-                                        void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  if (world < 1 || world > 64) return FGB_ERR_ARG;
+//  Count + scatter of n 16-byte records by owner[field], field = the nbits bits at bit pos of the record
+//  (nowner entries): d_out[bounds[w] .. bounds[w+1]) are the records of owner w, order inside a group free.
+static int group_by_owner(const void *d_src, long long n, int pos, int nbits, const int *owner, int nowner,
+                          int world, void *d_out, long long *bounds, cudaStream_t st)
+{ if (world < 1 || world > 64) return FGB_ERR_ARG;
   for (int w = 0; w <= world; w++) bounds[w] = 0;
   if (n <= 0) return FGB_OK;
-  int *d_owner = NULL; u64 *d_cnt = NULL;
-  int rc = FGB_OK;
+  dblock<int> d_owner; dblock<u64> d_cnt;
+  int rc;
   u64 cnt[64], base[65];
-  const int p_ic = 12 + bits[0] + bits[1] + bits[2];
-  if (fgb_dmalloc((void **) &d_owner,sizeof(int)*(size_t) nrank_contigs,st) != cudaSuccess ||
-      fgb_dmalloc((void **) &d_cnt,8*64*2,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc && (cudaMemcpyAsync(d_owner,owner,sizeof(int)*(size_t) nrank_contigs,cudaMemcpyHostToDevice,st) != cudaSuccess ||
-              cudaMemsetAsync(d_cnt,0,8*64*2,st) != cudaSuccess)) rc = FGB_ERR_CUDA;
-  if (!rc) rc = fgb_owner_count_device(d_seeds,n,p_ic,bits[3],d_owner,nrank_contigs,world,d_cnt,st);
-  if (!rc && (cudaMemcpyAsync(cnt,d_cnt,8*64,cudaMemcpyDeviceToHost,st) != cudaSuccess ||
-              cudaStreamSynchronize(st) != cudaSuccess)) rc = FGB_ERR_CUDA;
-  if (!rc)
-    { base[0] = 0;
-      for (int w = 0; w < world; w++) base[w+1] = base[w] + cnt[w];
-      if (cudaMemcpyAsync(d_cnt + 64,base,8*64,cudaMemcpyHostToDevice,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-    }
-  if (!rc) rc = fgb_owner_scatter_device(d_seeds,n,p_ic,bits[3],d_owner,nrank_contigs,world,d_cnt + 64,d_out,st);
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  fgb_dfree(d_owner,st); fgb_dfree(d_cnt,st);
-  if (rc) return rc;
+  CUDA_TRY(d_owner.alloc((size_t) nowner,st));
+  CUDA_TRY(d_cnt.alloc(64*2,st));
+  CUDA_TRY(cudaMemcpyAsync(d_owner,owner,sizeof(int)*(size_t) nowner,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemsetAsync(d_cnt,0,8*64*2,st));
+  if ((rc = fgb_owner_count_device(d_src,n,pos,nbits,d_owner,nowner,world,d_cnt,st))) return rc;
+  CUDA_TRY(cudaMemcpyAsync(cnt,d_cnt,8*64,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  base[0] = 0;
+  for (int w = 0; w < world; w++) base[w+1] = base[w] + cnt[w];
+  CUDA_TRY(cudaMemcpyAsync(d_cnt + 64,base,8*64,cudaMemcpyHostToDevice,st));
+  if ((rc = fgb_owner_scatter_device(d_src,n,pos,nbits,d_owner,nowner,world,d_cnt + 64,d_out,st))) return rc;
+  CUDA_TRY(cudaStreamSynchronize(st));
   for (int w = 0; w <= world; w++) bounds[w] = (long long) base[w];
   return FGB_OK;
 }
 
-//  k-mer records grouped by the rank that owns their first four bases: owner256[b] for top byte b;
-//  d_out[bounds[w] .. bounds[w+1]) are the records of owner w (count + scatter: cheaper than the radix
-//  pass of fgb_records_group_by_top_byte when only the destination matters)
+//  seeds grouped by the rank that owns their A-contig: owner[r] for contig RANK r (the icont field)
+extern "C" int fgb_seeds_group_by_owner(const void *d_seeds, long long n, const int *bits, const int *owner,
+                                        int nrank_contigs, int world, void *d_out, long long *bounds,
+                                        void *stream)
+{ return group_by_owner(d_seeds,n,12 + bits[0] + bits[1] + bits[2],bits[3],owner,nrank_contigs,world,d_out,bounds,
+                        (cudaStream_t) stream);
+}
+
+//  k-mer records grouped by the rank that owns their first four bases: owner256[b] for top byte b
+//  (cheaper than the radix pass of fgb_records_group_by_top_byte when only the destination matters)
 extern "C" int fgb_records_group_by_owner(const void *d_recs, long long n, const int *owner256, int world,
                                           void *d_out, long long *bounds, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  if (world < 1 || world > 64) return FGB_ERR_ARG;
-  for (int w = 0; w <= world; w++) bounds[w] = 0;
-  if (n <= 0) return FGB_OK;
-  int *d_owner = NULL; u64 *d_cnt = NULL;
-  int rc = FGB_OK;
-  u64 cnt[64], base[65];
-  if (fgb_dmalloc((void **) &d_owner,sizeof(int)*256,st) != cudaSuccess ||
-      fgb_dmalloc((void **) &d_cnt,8*64*2,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  if (!rc && (cudaMemcpyAsync(d_owner,owner256,sizeof(int)*256,cudaMemcpyHostToDevice,st) != cudaSuccess ||
-              cudaMemsetAsync(d_cnt,0,8*64*2,st) != cudaSuccess)) rc = FGB_ERR_CUDA;
-  if (!rc) rc = fgb_owner_count_device(d_recs,n,120,8,d_owner,256,world,d_cnt,st);
-  if (!rc && (cudaMemcpyAsync(cnt,d_cnt,8*64,cudaMemcpyDeviceToHost,st) != cudaSuccess ||
-              cudaStreamSynchronize(st) != cudaSuccess)) rc = FGB_ERR_CUDA;
-  if (!rc)
-    { base[0] = 0;
-      for (int w = 0; w < world; w++) base[w+1] = base[w] + cnt[w];
-      if (cudaMemcpyAsync(d_cnt + 64,base,8*64,cudaMemcpyHostToDevice,st) != cudaSuccess) rc = FGB_ERR_CUDA;
-    }
-  if (!rc) rc = fgb_owner_scatter_device(d_recs,n,120,8,d_owner,256,world,d_cnt + 64,d_out,st);
-  if (!rc && cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
-  fgb_dfree(d_owner,st); fgb_dfree(d_cnt,st);
-  if (rc) return rc;
-  for (int w = 0; w <= world; w++) bounds[w] = (long long) base[w];
-  return FGB_OK;
-}
+{ return group_by_owner(d_recs,n,120,8,owner256,256,world,d_out,bounds,(cudaStream_t) stream); }
 
 //  sorted seed set over n unsorted device records (copied); bits as fgb_seeds_merge returns them
 extern "C" int fgb_seeds_from_records(const void *d_recs, long long n, const int *bits, long long amxpos,
@@ -847,11 +776,10 @@ extern "C" int fgb_seeds_from_records(const void *d_recs, long long n, const int
   L.anti = bits[0]; L.band = bits[1]; L.jc = bits[2]; L.ic = bits[3];
   L.key = 12 + L.anti + L.band + L.jc + L.ic + 1;
   if (L.key > 128) return FGB_ERR_LIMIT;
-  rec128 *d_a = NULL;
-  CUDA_TRY(fgb_dmalloc((void **) &d_a,sizeof(rec128)*(n+1),st));
-  if (n > 0 && cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st) != cudaSuccess)
-    { fgb_dfree(d_a,st); return FGB_ERR_CUDA; }
-  return seeds_sort_impl(d_a,n,L,amxpos,bmxpos,false,sumlen,0,out,st);
+  dblock<rec128> d_a;
+  CUDA_TRY(d_a.alloc(n+1,st));
+  if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+  return seeds_sort_impl(std::move(d_a),n,L,amxpos,bmxpos,false,sumlen,0,out,st);
 }
 
 extern "C" long long fgb_seeds_size(const fgb_seeds *s) { return s->n; }
@@ -865,17 +793,16 @@ extern "C" int fgb_seeds_download(const fgb_seeds *s, void *rec)
 //  behind both drop-in sort seams.
 extern "C" int fgb_sort128_host(void *recs, long long n, int byte_lo, int byte_hi, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  rec128 *d_a = NULL, *d_b = NULL; void *d_tmp = NULL;
+  dblock<rec128> d_a, d_b; dblock<unsigned char> d_tmp;
   long long tmpb = fgb_sort128_tmp_bytes(n);
-  CUDA_TRY(fgb_dmalloc((void **) &d_a,sizeof(rec128)*(n+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_b,sizeof(rec128)*(n+1),st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_tmp,tmpb,st));
+  CUDA_TRY(d_a.alloc(n+1,st));
+  CUDA_TRY(d_b.alloc(n+1,st));
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
   CUDA_TRY(cudaMemcpyAsync(d_a,recs,sizeof(rec128)*n,cudaMemcpyHostToDevice,st));
   int inb = 0;
   int rc = fgb_sort128_device(d_a,d_b,n,byte_lo,byte_hi,d_tmp,tmpb,&inb,st);
   if (!rc) CUDA_TRY(cudaMemcpyAsync(recs,inb ? d_b : d_a,sizeof(rec128)*n,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  fgb_dfree(d_a,st); fgb_dfree(d_b,st); fgb_dfree(d_tmp,st);
   return rc;
 }
 
@@ -890,14 +817,12 @@ extern "C" int fgb_device_ready()
  *  Read_GDB and la_merge (FastGA.c:4927-5205), GIX construction included.
  **********************************************************************************************/
 
-struct fgb_overlaps;
 struct fgb_alns;
 extern "C" {
 int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B, int chain_break,
                int chain_min, int align_min, double align_rate, const short *tables, int ave_path,
                int tspace, fgb_overlaps **out, void *stream);
 int fgb_align_spec(double ave_corr, const float *freq, short *tables, int *ave_path);
-void fgb_overlaps_free(fgb_overlaps *o);
 long long fgb_overlaps_bytes(const fgb_overlaps *o);
 void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out);
 int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *perm2, int jc_bits, int ic_bits,
@@ -917,24 +842,29 @@ extern "C" int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const 
                                 int freq, int chain_break, int chain_min, int align_min,
                                 double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream);
 
-static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, fgb_gix *x1, fgb_gix *x2, bool own,
-                             const float *freqA, int freq, int chain_break, int chain_min, int align_min,
-                             double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream);
+static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
+                             std::unique_ptr<fgb_gix> *own, const float *freqA, int freq, int chain_break,
+                             int chain_min, int align_min, double align_rate, fgb_alns **out,
+                             fgb_run_stats *stats, void *stream);
 
 //  Device-resident genomes in, final alignments out (the timed "step" of bench.py).
 extern "C" int fgb_align_resident(const fgb_genome *A, const fgb_genome *B, const float *freqA,
                                   int freq, int chain_break, int chain_min, int align_min,
                                   double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ fgb_gix *x1 = NULL, *x2 = NULL;
+{ std::unique_ptr<fgb_gix> x[2];
+  fgb_gix *p = NULL;
   int rc;
   long long t0 = now_us();
   //  adaptamer side: forward strand only, and only the table (the merge reads the OTHER table's index)
-  if ((rc = gix_build_range(A,0u,(1u << 24) | GIX_FWD_ONLY | GIX_NO_INDEX,&x1,stream))) return rc;
-  if ((rc = fgb_gix_build(B,&x2,stream))) { fgb_gix_free(x1); return rc; }
+  if ((rc = gix_build_range(A,0u,(1u << 24) | GIX_FWD_ONLY | GIX_NO_INDEX,&p,stream))) return rc;
+  x[0].reset(p);
+  if ((rc = fgb_gix_build(B,&p,stream))) return rc;
+  x[1].reset(p);
   long long t1 = now_us();
   //  the tables are this call's own: they go back to the allocator as soon as the merge has read them
   //  (two tables + seeds + sort buffer of a multi-Gbp pair do not fit side by side)
-  rc = align_tables_impl(A,B,x1,x2,true,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream);
+  rc = align_tables_impl(A,B,x[0].get(),x[1].get(),x,freqA,freq,chain_break,chain_min,align_min,align_rate,
+                         out,stats,stream);
   if (stats) stats->us_gix = t1 - t0;
   return rc;
 }
@@ -943,42 +873,44 @@ extern "C" int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const 
                                 const fgb_gix *x2, const float *freqA,
                                 int freq, int chain_break, int chain_min, int align_min,
                                 double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ return align_tables_impl(A,B,(fgb_gix *) x1,(fgb_gix *) x2,false,freqA,freq,chain_break,chain_min,align_min,
-                           align_rate,out,stats,stream);
-}
+{ return align_tables_impl(A,B,x1,x2,NULL,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream); }
 
-static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, fgb_gix *x1, fgb_gix *x2, bool own,
-                             const float *freqA, int freq, int chain_break, int chain_min, int align_min,
-                             double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ fgb_seeds *sd = NULL; fgb_overlaps *ov = NULL;
+//  own: the two table handles when they are this call's to release (right after the merge), else NULL
+static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
+                             std::unique_ptr<fgb_gix> *own, const float *freqA, int freq, int chain_break,
+                             int chain_min, int align_min, double align_rate, fgb_alns **out,
+                             fgb_run_stats *stats, void *stream)
+{ fgb_seeds *ps = NULL; fgb_overlaps *po = NULL;
   int rc;
   long long t0 = now_us(), t1 = t0, t2, t3, t4;
   const long long n1 = x1->n_both, n2 = x2->n;
   { seed_bits L;
-    rec128 *d_a = NULL; long long n = 0, sumlen = 0, n1m = 0;
+    dblock<rec128> d_a; long long n = 0, sumlen = 0, n1m = 0;
     rc = seed_layout_of(x1,x2,A->maxlen,B->maxlen,&L);
-    if (!rc) rc = seeds_merge_impl(x1,x2,A->maxlen,B->maxlen,freq,false,L,&d_a,&n,&sumlen,&n1m,(cudaStream_t) stream);
-    if (own) { fgb_gix_free(x1); fgb_gix_free(x2); }
-    if (!rc) rc = seeds_sort_impl(d_a,n,L,A->maxlen,B->maxlen,false,sumlen,n1m,&sd,(cudaStream_t) stream);
+    if (!rc) rc = seeds_merge_impl(x1,x2,A->maxlen,B->maxlen,freq,false,L,d_a,&n,&sumlen,&n1m,(cudaStream_t) stream);
+    if (own) { own[0].reset(); own[1].reset(); }
+    if (!rc) rc = seeds_sort_impl(std::move(d_a),n,L,A->maxlen,B->maxlen,false,sumlen,n1m,&ps,(cudaStream_t) stream);
   }
   if (rc) return rc;
+  std::unique_ptr<fgb_seeds> sd(ps);
   const long long n1f = sd->n1_merged;
   t2 = now_us();
   short *tables = (short *) malloc(65536*sizeof(short));
   int ave = 0;
   fgb_align_spec(1.-align_rate,freqA,tables,&ave);           // FastGA.c:3760
-  rc = fgb_extend(sd,A,B,chain_break,chain_min,align_min,align_rate,tables,ave,100,&ov,stream);
+  rc = fgb_extend(sd.get(),A,B,chain_break,chain_min,align_min,align_rate,tables,ave,100,&po,stream);
   free(tables);
   t3 = now_us();
   long long nseeds = sd->n, sumlen = sd->sumlen;
   int jb = sd->jc_bits, ib = sd->ic_bits;
-  fgb_seeds_free(sd);
+  sd.reset();
   if (rc) return rc;
-  rc = fgb_filter(ov,A->perm.data(),B->perm.data(),jb,ib,1,out);
+  std::unique_ptr<fgb_overlaps> ov(po);
+  rc = fgb_filter(ov.get(),A->perm.data(),B->perm.data(),jb,ib,1,out);
   t4 = now_us();
   if (stats)
     { stats->us_gix = t1-t0; stats->us_seeds = t2-t1; stats->us_extend = t3-t2; stats->us_filter = t4-t3; unsigned long long c[16];
-      fgb_overlaps_counters(ov,c);
+      fgb_overlaps_counters(ov.get(),c);
       stats->nkmers1 = n1; stats->nkmers2 = n2; stats->nseeds = nseeds; stats->sumlen = sumlen;
       stats->nkmers1_fwd = n1f;
       stats->nhits = (long long) c[0]; stats->nla = (long long) c[1]; stats->nwaves = (long long) c[2];
@@ -989,9 +921,8 @@ static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, fgb_gix *
       stats->slow_cycles = (long long) ((c[15] >> 40) << 12); stats->slow_waves = (long long) ((c[15] >> 16) & 0xffffff);
       stats->paired_waves = (long long) c[11]; stats->pairings = (long long) c[12];
       stats->h2d_bytes = A->h2d_bytes + B->h2d_bytes + 65536*2;
-      stats->d2h_bytes = fgb_overlaps_bytes(ov) + 16 + 8*1024*2 + 64;
+      stats->d2h_bytes = fgb_overlaps_bytes(ov.get()) + 16 + 8*1024*2 + 64;
     }
-  fgb_overlaps_free(ov);
   return rc;
 }
 
@@ -1003,34 +934,36 @@ extern "C" int fgb_fastga_self(const unsigned char *bps, long long nb, int nc, c
                                const long long *boff, const float *freq4,
                                int freq, int chain_break, int chain_min, int align_min, double align_rate,
                                fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ fgb_genome *A = NULL; fgb_gix *x = NULL; fgb_seeds *sd = NULL; fgb_overlaps *ov = NULL;
+{ fgb_genome *pA = NULL; fgb_gix *px = NULL; fgb_seeds *ps = NULL; fgb_overlaps *po = NULL;
   int rc;
-  if ((rc = fgb_genome_create(bps,nb,nc,clen,boff,1,&A,stream))) return rc;
-  if ((rc = fgb_gix_build(A,&x,stream))) { fgb_genome_free(A); return rc; }
-  rc = fgb_seeds_find_self(x,A->maxlen,freq,&sd,stream);
+  if ((rc = fgb_genome_create(bps,nb,nc,clen,boff,1,&pA,stream))) return rc;
+  std::unique_ptr<fgb_genome> A(pA);
+  if ((rc = fgb_gix_build(A.get(),&px,stream))) return rc;
+  std::unique_ptr<fgb_gix> x(px);
+  rc = fgb_seeds_find_self(x.get(),A->maxlen,freq,&ps,stream);
   long long n1 = x->n;
-  fgb_gix_free(x);
-  if (rc) { fgb_genome_free(A); return rc; }
+  x.reset();
+  if (rc) return rc;
+  std::unique_ptr<fgb_seeds> sd(ps);
   short *tables = (short *) malloc(65536*sizeof(short));
   int ave = 0;
   fgb_align_spec(1.-align_rate,freq4,tables,&ave);
-  rc = fgb_extend(sd,A,A,chain_break,chain_min,align_min,align_rate,tables,ave,100,&ov,stream);
+  rc = fgb_extend(sd.get(),A.get(),A.get(),chain_break,chain_min,align_min,align_rate,tables,ave,100,&po,stream);
   free(tables);
   long long nseeds = sd->n, sumlen = sd->sumlen;
   int jb = sd->jc_bits, ib = sd->ic_bits;
-  fgb_seeds_free(sd);
-  if (rc) { fgb_genome_free(A); return rc; }
-  rc = fgb_filter(ov,A->perm.data(),A->perm.data(),jb,ib,1,out);
+  sd.reset();
+  if (rc) return rc;
+  std::unique_ptr<fgb_overlaps> ov(po);
+  rc = fgb_filter(ov.get(),A->perm.data(),A->perm.data(),jb,ib,1,out);
   if (stats)
     { memset(stats,0,sizeof(*stats));
       unsigned long long c[16];
-      fgb_overlaps_counters(ov,c);
+      fgb_overlaps_counters(ov.get(),c);
       stats->nkmers1 = stats->nkmers2 = n1; stats->nseeds = nseeds; stats->sumlen = sumlen;
       stats->nhits = (long long) c[0]; stats->nla = (long long) c[1]; stats->nwaves = (long long) c[2];
       stats->ncells = (long long) c[3];
     }
-  fgb_overlaps_free(ov);
-  fgb_genome_free(A);
   return rc;
 }
 
@@ -1040,11 +973,11 @@ extern "C" int fgb_fastga(const unsigned char *bpsA, long long nbA, int ncA, con
                           const long long *boffB,
                           int freq, int chain_break, int chain_min, int align_min, double align_rate,
                           fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ fgb_genome *A = NULL, *B = NULL;
+{ fgb_genome *p = NULL;
   int rc;
-  if ((rc = fgb_genome_create(bpsA,nbA,ncA,clenA,boffA,1,&A,stream))) return rc;
-  if ((rc = fgb_genome_create(bpsB,nbB,ncB,clenB,boffB,0,&B,stream))) { fgb_genome_free(A); return rc; }
-  rc = fgb_align_resident(A,B,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream);
-  fgb_genome_free(A); fgb_genome_free(B);
-  return rc;
+  if ((rc = fgb_genome_create(bpsA,nbA,ncA,clenA,boffA,1,&p,stream))) return rc;
+  std::unique_ptr<fgb_genome> A(p);
+  if ((rc = fgb_genome_create(bpsB,nbB,ncB,clenB,boffB,0,&p,stream))) return rc;
+  std::unique_ptr<fgb_genome> B(p);
+  return fgb_align_resident(A.get(),B.get(),freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream);
 }

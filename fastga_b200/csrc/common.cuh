@@ -68,6 +68,31 @@ void fgb_count_launch(int n);                 // kernels launched (bench.py gpu_
 cudaError_t fgb_dmalloc(void **p, size_t bytes, cudaStream_t st);
 void fgb_dfree(void *p, cudaStream_t st);
 
+//  Owner of one block of `count` T from fgb_dmalloc: the block goes back to the cache when the owner
+//  is destroyed (every return path), on reset(), or never once release() has handed it out.
+template<class T> struct dblock
+{ dblock() = default;
+  dblock(const dblock &) = delete;
+  dblock &operator=(const dblock &) = delete;
+  dblock(dblock &&o) noexcept : p(o.p), st(o.st) { o.p = nullptr; }
+  dblock &operator=(dblock &&o) noexcept
+    { if (this != &o) { reset(); p = o.p; st = o.st; o.p = nullptr; } return *this; }
+  ~dblock() { reset(); }
+  cudaError_t alloc(size_t count, cudaStream_t s)
+    { reset();
+      void *q = nullptr;
+      cudaError_t e = fgb_dmalloc(&q,sizeof(T)*count,s);
+      if (e == cudaSuccess) { p = (T *) q; st = s; }
+      return e;
+    }
+  void reset() { if (p != nullptr) { fgb_dfree(p,st); p = nullptr; } }
+  T *release() { T *q = p; p = nullptr; return q; }
+  operator T *() const { return p; }
+private:
+  T *p = nullptr;
+  cudaStream_t st = 0;
+};
+
 //  TMA 1-D bulk copy global -> shared (cp.async.bulk, SASS UBLKCP) completed on an mbarrier.
 //  dst/src 16-byte aligned, bytes a multiple of 16.  One elected thread issues; every thread of
 //  the CTA may wait on the barrier phase.

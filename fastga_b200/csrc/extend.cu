@@ -2288,19 +2288,7 @@ la_batch_kernel(ext_params P, const la_job *__restrict__ jobs, const unsigned *_
  *  Host side of the stage
  **********************************************************************************************/
 
-struct fgb_overlaps
-{ long long nrec = 0, nbytes = 0;
-  unsigned char *h_buf = nullptr;          // packed records (OUT_HDR + trace padded to 8)
-  unsigned long long counters[16] = {0};
-  long long nseg = 0, nwork = 0;
-  bool pinned = false;
-};
-
-extern "C" void fgb_overlaps_free(fgb_overlaps *o)
-{ if (!o) return;
-  if (o->h_buf) { if (o->pinned) cudaFreeHost(o->h_buf); else free(o->h_buf); }
-  delete o;
-}
+extern "C" void fgb_overlaps_free(fgb_overlaps *o) { delete o; }
 //  Wraps packed records produced elsewhere (tests feed the host filter without a GPU).
 extern "C" int fgb_overlaps_from_buffer(const unsigned char *buf, long long nbytes, fgb_overlaps **out)
 { fgb_overlaps *o = new fgb_overlaps();
@@ -2463,20 +2451,20 @@ extern "C" long long fgb_hit_groups_host(int nwork, const unsigned *hrange, cons
   return (long long) items.size();
 }
 
-//  Device blocks (and the result handle) of a call go back on EVERY way out of it, error returns included:
-//  the pointer variables are registered once, whatever they hold when the scope ends is released.
-struct dev_scope
-{ cudaStream_t st; std::vector<void **> slots;
-  explicit dev_scope(cudaStream_t s) : st(s) {}
-  template<class T> void own(T *&p) { slots.push_back((void **) &p); }
-  ~dev_scope() { for (void **s : slots) if (*s != NULL) { fgb_dfree(*s,st); *s = NULL; } }
-};
-struct ovl_scope
-{ fgb_overlaps *o;
-  explicit ovl_scope(fgb_overlaps *p) : o(p) {}
-  fgb_overlaps *release() { fgb_overlaps *p = o; o = NULL; return p; }
-  ~ovl_scope() { if (o != NULL) fgb_overlaps_free(o); }
-};
+//  The process-wide grow-only pinned staging buffer of the device-to-host copies (a cudaMallocHost per
+//  call costs ms); *buf gets room for at least `bytes`.
+static cudaError_t pinned_staging(size_t bytes, unsigned char **buf)
+{ static unsigned char *pin = NULL; static size_t pin_cap = 0;
+  if (bytes > pin_cap)
+    { if (pin) cudaFreeHost(pin);
+      pin = NULL; pin_cap = 0;
+      cudaError_t e = cudaMallocHost(&pin,bytes*2 + (8ull << 20));
+      if (e != cudaSuccess) { pin = NULL; return e; }
+      pin_cap = bytes*2 + (8ull << 20);
+    }
+  *buf = pin;
+  return cudaSuccess;
+}
 
 extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B,
                           int chain_break, int chain_min, int align_min, double align_rate,
@@ -2485,9 +2473,7 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
 { cudaStream_t st = (cudaStream_t) stream;
   if (A->d_rseq == NULL) return FGB_ERR_ARG;
   if (S->n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
-  fgb_overlaps *O = new fgb_overlaps();
-  ovl_scope Oown(O);
-  dev_scope G(st);
+  std::unique_ptr<fgb_overlaps> O(new fgb_overlaps());
   long long n = S->n;
   tr_mark("extend: enter");
 
@@ -2508,39 +2494,35 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   P.self_mode = S->self_mode;
   P.dscore = -tables[0] / TRIM_LEN;                     // SCORE[0] = -15 * dscore
 
-  short *d_tables = NULL;
-  u64 *d_counters = NULL, *d_total = NULL;
-  unsigned *d_flag = NULL, *d_seg = NULL, *d_work = NULL, *d_misc = NULL, *d_failed = NULL;
-  void *d_tmp = NULL;
-  G.own(d_tables); G.own(d_counters); G.own(d_total); G.own(d_flag); G.own(d_seg); G.own(d_work);
-  G.own(d_misc); G.own(d_failed); G.own(d_tmp);
-  CUDA_TRY(fgb_dmalloc((void **) &d_tables,65536*sizeof(short),st));
+  dblock<short> d_tables;
+  dblock<u64> d_counters, d_total;
+  dblock<unsigned> d_flag, d_seg, d_work, d_misc, d_failed;
+  dblock<unsigned char> d_tmp;
+  CUDA_TRY(d_tables.alloc(65536,st));
   CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
   P.score = d_tables; P.table = d_tables + 32768;
-  CUDA_TRY(fgb_dmalloc((void **) &d_counters,16*8,st));
+  CUDA_TRY(d_counters.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_counters,0,16*8,st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_total,8,st));
-  CUDA_TRY(fgb_dmalloc((void **) &d_misc,64,st));
+  CUDA_TRY(d_total.alloc(1,st));
+  CUDA_TRY(d_misc.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
   P.counters = d_counters;
 
   unsigned nseg = 0, nwork = 0;
   std::vector<unsigned> wsize; bool sizes_known = false;
-  ChunkPlan *d_plan = NULL; ChunkOut *d_couts = NULL; unsigned *d_first = NULL, *d_failed_w = NULL;
-  ChainHit *d_hits = NULL; uint2 *d_hrange = NULL; unsigned long long hit_cap = 0;
+  dblock<ChunkPlan> d_plan; dblock<ChunkOut> d_couts; dblock<unsigned> d_first, d_failed_w;
+  dblock<ChainHit> d_hits; dblock<uint2> d_hrange; unsigned long long hit_cap = 0;
   //  hit groups (first launch): items in launch order, and for each the first hit of the NEXT group of
   //  its triple (what its tube must not have reached for the groups to have been independent)
-  ExItem *d_items = NULL; long long *d_galast = NULL; int2 *d_tinfo = NULL;
-  G.own(d_plan); G.own(d_couts); G.own(d_first); G.own(d_failed_w); G.own(d_hits); G.own(d_hrange);
-  G.own(d_items); G.own(d_galast); G.own(d_tinfo);
+  dblock<ExItem> d_items; dblock<long long> d_galast; dblock<int2> d_tinfo;
   std::vector<ExItem> items; std::vector<long long> nxt_alow, nxt_ahgh;
   std::vector<unsigned> hwork, hcount;                 // work triples; hits of each pre-scanned one
   unsigned long long hits_done = 0;                    // hits of the pre-scanned triples the first launch completed
   if (n > 0)
     { ev_timer t(0,st);
       long long tmpb = fgb_dev_scan_tmp_bytes(n);
-      CUDA_TRY(fgb_dmalloc((void **) &d_flag,sizeof(unsigned)*(n+1),st));
-      CUDA_TRY(fgb_dmalloc((void **) &d_tmp,tmpb,st));
+      CUDA_TRY(d_flag.alloc(n+1,st));
+      CUDA_TRY(d_tmp.alloc(tmpb,st));
       int nb = (int) ((n + 255) / 256);
       seg_flag_kernel<<<nb,256,0,st>>>(S->d_rec,n,P.p_band,d_flag);
       int rc = fgb_dev_exclusive_scan_u32(d_flag,n,d_total,d_tmp,tmpb,st);
@@ -2550,8 +2532,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
       CUDA_TRY(cudaStreamSynchronize(st));
       nseg = (unsigned) tot;
       TR_SYNC("  seg flags + scan");
-      CUDA_TRY(fgb_dmalloc((void **) &d_seg,sizeof(unsigned)*(nseg+2),st));
-      CUDA_TRY(fgb_dmalloc((void **) &d_work,sizeof(unsigned)*(3ll*nseg+3),st));
+      CUDA_TRY(d_seg.alloc(nseg+2,st));
+      CUDA_TRY(d_work.alloc(3ll*nseg+3,st));
       nb = (int) ((n + 1 + 255) / 256);
       seg_fill2_kernel<<<nb,256,0,st>>>(S->d_rec,n,P.p_band,d_flag,d_seg,nseg);
       P.seg_start = d_seg; P.nseg = (int) nseg;
@@ -2602,12 +2584,12 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
           const int nplan = (int) plan.size();
           if (nplan > 0) {
           hit_cap = (unsigned long long) nplan * (CH_HCAP + 1) + nwork + 16;
-          CUDA_TRY(fgb_dmalloc((void **) &d_plan,sizeof(ChunkPlan)*(size_t) nplan,st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_couts,sizeof(ChunkOut)*(size_t) nplan,st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_first,sizeof(unsigned)*(size_t) (nwork + 1),st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_hits,sizeof(ChainHit)*(size_t) hit_cap,st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_hrange,sizeof(uint2)*(size_t) nwork,st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_tinfo,sizeof(int2)*(size_t) nwork,st));
+          CUDA_TRY(d_plan.alloc((size_t) nplan,st));
+          CUDA_TRY(d_couts.alloc((size_t) nplan,st));
+          CUDA_TRY(d_first.alloc((size_t) (nwork + 1),st));
+          CUDA_TRY(d_hits.alloc((size_t) hit_cap,st));
+          CUDA_TRY(d_hrange.alloc((size_t) nwork,st));
+          CUDA_TRY(d_tinfo.alloc((size_t) nwork,st));
           CUDA_TRY(cudaMemcpyAsync(d_plan,plan.data(),sizeof(ChunkPlan)*(size_t) nplan,cudaMemcpyHostToDevice,st));
           CUDA_TRY(cudaMemcpyAsync(d_first,first.data(),sizeof(unsigned)*(size_t) (nwork + 1),cudaMemcpyHostToDevice,st));
           CUDA_TRY(cudaMemsetAsync(d_misc + 8,0,8,st));
@@ -2640,26 +2622,16 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
             if (getenv("FGB_SPEC_SLACK") != NULL) SPEC_SLACK = atoll(getenv("FGB_SPEC_SLACK"));
             long long SPEC_GAP = -1;                                   // tests: cut at every gap >= this instead
             if (getenv("FGB_SPEC_GAP") != NULL) SPEC_GAP = atoll(getenv("FGB_SPEC_GAP"));
-            //  the small result arrays come back through one pinned scratch buffer (grow-only): four copies in
-            //  flight and one synchronisation instead of a staged, synchronous copy each
-            static unsigned char *hpin = NULL; static size_t hpin_cap = 0;
-            auto pinned = [&](size_t bytes) -> unsigned char *
-              { if (bytes > hpin_cap)
-                  { if (hpin) cudaFreeHost(hpin);
-                    hpin = NULL; hpin_cap = 0;
-                    if (cudaMallocHost(&hpin,bytes*2 + 4096) != cudaSuccess) return NULL;
-                    hpin_cap = bytes*2 + 4096;
-                  }
-                return hpin;
-              };
+            //  the small result arrays come back through the pinned staging buffer: four copies in flight and
+            //  one synchronisation instead of a staged, synchronous copy each
             unsigned long long hused = 0;
             std::vector<uint2> hrange(nwork);
             std::vector<int2> tinfo(nwork);
             hwork.resize(nwork); hcount.assign(nwork,0u);
             { const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork,
                            o4 = o3 + sizeof(unsigned)*(size_t) nwork;
-              unsigned char *hp = pinned(o4);
-              if (hp == NULL) return FGB_ERR_CUDA;
+              unsigned char *hp;
+              CUDA_TRY(pinned_staging(o4,&hp));
               CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
               CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
               CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
@@ -2673,8 +2645,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
             if (hused > hit_cap) hused = hit_cap;
             std::vector<ChainHit> hh((size_t) hused + 1);
             if (hused > 0)
-              { unsigned char *hp = pinned(sizeof(ChainHit)*(size_t) hused);
-                if (hp == NULL) return FGB_ERR_CUDA;
+              { unsigned char *hp;
+                CUDA_TRY(pinned_staging(sizeof(ChainHit)*(size_t) hused,&hp));
                 CUDA_TRY(cudaMemcpyAsync(hp,d_hits,sizeof(ChainHit)*(size_t) hused,cudaMemcpyDeviceToHost,st));
                 CUDA_TRY(cudaStreamSynchronize(st));
                 memcpy(hh.data(),hp,sizeof(ChainHit)*(size_t) hused);
@@ -2682,8 +2654,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
             build_hit_groups(nwork,hrange.data(),tinfo.data(),hh.data(),hused,SPEC_BANDS,SPEC_SLACK,SPEC_GAP,
                              items,nxt_alow,nxt_ahgh,hcount);
             if (!items.empty())
-              { CUDA_TRY(fgb_dmalloc((void **) &d_items,sizeof(ExItem)*items.size(),st));
-                CUDA_TRY(fgb_dmalloc((void **) &d_galast,sizeof(long long)*items.size(),st));
+              { CUDA_TRY(d_items.alloc(items.size(),st));
+                CUDA_TRY(d_galast.alloc(items.size(),st));
                 CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
               }                                                      // (`items` lives until the launches are over)
             TR_SYNC("  chain: hit groups");
@@ -2694,8 +2666,7 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   O->nseg = nseg; O->nwork = nwork;
   tr_mark("extend: triples+prefilter");
 
-  unsigned char *d_out = NULL;
-  G.own(d_out);
+  dblock<unsigned char> d_out;
   u64 out_cap = 0, out_used = 0;
   if (nwork > 0)
     { int dev = 0, nsm = 132;
@@ -2715,8 +2686,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
       if (nblocks > want) nblocks = want;
       long long nwarps = nblocks * EX_WARPS;
 
-      CUDA_TRY(fgb_dmalloc((void **) &d_failed,sizeof(unsigned)*(nwork+1),st));
-      CUDA_TRY(fgb_dmalloc((void **) &d_failed_w,sizeof(unsigned)*(nwork+1),st));
+      CUDA_TRY(d_failed.alloc(nwork+1,st));
+      CUDA_TRY(d_failed_w.alloc(nwork+1,st));
       P.work = d_work; P.nwork = (int) nwork;
       P.queue = d_misc + 1; P.nfailed = d_misc + 2; P.failed = d_failed; P.failed_w = d_failed_w; P.widx = NULL; P.need = d_misc + 10;
       P.out_used = (u64 *) (d_misc + 4);
@@ -2726,28 +2697,26 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
       out_cap = (u64) nwork * 512 + (64ull << 20);
       std::vector<std::pair<unsigned,int> > todo;    // (triple, launch number) of every re-run
       unsigned *d_list = d_work; unsigned nlist = use_items ? (unsigned) items.size() : nwork;
-      unsigned *d_work2 = NULL;
-      dev_scope G2(st); G2.own(d_work2);
+      dblock<unsigned> d_work2;
       u64 used_before = 0;
       for (int attempt = 0; nlist > 0; attempt++)
-        { Peb *d_cells = NULL; unsigned char *d_stage = NULL; unsigned char *d_big = NULL;
-          unsigned long long *d_wlog = NULL;
-          dev_scope L(st); L.own(d_cells); L.own(d_stage); L.own(d_big); L.own(d_wlog);
-          CUDA_TRY(fgb_dmalloc((void **) &d_cells,sizeof(Peb)*cells_per_warp*nwarps,st));
-          CUDA_TRY(fgb_dmalloc((void **) &d_stage,2ll*stage_bytes*nwarps,st));
-          if (d_out == NULL) CUDA_TRY(fgb_dmalloc((void **) &d_out,out_cap,st));
+        { dblock<Peb> d_cells; dblock<unsigned char> d_stage, d_big;
+          dblock<unsigned long long> d_wlog;
+          CUDA_TRY(d_cells.alloc(cells_per_warp*nwarps,st));
+          CUDA_TRY(d_stage.alloc(2ll*stage_bytes*nwarps,st));
+          if (d_out == NULL) CUDA_TRY(d_out.alloc(out_cap,st));
           P.cells = d_cells; P.cells_per_warp = cells_per_warp;
           P.stage = d_stage; P.stage_bytes = stage_bytes;
           P.out = d_out; P.out_cap = out_cap;
           P.work = d_list; P.nwork = (int) nlist;
-          P.items = use_items ? d_items : NULL; P.galast = d_galast; P.attempt = attempt;
+          P.items = use_items ? (ExItem *) d_items : NULL; P.galast = d_galast; P.attempt = attempt;
           if (attempt > 0)                                     // retries: wide-band kernel, state in HBM
-            { CUDA_TRY(fgb_dmalloc((void **) &d_big,(size_t) nwarps * WSTATE_BYTES(EX_WBIG),st));
+            { CUDA_TRY(d_big.alloc((size_t) nwarps * WSTATE_BYTES(EX_WBIG),st));
               P.bigstate = d_big;
             }
           tr_mark("extend: arenas allocated");
           if (attempt == 0 && getenv("FGB_WLOG") != NULL)
-            { CUDA_TRY(fgb_dmalloc((void **) &d_wlog,32ull*(nlist+1),st));
+            { CUDA_TRY(d_wlog.alloc(4ull*(nlist+1),st));
               CUDA_TRY(cudaMemsetAsync(d_wlog,0,32ull*(nlist+1),st));
             }
           P.wlog = d_wlog;
@@ -2778,21 +2747,20 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
                             P.items != NULL ? (items[q].hn & 0x7fffffffu) : 0u,P.items != NULL ? items[q].g : 0u);
                   fclose(f);
                 }
-              fgb_dfree(d_wlog,st); d_wlog = NULL;
+              d_wlog.reset();
             }
-          fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_big,st);
-          d_cells = NULL; d_stage = NULL; d_big = NULL;
+          d_cells.reset(); d_stage.reset(); d_big.reset();     // before the record buffer may grow
           out_used = ((u64) misc[5] << 32) | misc[4];
           unsigned nfailed = misc[2];
           if (out_used > out_cap)
             { //  record buffer too small: grow it (keeping earlier attempts' records) and
               //  repeat this attempt
               if (attempt > 12) return FGB_ERR_OVERFLOW;
-              unsigned char *d_new = NULL;
+              dblock<unsigned char> d_new;
               u64 ncap = out_used * 2 + (64ull << 20);
-              CUDA_TRY(fgb_dmalloc((void **) &d_new,ncap,st));
+              CUDA_TRY(d_new.alloc(ncap,st));
               if (used_before) CUDA_TRY(cudaMemcpy(d_new,d_out,used_before,cudaMemcpyDeviceToDevice));
-              fgb_dfree(d_out,st); d_out = d_new; out_cap = ncap;
+              d_out = std::move(d_new); out_cap = ncap;
               CUDA_TRY(cudaMemcpy(d_misc+4,&used_before,8,cudaMemcpyHostToDevice));
               out_used = used_before;
               for (size_t q = 0; q < todo.size(); q++)            // the repeat runs under the next launch number
@@ -2833,7 +2801,7 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
           //  rerun only the failed triples (whole, hit after hit) with larger arenas on fewer warps; the
           //  records of their earlier launches are dropped by the host below.
           for (size_t q = 0; q < f.size(); q++) todo.push_back(std::make_pair(f[q],attempt + 1));
-          if (d_work2 == NULL) CUDA_TRY(cudaMalloc(&d_work2,sizeof(unsigned)*2*(nwork+1)));
+          if (d_work2 == NULL) CUDA_TRY(d_work2.alloc(2*(nwork+1),st));
           CUDA_TRY(cudaMemcpy(d_work2,f.data(),sizeof(unsigned)*nfailed,cudaMemcpyHostToDevice));
           CUDA_TRY(cudaMemcpy(d_work2 + nwork + 1,fw.data(),sizeof(unsigned)*nfailed,cudaMemcpyHostToDevice));
           P.widx = d_work2 + nwork + 1;
@@ -2848,20 +2816,14 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
           nblocks = nb2 < maxb ? nb2 : maxb;
           nwarps = nblocks * EX_WARPS;
         }
-      fgb_dfree(d_work2,st); d_work2 = NULL;
+      d_work2.reset();
 
       //  bring the records back and drop partial output of triples that were re-run
       O->nbytes = (long long) out_used;
       tr_mark("extend: attempts done");
-      //  D2H through a grow-only pinned staging buffer (cudaMallocHost per step costs ms)
-      static unsigned char *pin = NULL; static u64 pin_cap = 0;
-      if (out_used + 64 > pin_cap)
-        { if (pin) cudaFreeHost(pin);
-          pin_cap = out_used * 2 + (8ull << 20);
-          CUDA_TRY(cudaMallocHost(&pin,pin_cap));
-        }
+      unsigned char *pin;
+      CUDA_TRY(pinned_staging(out_used + 64,&pin));
       O->h_buf = (unsigned char *) malloc(out_used + 64);
-      O->pinned = false;
       { ev_timer t(2,st);
         CUDA_TRY(cudaMemcpyAsync(pin,d_out,out_used,cudaMemcpyDeviceToHost,st));
       }
@@ -2910,7 +2872,7 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
     O->nrec = cnt;
   }
   tr_mark("extend: leave");
-  *out = Oown.release();                                     // (the device blocks go back as G leaves scope)
+  *out = O.release();                                        // (the device blocks go back as the call returns)
   return FGB_OK;
 }
 
@@ -2949,25 +2911,23 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   const long long cells_per_warp = 1ll << 18;
   const int stage_bytes = 1 << 16;
   const size_t smem = (size_t) EX_WARPS * STATE_BYTES;
-  short *d_tables = NULL; la_job *d_jobs = NULL; int *d_status = NULL; unsigned *d_misc = NULL;
-  Peb *d_cells = NULL; unsigned char *d_stage = NULL, *d_out = NULL, *d_big = NULL; unsigned *d_idx = NULL;
+  dblock<short> d_tables; dblock<la_job> d_jobs; dblock<int> d_status; dblock<unsigned> d_misc;
+  dblock<Peb> d_cells; dblock<unsigned char> d_stage, d_out, d_big; dblock<unsigned> d_idx;
   long long cells_big = cells_per_warp; int stage_big = stage_bytes;
   std::vector<unsigned char> h;
   std::vector<int> hs(n);
   u64 out_cap = (u64) n * 256 + (u64) traces_cap + (1ull << 20), out_used = 0;
-  int rc = FGB_OK;
-#define LA_TRY(call) do { if ((call) != cudaSuccess) { rc = FGB_ERR_CUDA; goto done; } } while (0)
-  LA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
-  LA_TRY(fgb_dmalloc((void **) &d_tables,65536*sizeof(short),st));
-  LA_TRY(fgb_dmalloc((void **) &d_jobs,sizeof(la_job)*(size_t) n,st));
-  LA_TRY(fgb_dmalloc((void **) &d_status,sizeof(int)*(size_t) n,st));
-  LA_TRY(fgb_dmalloc((void **) &d_misc,64,st));
-  LA_TRY(fgb_dmalloc((void **) &d_cells,sizeof(Peb)*cells_per_warp*nwarps,st));
-  LA_TRY(fgb_dmalloc((void **) &d_stage,2ll*stage_bytes*nwarps,st));
-  LA_TRY(fgb_dmalloc((void **) &d_out,out_cap,st));
-  LA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
-  LA_TRY(cudaMemcpyAsync(d_jobs,jobs,sizeof(la_job)*(size_t) n,cudaMemcpyHostToDevice,st));
-  LA_TRY(cudaMemsetAsync(d_misc,0,64,st));
+  CUDA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
+  CUDA_TRY(d_tables.alloc(65536,st));
+  CUDA_TRY(d_jobs.alloc((size_t) n,st));
+  CUDA_TRY(d_status.alloc((size_t) n,st));
+  CUDA_TRY(d_misc.alloc(16,st));
+  CUDA_TRY(d_cells.alloc(cells_per_warp*nwarps,st));
+  CUDA_TRY(d_stage.alloc(2ll*stage_bytes*nwarps,st));
+  CUDA_TRY(d_out.alloc(out_cap,st));
+  CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(d_jobs,jobs,sizeof(la_job)*(size_t) n,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
   P.score = d_tables; P.table = d_tables + 32768;
   P.cells = d_cells; P.cells_per_warp = cells_per_warp;
   P.stage = d_stage; P.stage_bytes = stage_bytes;
@@ -2975,11 +2935,11 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   P.queue = d_misc + 1;
   la_batch_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P,d_jobs,NULL,(int) n,d_status);
   fgb_count_launch(1);
-  LA_TRY(cudaGetLastError());
-  LA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
-  LA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
-  LA_TRY(cudaStreamSynchronize(st));
-  if (out_used > out_cap) { rc = FGB_ERR_OVERFLOW; goto done; }
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (out_used > out_cap) return FGB_ERR_OVERFLOW;
   //  calls that did not fit (a band wider than EX_W diagonals, a full arena): again on the wide-band
   //  kernel with the wave state in HBM, growing the arenas each round, as fgb_extend re-runs its triples.
   //  A failed call emitted nothing, so its record comes from the round that completes it.
@@ -2988,7 +2948,7 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       for (long long i = 0; i < n; i++)
         if (hs[i] != ST_OK) redo.push_back((unsigned) i);
       if (redo.empty()) break;
-      if (attempt > 4) { rc = FGB_ERR_OVERFLOW; goto done; }
+      if (attempt > 4) return FGB_ERR_OVERFLOW;
       if (attempt > 1) { cells_big *= 8; stage_big *= 4; }
       const size_t smem_big = (size_t) EX_WARPS * BIG_SMEM_PER_WARP;
       long long nb2 = ((long long) redo.size() + EX_WARPS - 1) / EX_WARPS;
@@ -2996,52 +2956,45 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       long long maxb = (24ll << 30) / ((long long) sizeof(Peb) * cells_big * EX_WARPS);
       if (nb2 > maxb) nb2 = maxb > 1 ? maxb : 1;
       const long long nw2 = nb2 * EX_WARPS;
-      fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_big,st); fgb_dfree(d_idx,st);
-      d_cells = NULL; d_stage = NULL; d_big = NULL; d_idx = NULL;
-      LA_TRY(fgb_dmalloc((void **) &d_cells,sizeof(Peb)*cells_big*nw2,st));
-      LA_TRY(fgb_dmalloc((void **) &d_stage,2ll*stage_big*nw2,st));
-      LA_TRY(fgb_dmalloc((void **) &d_big,(size_t) nw2 * WSTATE_BYTES(EX_WBIG),st));
-      LA_TRY(fgb_dmalloc((void **) &d_idx,sizeof(unsigned)*redo.size(),st));
-      LA_TRY(cudaMemcpyAsync(d_idx,redo.data(),sizeof(unsigned)*redo.size(),cudaMemcpyHostToDevice,st));
-      LA_TRY(cudaMemsetAsync(d_misc + 1,0,4,st));                 // queue
-      LA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
+      d_cells.reset(); d_stage.reset(); d_big.reset(); d_idx.reset();      // all four before the larger ones
+      CUDA_TRY(d_cells.alloc(cells_big*nw2,st));
+      CUDA_TRY(d_stage.alloc(2ll*stage_big*nw2,st));
+      CUDA_TRY(d_big.alloc((size_t) nw2 * WSTATE_BYTES(EX_WBIG),st));
+      CUDA_TRY(d_idx.alloc(redo.size(),st));
+      CUDA_TRY(cudaMemcpyAsync(d_idx,redo.data(),sizeof(unsigned)*redo.size(),cudaMemcpyHostToDevice,st));
+      CUDA_TRY(cudaMemsetAsync(d_misc + 1,0,4,st));                 // queue
+      CUDA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
       P.cells = d_cells; P.cells_per_warp = cells_big;
       P.stage = d_stage; P.stage_bytes = stage_big;
       P.bigstate = d_big;
       la_batch_kernel<EX_WBIG><<<(unsigned) nb2,EX_WARPS*32,smem_big,st>>>(P,d_jobs,d_idx,(int) redo.size(),d_status);
       fgb_count_launch(1);
-      LA_TRY(cudaGetLastError());
-      LA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
-      LA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
-      LA_TRY(cudaStreamSynchronize(st));
-      if (out_used > out_cap) { rc = FGB_ERR_OVERFLOW; goto done; }
+      CUDA_TRY(cudaGetLastError());
+      CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      if (out_used > out_cap) return FGB_ERR_OVERFLOW;
     }
   h.resize((size_t) out_used + 64);
-  LA_TRY(cudaMemcpy(h.data(),d_out,out_used,cudaMemcpyDeviceToHost));
-  { long long used = 0;
-    for (long long i = 0; i < n; i++)
-      { int *p = paths + 7*i;
-        p[0] = p[1] = p[2] = p[3] = p[4] = p[5] = 0; p[6] = hs[i];
-        toff[i] = 0;
-      }
-    for (u64 off = 0; off < out_used; )
-      { const int *r = (const int *) (h.data() + off);
-        const long long i = r[0];
-        int *p = paths + 7*i;
-        p[0] = r[3]; p[1] = r[4]; p[2] = r[5]; p[3] = r[6]; p[4] = r[7]; p[5] = r[8];
-        toff[i] = used;
-        if (used + r[8] <= traces_cap) memcpy(traces + used,h.data() + off + OUT_HDR,(size_t) r[8]);
-        used += r[8];
-        off += OUT_HDR + ((r[8] + 7) & ~7);
-      }
-    *traces_used = used;
-    if (used > traces_cap) rc = FGB_ERR_OVERFLOW;
-  }
-done:
-#undef LA_TRY
-  fgb_dfree(d_tables,st); fgb_dfree(d_jobs,st); fgb_dfree(d_status,st); fgb_dfree(d_misc,st);
-  fgb_dfree(d_cells,st); fgb_dfree(d_stage,st); fgb_dfree(d_out,st); fgb_dfree(d_big,st); fgb_dfree(d_idx,st);
-  return rc;
+  CUDA_TRY(cudaMemcpy(h.data(),d_out,out_used,cudaMemcpyDeviceToHost));
+  long long used = 0;
+  for (long long i = 0; i < n; i++)
+    { int *p = paths + 7*i;
+      p[0] = p[1] = p[2] = p[3] = p[4] = p[5] = 0; p[6] = hs[i];
+      toff[i] = 0;
+    }
+  for (u64 off = 0; off < out_used; )
+    { const int *r = (const int *) (h.data() + off);
+      const long long i = r[0];
+      int *p = paths + 7*i;
+      p[0] = r[3]; p[1] = r[4]; p[2] = r[5]; p[3] = r[6]; p[4] = r[7]; p[5] = r[8];
+      toff[i] = used;
+      if (used + r[8] <= traces_cap) memcpy(traces + used,h.data() + off + OUT_HDR,(size_t) r[8]);
+      used += r[8];
+      off += OUT_HDR + ((r[8] + 7) & ~7);
+    }
+  *traces_used = used;
+  return used > traces_cap ? FGB_ERR_OVERFLOW : FGB_OK;
 }
 
 extern "C" long long fgb_overlaps_count(const fgb_overlaps *o) { return o->nrec; }

@@ -459,26 +459,22 @@ extern "C" int fgb_forward_view_device(const void *d_T, long long n, void *d_out
 { cudaStream_t st = (cudaStream_t) stream;
   *h_nfwd = 0;
   if (n <= 0) return FGB_OK;
-  unsigned *d_flag = NULL; void *d_tmp = NULL; unsigned long long *d_total = NULL;
+  dblock<unsigned> d_flag; dblock<unsigned char> d_tmp; dblock<unsigned long long> d_total;
   long long tmpb = fgb_dev_scan_tmp_bytes(n);
-  cudaError_t e;
-  if ((e = fgb_dmalloc((void **) &d_flag,sizeof(unsigned)*(n+1),st)) != cudaSuccess ||
-      (e = fgb_dmalloc(&d_tmp,tmpb,st)) != cudaSuccess ||
-      (e = fgb_dmalloc((void **) &d_total,8,st)) != cudaSuccess)
-    { fgb_dfree(d_flag,st); fgb_dfree(d_tmp,st); fgb_dfree(d_total,st); return FGB_ERR_CUDA; }
+  CUDA_TRY(d_flag.alloc(n+1,st));
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
+  CUDA_TRY(d_total.alloc(1,st));
   int nb = (int) ((n + 255) / 256);
   fwd_flag_kernel<<<nb,256,0,st>>>((const rec128 *) d_T,n,d_flag);
   int rc = fgb_dev_exclusive_scan_u32(d_flag,n,d_total,d_tmp,tmpb,st);
+  if (rc) return rc;
   unsigned long long tot = 0;
-  if (!rc)
-    { fwd_scatter_kernel<<<nb,256,0,st>>>((const rec128 *) d_T,n,d_flag,(rec128 *) d_out);
-      fgb_count_launch(2);
-      if (cudaMemcpyAsync(&tot,d_total,8,cudaMemcpyDeviceToHost,st) != cudaSuccess ||
-          cudaStreamSynchronize(st) != cudaSuccess) rc = FGB_ERR_CUDA;
-    }
-  fgb_dfree(d_flag,st); fgb_dfree(d_tmp,st); fgb_dfree(d_total,st);
+  fwd_scatter_kernel<<<nb,256,0,st>>>((const rec128 *) d_T,n,d_flag,(rec128 *) d_out);
+  fgb_count_launch(2);
+  CUDA_TRY(cudaMemcpyAsync(&tot,d_total,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   *h_nfwd = (long long) tot;
-  return rc;
+  return FGB_OK;
 }
 
 /***********************************************************************************************
@@ -609,8 +605,8 @@ static int merge_launch(const rec128 *T1, unsigned n1, const rec128 *T2, const u
 { const int smem = (int) sizeof(mg_stage<TILE>);
   CUDA_TRY(cudaFuncSetAttribute(adaptamer_merge_kernel<TILE>,cudaFuncAttributeMaxDynamicSharedMemorySize,smem));
   unsigned nb = (unsigned) (((unsigned long long) n1 + TILE - 1) / TILE);
-  uint4 *d_rng = NULL;
-  CUDA_TRY(fgb_dmalloc((void **) &d_rng,sizeof(uint4)*(size_t) nb,st));
+  dblock<uint4> d_rng;
+  CUDA_TRY(d_rng.alloc((size_t) nb,st));
   cudaEvent_t ea, eb;
   cudaEventCreate(&ea); cudaEventCreate(&eb);
   cudaEventRecord(ea,st);
@@ -622,7 +618,6 @@ static int merge_launch(const rec128 *T1, unsigned n1, const rec128 *T2, const u
   fgb_timing_add(3,ms);
   fgb_count_launch(2);
   cudaEventDestroy(ea); cudaEventDestroy(eb);
-  fgb_dfree(d_rng,st);
   return FGB_OK;
 }
 

@@ -97,15 +97,15 @@ extern "C" void fgb_msd_sort(unsigned char *array, long long nelem, int rsize, i
   poff[0] = 0;
   for (int x = 0; x < np; x++) poff[x+1] = poff[x] + part[beg+x]/rsize;
   cudaStream_t st = 0;
-  unsigned char *d_src = NULL, *d_dst = NULL; long long *d_poff = NULL;
-  rec128 *d_a = NULL, *d_b = NULL; void *d_tmp = NULL;
+  dblock<unsigned char> d_src, d_dst; dblock<long long> d_poff;
+  dblock<rec128> d_a, d_b; dblock<unsigned char> d_tmp;
   long long tmpb = fgb_sort128_tmp_bytes(nelem);
-  bool ok = fgb_dmalloc((void **) &d_src,asize+16,st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_dst,asize+16,st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_poff,8*(np+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_a,16*(nelem+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_b,16*(nelem+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_tmp,tmpb,st) == cudaSuccess;
+  bool ok = d_src.alloc(asize+16,st) == cudaSuccess &&
+            d_dst.alloc(asize+16,st) == cudaSuccess &&
+            d_poff.alloc(np+1,st) == cudaSuccess &&
+            d_a.alloc(nelem+1,st) == cudaSuccess &&
+            d_b.alloc(nelem+1,st) == cudaSuccess &&
+            d_tmp.alloc(tmpb,st) == cudaSuccess;
   if (!ok) { fprintf(stderr,"fastga_b200: fgb_msd_sort: out of device memory\n"); exit(1); }
   cudaMemcpyAsync(d_src,array,asize,cudaMemcpyHostToDevice,st);
   cudaMemcpyAsync(d_poff,poff,8*(np+1),cudaMemcpyHostToDevice,st);
@@ -121,8 +121,6 @@ extern "C" void fgb_msd_sort(unsigned char *array, long long nelem, int rsize, i
   //  first records of the panels are set by the boundary rule; the very first is 0 (MSDsort.c:485)
   array[0] = 0;
   array[asize] = 1;
-  fgb_dfree(d_src,st); fgb_dfree(d_dst,st); fgb_dfree(d_poff,st);
-  fgb_dfree(d_a,st); fgb_dfree(d_b,st); fgb_dfree(d_tmp,st);
   free(poff);
 }
 
@@ -185,14 +183,14 @@ extern "C" int fgb_rmsd_sort(unsigned char *array, long long nelem, int rsize, i
   poff[0] = 0;
   for (x = 0; x < nparts; x++) poff[x+1] = poff[x] + part[x]/rsize;
   cudaStream_t st = 0;
-  unsigned char *d_src = NULL; long long *d_poff = NULL;
-  rec128 *d_a = NULL, *d_b = NULL; void *d_tmp = NULL;
+  dblock<unsigned char> d_src; dblock<long long> d_poff;
+  dblock<rec128> d_a, d_b; dblock<unsigned char> d_tmp;
   long long tmpb = fgb_sort128_tmp_bytes(nelem);
-  bool ok = fgb_dmalloc((void **) &d_src,asize+16,st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_poff,8*(nparts+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_a,16*(nelem+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_b,16*(nelem+1),st) == cudaSuccess &&
-            fgb_dmalloc((void **) &d_tmp,tmpb,st) == cudaSuccess;
+  bool ok = d_src.alloc(asize+16,st) == cudaSuccess &&
+            d_poff.alloc(nparts+1,st) == cudaSuccess &&
+            d_a.alloc(nelem+1,st) == cudaSuccess &&
+            d_b.alloc(nelem+1,st) == cudaSuccess &&
+            d_tmp.alloc(tmpb,st) == cudaSuccess;
   if (!ok) { fprintf(stderr,"fastga_b200: fgb_rmsd_sort: out of device memory\n"); exit(1); }
   cudaMemcpyAsync(d_src,array,asize,cudaMemcpyHostToDevice,st);
   cudaMemcpyAsync(d_poff,poff,8*(nparts+1),cudaMemcpyHostToDevice,st);
@@ -208,7 +206,6 @@ extern "C" int fgb_rmsd_sort(unsigned char *array, long long nelem, int rsize, i
   cudaMemcpyAsync(array,d_src,asize,cudaMemcpyDeviceToHost,st);
   if (cudaStreamSynchronize(st) != cudaSuccess)
     { fprintf(stderr,"fastga_b200: fgb_rmsd_sort: %s\n",cudaGetErrorString(cudaGetLastError())); exit(1); }
-  fgb_dfree(d_src,st); fgb_dfree(d_poff,st); fgb_dfree(d_a,st); fgb_dfree(d_b,st); fgb_dfree(d_tmp,st);
   free(poff);
   return n;
 }

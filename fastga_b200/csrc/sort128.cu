@@ -807,9 +807,9 @@ static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins
     if (gc) groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0));
   }
 
-  uint4 *d_groups = NULL;
+  dblock<uint4> d_groups;
   if (!groups.empty())
-    { CUDA_TRY(fgb_dmalloc((void **) &d_groups,sizeof(uint4)*groups.size(),st));
+    { CUDA_TRY(d_groups.alloc(groups.size(),st));
       CUDA_TRY(cudaMemcpyAsync(d_groups,groups.data(),sizeof(uint4)*groups.size(),cudaMemcpyHostToDevice,st));
       kmer_bucket_sort_kernel<<<(unsigned) groups.size(),BK_THREADS,BUCKET_SMEM,st>>>(src,dst,d_groups,binshift);
       fgb_count_launch(1);
@@ -819,12 +819,12 @@ static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins
     { int nseg = (int) ofrom.size();
       opre.push_back(ototal);
       std::vector<unsigned> cfrom(opre.begin(),opre.end()-1);            // position in the compact array
-      rec128 *d_c1 = NULL, *d_c2 = NULL; void *d_ctmp = NULL; unsigned *d_seg = NULL;
+      dblock<rec128> d_c1, d_c2; dblock<unsigned char> d_ctmp; dblock<unsigned> d_seg;
       long long ctb = fgb_sort128_tmp_bytes(ototal);
-      CUDA_TRY(fgb_dmalloc((void **) &d_c1,sizeof(rec128)*((size_t) ototal+1),st));
-      CUDA_TRY(fgb_dmalloc((void **) &d_c2,sizeof(rec128)*((size_t) ototal+1),st));
-      CUDA_TRY(fgb_dmalloc(&d_ctmp,ctb,st));
-      CUDA_TRY(fgb_dmalloc((void **) &d_seg,sizeof(unsigned)*(3*(size_t) nseg+1),st));
+      CUDA_TRY(d_c1.alloc((size_t) ototal+1,st));
+      CUDA_TRY(d_c2.alloc((size_t) ototal+1,st));
+      CUDA_TRY(d_ctmp.alloc(ctb,st));
+      CUDA_TRY(d_seg.alloc(3*(size_t) nseg+1,st));
       CUDA_TRY(cudaMemcpyAsync(d_seg,ofrom.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
       CUDA_TRY(cudaMemcpyAsync(d_seg+nseg,cfrom.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
       CUDA_TRY(cudaMemcpyAsync(d_seg+2*nseg,opre.data(),sizeof(unsigned)*(nseg+1),cudaMemcpyHostToDevice,st));
@@ -837,10 +837,8 @@ static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins
       fgb_count_launch(2);
       CUDA_TRY(cudaGetLastError());
       CUDA_TRY(cudaStreamSynchronize(st));                // the staging vectors above must outlive the copies
-      fgb_dfree(d_c1,st); fgb_dfree(d_c2,st); fgb_dfree(d_ctmp,st); fgb_dfree(d_seg,st);
     }
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (d_groups) fgb_dfree(d_groups,st);
   return FGB_OK;
 }
 
@@ -865,8 +863,8 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
   if (rc) return rc;
   rec128 *src = (rec128 *) (inb ? d_b : d_a), *dst = (rec128 *) (inb ? d_a : d_b);
 
-  unsigned *d_bins = NULL;
-  CUDA_TRY(fgb_dmalloc((void **) &d_bins,sizeof(unsigned)*(size_t) (nbins+1),st));
+  dblock<unsigned> d_bins;
+  CUDA_TRY(d_bins.alloc((size_t) (nbins+1),st));
   { int nb = (int) ((n + 1 + 255) / 256);
     kmer_bins_kernel<<<nb,256,0,st>>>(src,n,binshift,base,d_bins,nbins);
     fgb_count_launch(1);
@@ -874,7 +872,7 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
   std::vector<unsigned> bins((size_t) nbins + 1);
   CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*(size_t) (nbins+1),cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  fgb_dfree(d_bins,st);
+  d_bins.reset();                                       // before the bucket sort allocates its own
   rc = kmer_sort_binned(src,dst,bins.data(),nbins,sh,plo,st);
   if (rc) return rc;
   *result_in_b = inb ^ 1;

@@ -48,6 +48,14 @@ def device_ready():
     return bool(load_library().fgb_device_ready())
 
 
+def device_live_bytes():
+    """bytes of device blocks the library's block cache has handed out and not taken back"""
+    L = load_library()
+    L.fgb_device_live_bytes.restype = c_ll
+    L.fgb_device_live_bytes.argtypes = []
+    return L.fgb_device_live_bytes()
+
+
 class DeviceGenome:
     """fgb_genome handle: the staged 2-bit contigs of one genome in HBM."""
 

@@ -246,6 +246,7 @@ long long fgb_hit_groups_host(int nwork, const unsigned *hrange, const int *tinf
 /* ---- housekeeping ---- */
 int  fgb_device_ready(void);
 void fgb_release_cache(void);      /* return cached device blocks to the driver */
+long long fgb_device_live_bytes(void);   /* bytes of device blocks handed out and not yet released */
 void fgb_timings_reset(void);
 void fgb_timings_get(fgb_timings *out);
 
