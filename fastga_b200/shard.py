@@ -164,11 +164,14 @@ def exchange_rows(dist, rows, send_rows, async_op=False):
 
 def align_sharded(dA, dB, freqA, dist, device, **kw):
     """The whole path on world GPUs from device-resident genomes (every rank holds both genomes:
-    2 bits per base).  Returns (Alignments of this rank's A-contigs with GLOBAL contig numbers, stats)."""
+    2 bits per base).  Returns (Alignments of this rank's A-contigs with GLOBAL contig numbers, stats).
+    on_seeds: called with (the seed records this rank received, their layout bits) before they are
+    sorted -- lets a caller check the owner routing, which the records alone cannot show."""
     import torch
     from . import lib
     rank, world = dist.get_rank(), dist.get_world_size()
     gA, gB = dA.genome, dB.genome
+    on_seeds = kw.pop("on_seeds", None)
     p = dict(lib.DEFAULTS)
     p.update(kw)
     import os, sys, time
@@ -237,6 +240,8 @@ def align_sharded(dA, dB, freqA, dist, device, **kw):
     send = [int(bounds[r + 1] - bounds[r]) for r in range(world)]
     recv = exchange_rows(dist, grouped, send)
     mark("exchange seeds")
+    if on_seeds is not None:
+        on_seeds(recv, bits)
     del grouped
     S = lib.seeds_from_records(recv.data_ptr() if recv.shape[0] else 0, int(recv.shape[0]), bits, amx, bmx)
     nseeds_mine = int(recv.shape[0])

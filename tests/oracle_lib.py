@@ -388,11 +388,16 @@ def seed_layout(gA, gB):
             int(max(gA.ncontig - 1, 1)).bit_length(), amx, bmx)
 
 
-def oracle_pipeline(gA, gB, **kw):
-    """The whole path through the CPU oracle + the product's host filter.  Returns a dict."""
+def oracle_pipeline(gA, gB, rank=None, **kw):
+    """The whole path through the CPU oracle + the product's host filter.  Returns a dict.
+    rank: (rank of every A contig, of every B contig) in place of contig_rank's, for genomes whose
+    length ties leave the order open."""
     from fastga_b200 import lib
     pa, ra = contig_rank(gA.clen)
     pb, rb = contig_rank(gB.clen)
+    if rank is not None:
+        ra, rb = (np.asarray(r, dtype=np.int32) for r in rank)
+        pa, pb = np.argsort(ra).astype(np.int32), np.argsort(rb).astype(np.int32)
     tA, sA = gix_build(gA, ra)
     tB, sB = gix_build(gB, rb)
     seeds, sumlen = merge(tA, tB, sB, kw.get("freq", 10))

@@ -8,6 +8,7 @@ import tempfile
 
 import pytest
 
+import edge_cases
 import oracle_lib as ol
 from fastga_b200 import formats, synth
 
@@ -32,14 +33,32 @@ def _pair(wd, seed, total, ncontig, div, sv):
 def test_dropin_1aln_equals_stock_binary():
     with tempfile.TemporaryDirectory() as wd:
         _pair(wd, 31, 3_000_000, 4, 0.05, 60_000)
-        stock = os.path.join(ol.REF_DIR, "FastGA")
-        _, log_ref = _run(stock, ["-v", "-k", "-T8", "-P" + wd, "-1:ref", "A", "B"], wd)
-        _, log_b200 = _run(DROPIN, ["-v", "-T8", "-P" + wd, "-1:b200", "A", "B"], wd)
-        ref = ol.oneview_records(os.path.join(wd, "ref.1aln"))
-        got = ol.oneview_records(os.path.join(wd, "b200.1aln"))
-        assert len(ref) > 10 and got == ref
-        a, b = ol.parse_fastga_log(log_ref), ol.parse_fastga_log(log_b200)      # the -v lines scripts parse
-        assert (a["seeds"], a["hits"], a["alns"], a["kept"]) == (b["seeds"], b["hits"], b["alns"], b["kept"])
+        _same_1aln(wd)
+
+
+@pytest.mark.skipif(not (ol.have_ref() and os.path.exists(DROPIN)), reason="oracle/_ref/b200/FastGA not built")
+def test_dropin_1aln_equals_stock_binary_past_255_contigs():
+    """the icont_straddles pair of tests/edge_cases.py: 300 A contigs, so the hook converts records
+    whose contig ids do not fit a byte, from seeds whose icont field straddles bit 64"""
+    A, B, _, _ = edge_cases.icont_straddles()
+    with tempfile.TemporaryDirectory() as wd:
+        formats.write_fasta(os.path.join(wd, "A.fasta"), synth.scaffolds_of(A, "sa", 1))
+        formats.write_fasta(os.path.join(wd, "B.fasta"), synth.scaffolds_of(B, "sb", 1))
+        ref = _same_1aln(wd)
+        assert max(int(r.split()[1]) for r in ref) > 255
+
+
+def _same_1aln(wd):
+    """stock FastGA and the drop-in on A and B in wd: same canonical records, same -v counters"""
+    stock = os.path.join(ol.REF_DIR, "FastGA")
+    _, log_ref = _run(stock, ["-v", "-k", "-T8", "-P" + wd, "-1:ref", "A", "B"], wd)
+    _, log_b200 = _run(DROPIN, ["-v", "-T8", "-P" + wd, "-1:b200", "A", "B"], wd)
+    ref = ol.oneview_records(os.path.join(wd, "ref.1aln"))
+    got = ol.oneview_records(os.path.join(wd, "b200.1aln"))
+    assert len(ref) > 10 and got == ref
+    a, b = ol.parse_fastga_log(log_ref), ol.parse_fastga_log(log_b200)      # the -v lines scripts parse
+    assert (a["seeds"], a["hits"], a["alns"], a["kept"]) == (b["seeds"], b["hits"], b["alns"], b["kept"])
+    return ref
 
 
 @pytest.mark.skipif(not (ol.have_ref() and os.path.exists(DROPIN)), reason="oracle/_ref/b200/FastGA not built")

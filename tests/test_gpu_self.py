@@ -10,7 +10,7 @@ from test_oracle_pin import _self_genomes
 pytestmark = pytest.mark.gpu
 
 
-@pytest.mark.parametrize("name", ["dup", "tandem61", "tandem62"])
+@pytest.mark.parametrize("name", ["dup", "tandem61", "tandem62", "contigs300"])
 def test_self_mode_bit_exact_vs_oracle(name):
     g = formats.genome_from_arrays(_self_genomes()[name])
     want = ol.oracle_pipeline_self(g)

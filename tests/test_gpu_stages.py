@@ -253,11 +253,14 @@ class _Range(C.Structure):
     _fields_ = [("beg", C.c_int), ("end", C.c_int), ("off", C.c_int64)]
 
 
-def test_msd_sort_seam_matches_reference():
-    from fastga_b200 import load_library
-    L = load_library()
+MSD_SHAPES = {15: "seam/msd_sort",            # GIXmake's shape on EXAMPLE: swide 15, KBYTES 10
+              17: "seam/msd_sort_swide17"}    # 4-byte posts and 2-byte contigs: swide 11 + 4 + 2
+
+
+def _msd_case(rsize):
+    """GIXmake's msd_sort call on records of rsize bytes: (inputs, sort(f), the reference's result)"""
     rng = np.random.default_rng(9)
-    rsize, ksize, beg, end = 15, 10, 3, 40           # GIXmake's shape on EXAMPLE: swide 15, KBYTES 10
+    ksize, beg, end = 10, 3, 40
     counts = rng.integers(0, 3000, end - beg)
     counts[5] = 0
     n = int(counts.sum())
@@ -271,7 +274,7 @@ def test_msd_sort_seam_matches_reference():
     def canon(r):                                    # payloads: same multiset per equal-key run
         run = np.cumsum(r[:, 0] != 0)
         pay = np.zeros(n, dtype=np.uint64)
-        for k in range(ksize, rsize):
+        for k in range(ksize, rsize):                # <= 8 payload bytes
             pay |= r[:, k].astype(np.uint64) << np.uint64(8 * (k - ksize))
         return pay[np.lexsort((pay, run))]
 
@@ -281,19 +284,34 @@ def test_msd_sort_seam_matches_reference():
         f(a.ctypes.data, n, rsize, ksize, part.ctypes.data, beg, end, 4)
         r = a[:n * rsize].reshape(n, rsize)
         return {"end": int(a[n * rsize]), "keys_md5": _md5(r[:, :ksize]), "payload_md5": _md5(canon(r))}
-    want = ol.reference("seam/msd_sort", ol.digest(arr, part), lambda: sort(C.CDLL(ol.REF_SO).msd_sort))
-    got = sort(L.fgb_msd_sort)
+    return sort, ol.reference(MSD_SHAPES[rsize], ol.digest(arr, part), lambda: sort(C.CDLL(ol.REF_SO).msd_sort))
+
+
+def test_msd_sort_seam_matches_reference():
+    _msd_compare(15)
+
+
+def test_msd_sort_seam_matches_reference_at_4_byte_posts_and_2_byte_contigs():
+    _msd_compare(17)
+
+
+def _msd_compare(rsize):
+    from fastga_b200 import load_library
+    sort, want = _msd_case(rsize)
+    got = sort(load_library().fgb_msd_sort)
     assert want["end"] == got["end"] == 1
     assert got["keys_md5"] == want["keys_md5"]                   # LCP byte + key bytes identical
     assert got["payload_md5"] == want["payload_md5"]
 
 
-def test_rmsd_sort_seam_matches_reference():
-    from fastga_b200 import load_library
-    L = load_library()
+RMSD_SHAPES = {(9, 37): "seam/rmsd_sort",                 # FastGA's seed record on EXAMPLE: swide 9
+               (12, 300): "seam/rmsd_sort_swide12"}       # DBYTE 4, JCONT 2: swide 12, > 256 parts
+
+
+def _rmsd_case(rsize, nparts):
     rng = np.random.default_rng(10)
-    rsize, nparts, nthreads = 9, 37, 8                # FastGA's seed record on EXAMPLE: swide 9
-    counts = rng.integers(0, 5000, nparts)
+    nthreads = 8
+    counts = rng.integers(0, 5000 if nparts < 256 else 600, nparts)
     counts[[0, 7]] = 0
     n = int(counts.sum())
     arr = rng.integers(0, 256, (n, rsize), dtype=np.uint8)
@@ -306,5 +324,19 @@ def test_rmsd_sort_seam_matches_reference():
         f.argtypes = argt
         k = f(a.ctypes.data, n, rsize, rsize, nparts, part.ctypes.data, nthreads, p)
         return {"ranges": [[p[i].beg, p[i].end, p[i].off] for i in range(k)], "md5": _md5(a)}
-    want = ol.reference("seam/rmsd_sort", ol.digest(arr, part), lambda: sort(C.CDLL(ol.REF_SO).rmsd_sort))
-    assert sort(L.fgb_rmsd_sort) == want
+    return sort, ol.reference(RMSD_SHAPES[rsize, nparts], ol.digest(arr, part),
+                              lambda: sort(C.CDLL(ol.REF_SO).rmsd_sort))
+
+
+def test_rmsd_sort_seam_matches_reference():
+    _rmsd_compare(9, 37)
+
+
+def test_rmsd_sort_seam_matches_reference_at_12_byte_seeds_and_300_parts():
+    _rmsd_compare(12, 300)
+
+
+def _rmsd_compare(rsize, nparts):
+    from fastga_b200 import load_library
+    sort, want = _rmsd_case(rsize, nparts)
+    assert sort(load_library().fgb_rmsd_sort) == want

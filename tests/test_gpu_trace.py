@@ -8,6 +8,7 @@ import hashlib
 import numpy as np
 import pytest
 
+import edge_cases
 import oracle_lib as ol
 from fastga_b200 import formats, lib, synth
 
@@ -49,14 +50,24 @@ def _check_pair(name, seed, total, ncontig, div, sv, flip=()):
     A, B = synth.make_pair(seed, total, ncontig, div, sv_every=sv)
     for i in flip:                                   # whole contigs on the opposite strand
         B[i] = (3 - B[i][::-1]).astype(np.uint8)
+    return _check_contigs(name, A, B)
+
+
+def reference_scripts(name, A, B):
+    """the reference's script key of every record the path must emit on A, B: the oracle's records,
+    which the e2e tests pin bit-exactly"""
     gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
 
     def run():
-        # the reference on the records the path must emit: the oracle's, which the e2e tests pin bit-exactly
         ralns = ol.oracle_pipeline(gA, gB)["alns"]
         return {_aln_key(ralns, i): _script_key(sc, df)
                 for i, (sc, df) in enumerate(_reference_scripts(gA, gB, ralns))}
-    want = ol.reference("trace_pts/" + name, ol.digest(A, B), run)
+    return ol.reference("trace_pts/" + name, ol.digest(A, B), run)
+
+
+def _check_contigs(name, A, B):
+    want = reference_scripts(name, A, B)
+    gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
     alns, _ = lib.fastga(gA, gB)
     assert len(alns) > 0 and len(alns) == len(want)
     dA, dB = lib.DeviceGenome(gA), lib.DeviceGenome(gB, want_revcomp=True)
@@ -67,17 +78,25 @@ def _check_pair(name, seed, total, ncontig, div, sv, flip=()):
         got = script[soff[i]:soff[i + 1]]
         assert _script_key(got, int(diffs[i])) == want[_aln_key(alns, i)], (i, got[:8], int(diffs[i]))
         ncomp += int(alns.fields[i, 0])
-    return len(alns), ncomp
+    return len(alns), ncomp, alns
 
 
 def test_scripts_match_reference_5pct():
-    n, ncomp = _check_pair("5pct", 21, 3_000_000, 4, 0.05, 60_000)
+    n, ncomp, _ = _check_pair("5pct", 21, 3_000_000, 4, 0.05, 60_000)
     assert n > 10
 
 
 def test_scripts_match_reference_15pct_both_strands():
-    n, ncomp = _check_pair("15pct_both_strands", 22, 2_000_000, 5, 0.15, 30_000, flip=(0, 3))
+    n, ncomp, _ = _check_pair("15pct_both_strands", 22, 2_000_000, 5, 0.15, 30_000, flip=(0, 3))
     assert n > 10 and ncomp > 0
+
+
+def test_scripts_match_reference_past_2_24():
+    """the long_contigs pair of tests/edge_cases.py: alignments at coordinates >= 2^24 on both strands"""
+    A, B, _, _ = edge_cases.long_contigs()
+    n, ncomp, alns = _check_contigs("long_contigs", A, B)
+    past = alns.fields[:, 5] > (1 << 24)
+    assert past.any() and 0 < int(alns.fields[past, 0].sum()) < int(past.sum())
 
 
 def test_inconsistent_trace_points_are_flagged_not_fatal():

@@ -250,3 +250,50 @@ def test_hit_groups_gap_rule_and_triples_without_a_list():
     assert [x[:2] for x in g[0]] == [(0, 2), (2, 1)]
     g, _ = _groups([(0, 3)], [(1, 1)], hits, gap=10**9)
     assert [x[:2] for x in g[0]] == [(0, 3)]
+
+
+import edge_cases  # noqa: E402
+
+
+@pytest.mark.parametrize("name", sorted(edge_cases.REGIMES))
+def test_width_cases_reach_their_regime(name):
+    """every width case of tests/edge_cases.py reaches the record widths it is named for: seed key
+    bits (past 64 the upper fields live in the second word), .ktab post / contig bytes of both
+    genomes, and for the long cases contigs past 2^24"""
+    want = edge_cases.REGIMES[name]
+    A, B, _, _ = edge_cases.CASES[name]()
+    gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
+    anti, band, jc, ic, amx, bmx = ol.seed_layout(gA, gB)
+    assert 12 + anti + band + jc + ic + 1 == want["key"]
+    assert formats.gix_bytes(gA) == want["gixA"] and formats.gix_bytes(gB) == want["gixB"]
+    if "maxlen" in want:
+        assert amx > want["maxlen"] and bmx > want["maxlen"]
+    else:
+        assert max(amx, bmx) < 1 << 24
+    if "ncontigA" in want:
+        assert gA.ncontig == want["ncontigA"]
+
+
+@pytest.mark.parametrize("name", ["seed_key_65", "icont_straddles"])
+def test_seed_fields_that_straddle_bit_64_round_trip_through_the_oracle_records(name):
+    """the oracle's seed records (what the device records are compared with) keep every field at the
+    layout's bit position when the key crosses into the second word: decode each field back from
+    the 128-bit record and compare with the seed it was made from"""
+    A, B, _, _ = edge_cases.CASES[name]()
+    gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
+    _, ra = ol.contig_rank(gA.clen)
+    _, rb = ol.contig_rank(gB.clen)
+    tA, _ = ol.gix_build(gA, ra)
+    tB, sB = ol.gix_build(gB, rb)
+    seeds, _ = ol.merge(tA, tB, sB)
+    layout = ol.seed_layout(gA, gB)
+    recs = ol.seed_records(seeds, layout, sort=False)
+    anti, band, jc, ic = layout[:4]
+    v = [int(lo) | (int(hi) << 64) for lo, hi in recs]
+    field = lambda pos, n: np.array([(x >> pos) & ((1 << n) - 1) for x in v], dtype=np.int64)
+    p_jc = 12 + anti + band
+    assert np.array_equal(field(p_jc, jc), seeds["jcont"])
+    assert np.array_equal(field(p_jc + jc, ic), seeds["icont"])
+    assert np.array_equal(field(p_jc + jc + ic, 1), seeds["comp"])
+    assert np.array_equal(field(0, 6), seeds["plen"])
+    assert (recs[:, 1] != 0).any() and field(p_jc + jc, ic).max() >= 1 << (ic - 1)

@@ -208,6 +208,22 @@ def test_oracle_edge_cases_vs_live_reference(name):
     check(r["alns"], r["nhit"])
 
 
+def test_max_contigs_records_do_not_depend_on_the_filler_tie_order():
+    """the max_contigs fillers have repeated lengths, so their ranks depend on how a sort breaks ties
+    (the reference's and the library's libc qsort, the oracle's stable argsort).  Ties broken the other
+    way round give the reference's records too, which is what lets the case be compared at all."""
+    A, B, _, _ = edge_cases.max_contigs()
+    gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
+    st = edge_cases.reference_run("max_contigs")
+    perm = np.lexsort((-np.arange(gA.ncontig), -gA.clen))          # equal lengths: last index first
+    ra = np.empty(gA.ncontig, np.int32)
+    ra[perm] = np.arange(gA.ncontig)
+    assert not np.array_equal(ra, ol.contig_rank(gA.clen)[1])
+    r = ol.oracle_pipeline(gA, gB, rank=(ra, ol.contig_rank(gB.clen)[1]))
+    assert r["nseeds"] == st["seeds"]
+    assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+
+
 def test_oracle_on_example_regions_vs_live_reference(tmp_path):
     """the EXAMPLE regions fixture of the GPU regression test, oracle against the reference's run"""
     z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "example_regions.npz"))
@@ -260,11 +276,21 @@ def _self_genomes():
         [rng.integers(0, 4, 50_000, dtype=np.uint8)] +
         [synth._small_mutations(rng, unit, 0.04) for _ in range(30)] +
         [rng.integers(0, 4, 50_000, dtype=np.uint8)])]
+    # 300 contigs with a 600 kbp longest: a 67-bit seed key whose icont field straddles bit 64;
+    # every other short contig is a diverged copy of a piece of the long one
+    rng = np.random.default_rng(103)
+    a = rng.integers(0, 4, 600_000, dtype=np.uint8)
+    g = [np.concatenate([a[:540_000], synth.diverged_copy(rng, a[100_000:160_000], 0.05, sv_every=0)])]
+    for k in range(299):
+        n = int(rng.integers(2_000, 6_000))
+        s = int(rng.integers(0, 600_000 - n))
+        g.append(synth._small_mutations(rng, a[s:s + n], 0.05) if k % 2 else rng.integers(0, 4, n, dtype=np.uint8))
+    out["contigs300"] = edge_cases._distinct(g)
     return out
 
 
 @pytest.mark.parametrize("name", ["dup", "tandem61", "tandem62", "inverted_dup", "identical_contigs",
-                                  "palindrome", "near_diagonal_repeats"])
+                                  "palindrome", "near_diagonal_repeats", "contigs300"])
 def test_oracle_self_mode_vs_live_reference(name, tmp_path):
     """SURVEY row a-7 groundwork: the oracle's SELF mode (self block rule, band borders for a contig
     against itself) against `FastGA A` of the reference"""
