@@ -5,14 +5,17 @@
 //   Local_Alignment, forward_wave, reverse_wave align.c:1423-1576, 352-874, 878-1418
 //   Compress_TraceTo8                           align.c:3892
 //
-// Unit of parallel work = one TRIPLE (two adjacent 64-wide diagonal bands of one
-// (strand, A-contig, B-contig) group): inside a triple the reference carries `alast` from chain
-// to chain and the next Local_Alignment starts where the previous ended, so a triple is a
-// sequential program; triples are independent (FastGA.c:3087).  One warp PAIR owns one triple:
-//   * the chain scan is warp-parallel on the front warp (32 merged seeds per step);
+// A TRIPLE is two adjacent 64-wide diagonal bands of one (strand, A-contig, B-contig) group: inside
+// a triple the reference carries `alast` from chain to chain and the next Local_Alignment starts
+// where the previous ended, so a triple is a sequential program; triples are independent
+// (FastGA.c:3087).  Chains are found ahead of the extension (chain_* kernels) and a triple's hit
+// list is cut into hit groups that run as independent work items; the host checks afterwards that
+// the groups really were independent and re-runs a triple in one piece where they were not.
+// Every launch of extend_kernel runs over one ExItem list.  One warp TEAM (front, T, P) runs an item:
+//   * a triple without a hit list is scanned warp-parallel on the front warp (32 merged seeds per step);
 //   * a wave is data-parallel over its diagonals.  While the band fits a warp the state
 //     (V, T, HA, HM, NA) lives in registers of the lane owning the diagonal and the pass is split
-//     between the front warp (V recurrence, snake, band trim) and the back warp (bit-vectors, trim
+//     between the front warp (V recurrence, snake, band trim) and the back warps (bit-vectors, trim
 //     tests, pebbles) through a ring in shared memory (struct PairBox); wider or bordered bands run
 //     on the front warp alone, in 32-diagonal chunks over circular arrays in shared memory / HBM;
 //   * the running maxima besta/lasta/trim* (strict '>' in descending-k order) are reproduced
@@ -61,8 +64,8 @@ typedef unsigned long long u64;
 struct __align__(16) Peb { int ptr, diag, diff, mark; };
 
 struct ChainHit;
-//  Work item of the first launch: hits [h0,h0+hn) of work triple w, whose first hit is number g of
-//  its triple (hn bit 31: no hit list, the triple is scanned in the kernel).
+//  Work item of a launch: hits [h0,h0+hn) of work triple w, whose first hit is number g of its triple
+//  (hn bit 31: no hit list, the triple is scanned in the kernel).  A re-run item is a whole triple (g = 0).
 struct ExItem { unsigned w, h0, hn, g; };
 #define SPEC_SEQ_BITS 14                 // records of a hit group are numbered (g << 14) + 0, 1, ...
 struct ext_params
@@ -70,14 +73,13 @@ struct ext_params
   int p_anti, anti_bits, p_band, band_bits, p_jc, jc_bits, p_ic, ic_bits, p_cp;
   long long amxpos, bmxpos;
   const unsigned *seg_start; int nseg;
-  const unsigned *work; int nwork; unsigned *queue;
-  const unsigned *widx;                                // retry launches: position of work[w] in the first launch's list
-  const ChainHit *hits; const uint2 *hit_range;        // pre-scanned chains of every triple of the first list (NULL: scan here)
-  unsigned *failed_w;                                  // positions (first list) of the triples in failed[]
-  unsigned *need;                                      // bit ST_* set when a triple failed for that reason
-  unsigned long long *wlog;                            // diagnostics (FGB_WLOG): 4 words per work item, or NULL
-  const ExItem *items;                                 // first launch: hit groups (NULL: work[] holds whole triples)
-  long long *galast;                                   //   per item: where the tube stood after its last hit
+  const unsigned *work; int nwork;                     // work triples (long ones first); ExItem::w indexes this
+  const ChainHit *hits;                                // pre-scanned chains of the work triples
+  const ExItem *items; int nitems; unsigned *queue;    // this launch's items and the counter that hands them out
+  int groups;                                          // the items are hit groups: their hits are counted by the host
+  long long *galast;                                   //   and, per item, where the tube stood after its last hit
+  unsigned *failed; unsigned *nfailed;                 // items that overflowed an arena (or their record numbering)
+  unsigned *need;                                      // bit ST_* set when an item failed for that reason
   int attempt;                                         // launch number, stamped on every record
   const u64 *aseq, *arseq; const long long *awoff, *aclen; const int *aperm;
   const u64 *bseq;         const long long *bwoff, *bclen; const int *bperm;
@@ -87,8 +89,7 @@ struct ext_params
   unsigned char *stage; int stage_bytes;               // per warp: 2 x stage_bytes
   unsigned char *out; u64 out_cap; u64 *out_used;
   u64 *counters;                                       // 0 hits 1 LA calls 2 waves 3 cells 4 records
-  unsigned *failed; unsigned *nfailed;                 // triples that overflowed an arena
-  unsigned char *bigstate;                             // wide-band kernel: per-warp wave state in HBM
+  unsigned char *bigstate;                            // wide-band kernel: per-warp wave state in HBM
   int self_mode;                                       // FastGA A: genome against itself (align_contigs :3030)
 };
 
@@ -1378,165 +1379,10 @@ static __device__ void emit_record(const ext_params &P, Ctx &c, const LAres &R, 
     }
 }
 
-//  Walks one triple: chain scan (FastGA.c:3087-3162), tube stepping (:3205-3340).
-//  ALIGN = false: count qualifying chains only (prefilter).
-
-//  Sequential reader over the sorted seeds.  STAGED (warp-uniform callers): a 32-record window
-//  is staged in shared memory with one coalesced 512-byte load, so the serial chain scan sees
-//  shared-memory latency instead of a dependent HBM/L2 round trip per seed.
-
-template<bool STAGED> struct SeedRd
-{ const rec128 *S; rec128 *buf; unsigned base, n;
-  __device__ __forceinline__ void init(const rec128 *s, rec128 *b, unsigned nn)
-    { S = s; buf = b; n = nn; base = 0xffffffffu; }
-  __device__ __forceinline__ rec128 get(unsigned i)
-    { if (!STAGED) return S[i];
-      if (i - base >= 32u)
-        { __syncwarp();
-          base = i;
-          unsigned k = i + (threadIdx.x & 31);
-          if (k < n) st_rec(buf + (threadIdx.x & 31),ld_rec(S + k));
-          __syncwarp();
-        }
-      return buf[i - base];
-    }
-};
-
-template<bool ALIGN>
-static __device__ int scan_triple(const ext_params &P, Ctx &c, unsigned j, unsigned &nhit_out,
-                                  u64 &nla, rec128 *stagebuf)
-{ const rec128 *S = P.seeds;
-  unsigned b = P.seg_start[j], m = P.seg_start[j+1];
-  SeedRd<ALIGN> RL, RU;
-  RL.init(S,stagebuf,(unsigned) P.nseeds);
-  RU.init(S,stagebuf + 32,(unsigned) P.nseeds);
-  rec128 r0 = S[b];
-  u64 grp = get_bits(r0,P.p_jc,P.jc_bits + P.ic_bits + 1);
-  long long cdiag = (long long) get_bits(r0,P.p_band,P.band_bits);
-  bool isnew = true, aux = false;
-  if (j > 0)
-    { rec128 rp = S[P.seg_start[j-1]];
-      if (get_bits(rp,P.p_jc,P.jc_bits + P.ic_bits + 1) == grp &&
-          (long long) get_bits(rp,P.p_band,P.band_bits) == cdiag-1)
-        isnew = false;
-    }
-  unsigned e = m;
-  if (j+1 < (unsigned) P.nseg)
-    { rec128 rn = S[m];
-      if (get_bits(rn,P.p_jc,P.jc_bits + P.ic_bits + 1) == grp &&
-          (long long) get_bits(rn,P.p_band,P.band_bits) == cdiag+1)
-        { aux = true; e = P.seg_start[j+2]; }
-    }
-  nhit_out = 0;
-  if (!isnew && !aux) return ST_OK;
-
-  int comp = (int) get_bits(r0,P.p_cp,1);
-  unsigned pairkey = (unsigned) get_bits(r0,P.p_jc,P.jc_bits + P.ic_bits + 1);
-  long long alen = 0, blen = 0, mlen = 0, doffset = 0, aoffset = 0;
-  if (ALIGN)
-    { int ctg1 = P.aperm[get_bits(r0,P.p_ic,P.ic_bits)];
-      int ctg2 = P.bperm[get_bits(r0,P.p_jc,P.jc_bits)];
-      alen = P.aclen[ctg1]; blen = P.bclen[ctg2]; mlen = alen + blen;
-      doffset = alen - (P.amxpos + P.bmxpos); aoffset = alen - P.amxpos;
-      c.A = (const unsigned *) ((comp ? P.arseq : P.aseq) + P.awoff[ctg1]);
-      c.B = (const unsigned *) (P.bseq + P.bwoff[ctg2]);
-      c.alen = (int) alen; c.blen = (int) blen;
-      c.anw = (alen + 31) >> 5; c.bnw = (blen + 31) >> 5;
-    }
-
-  const long long LMAX = 0x7fffffffffffffffll;
-  long long alast = -1, ahgh, alow, amid, anti, eant, ipost, apost;
-  unsigned s = b, t = m;
-  int go = 1, lcp, wch, mix = 0, cov = 0, dgmin, dgmax, dg, seq = 0;
-
-  ipost = (long long) get_bits(RL.get(s),P.p_anti,P.anti_bits);
-  apost = aux ? (long long) get_bits(RU.get(t),P.p_anti,P.anti_bits) : LMAX;
-  dgmin = 2*BUCK_WIDTH; dgmax = 0;
-  ahgh  = -P.chain_break;
-  alow  = (apost < ipost) ? apost : ipost;
-  while (go)
-    { if (apost < ipost)
-        { rec128 r = RU.get(t);
-          lcp = (int) (r.lo & 63); dg = (int) ((r.lo >> 6) & 63) + BUCK_WIDTH;
-          anti = apost;
-          t += 1;
-          apost = (t >= e) ? LMAX : (long long) get_bits(RU.get(t),P.p_anti,P.anti_bits);
-          wch = 2;
-        }
-      else
-        { if (s < m) { rec128 r = RL.get(s); lcp = (int) (r.lo & 63); dg = (int) ((r.lo >> 6) & 63); }
-          else       { lcp = 0; dg = 0; }
-          anti = ipost;
-          s += 1;
-          if (s >= m) { if (s > m) go = 0; else ipost = LMAX; }
-          else ipost = (long long) get_bits(RL.get(s),P.p_anti,P.anti_bits);
-          wch = 1;
-        }
-      lcp <<= 1;
-
-      if (anti < ahgh + P.chain_break)
-        { long long cps = anti + lcp;
-          if (cps > ahgh)
-            { if (anti >= ahgh) cov += lcp; else cov += (int) (cps - ahgh);
-              ahgh = cps;
-            }
-          mix |= wch;
-          if (dg < dgmin) dgmin = dg; else if (dg > dgmax) dgmax = dg;
-        }
-      else
-        { if (cov >= P.chain_min && (mix != 1 || isnew))
-            { nhit_out += 1;
-              if (ALIGN)
-                { dgmin += (int) (cdiag << BUCK_SHIFT);
-                  dgmax += (int) (cdiag << BUCK_SHIFT);
-                  if (comp)
-                    { dgmin += (int) doffset; dgmax += (int) doffset; alow += aoffset; ahgh += aoffset; }
-                  else
-                    { dgmin -= (int) P.bmxpos; dgmax -= (int) P.bmxpos; }
-                  if (ahgh > alast)
-                    { if (alow < alast) alow = alast;
-                      ahgh -= BUCK_ANTI;
-                      do
-                        { amid = alow + BUCK_ANTI;
-                          if (amid > ahgh)
-                            { amid = ahgh;
-                              if (amid + dgmin < 0)
-                                { dgmin = (int) -amid;
-                                  if (dgmin > dgmax) break;
-                                }
-                            }
-                          LAres R;
-                          int st = local_alignment<EX_W>(c,comp,dgmin,dgmax,(int) amid,R);
-                          if (st) return st;
-                          nla += 1;
-                          int ab = R.abpos, bb = R.bbpos, ae = R.aepos, be = R.bepos;
-                          int rlen = ae - ab;              // same after the ACOMP flip
-                          if (rlen >= P.aln_min && P.aln_rate*rlen >= (double) R.diffs)
-                            { emit_record(P,c,R,comp,j,seq,pairkey);
-                              seq += 1;
-                            }
-                          //  eant in the flipped frame (FastGA.c:3309-3312) == un-flipped end
-                          if (comp) eant = mlen - ((alen - ae) + (blen - be));
-                          else      eant = (long long) ae + be;
-                          (void) ab; (void) bb;
-                          if (eant <= alow) alow = amid; else alow = eant;
-                        }
-                      while (alow < ahgh);
-                      alast = alow;
-                    }
-                }
-            }
-          if (go)
-            { cov = lcp; ahgh = anti + lcp; mix = wch; alow = anti; dgmin = dgmax = dg; }
-        }
-    }
-  return ST_OK;
-}
-
 /***********************************************************************************************
- *  Warp-parallel chain scan of one triple (the extension stage's version of the loop above).
+ *  Warp-parallel chain scan of one triple.
  *
- *  The serial scan keeps ahgh = running maximum of anti+2*lcp over the current chain and breaks
+ *  The serial scan (FastGA.c:3087-3162, serial_has_chain below) keeps ahgh = running maximum of anti+2*lcp over the current chain and breaks
  *  the chain when anti >= ahgh + CHAIN_BREAK.  Because seeds arrive in anti order and one seed
  *  spans at most 80 anti-diagonals, every seed of an earlier chain ends more than CHAIN_BREAK-80
  *  below the current one, so the chain-local running maximum equals the running maximum over
@@ -1827,9 +1673,6 @@ static __device__ int scan_triple_warp(const ext_params &P, Ctx &c, unsigned j, 
 
 #define CH_SEEDS 1024            // seeds per chunk (both bands), x1.5
 #define CH_HCAP  48              // hits recorded per chunk (more: the triple is scanned in extend_kernel)
-#ifndef CH_TOPK
-#define CH_TOPK  (1 << 30)             // only the largest triples are pre-scanned: theirs is the scan that sits on the kernel's
-#endif                           //   critical path; the others are scanned inside extend_kernel, which has idle warps to spare
 
 struct ChainHit { long long alow, ahgh; int dgmin, dgmax; };
 
@@ -1956,21 +1799,21 @@ chain_chunk_kernel(ext_params P, const ChunkPlan *__restrict__ plan, int nplan, 
 __global__ void chain_stitch_kernel(ext_params P, const ChunkPlan *__restrict__ plan, const ChunkOut *__restrict__ outs,
                                     const unsigned *__restrict__ first_chunk, int ntrip, ChainHit *__restrict__ hits,
                                     unsigned long long *__restrict__ hit_used, unsigned long long hit_cap,
-                                    uint2 *__restrict__ hit_range /* start, count | 0x80000000: scan in extend_kernel */,
+                                    uint2 *__restrict__ hrange /* start, count | 0x80000000: scan in extend_kernel */,
                                     int2 *__restrict__ tinfo /* (strand, contig pair) key and band of the triple */)
 { int w = blockIdx.x * blockDim.x + threadIdx.x;
   if (w >= ntrip) return;
   tinfo[w] = make_int2(-1,0);
   const unsigned c0 = first_chunk[w], c1 = first_chunk[w+1];
   TripleCtx T; unsigned b, m, e;
-  if (c1 == c0) { hit_range[w] = make_uint2(0u,0x80000000u); return; }          // not pre-scanned
-  if (!triple_setup(P,plan[c0].j,T,b,m,e)) { hit_range[w] = make_uint2(0u,0u); return; }
+  if (c1 == c0) { hrange[w] = make_uint2(0u,0x80000000u); return; }          // not pre-scanned
+  if (!triple_setup(P,plan[c0].j,T,b,m,e)) { hrange[w] = make_uint2(0u,0u); return; }
   tinfo[w] = make_int2((int) T.pairkey,(int) T.cdiag);
   unsigned long long total = 0; bool over = false;
   for (unsigned k = c0; k < c1; k++) { total += (unsigned long long) outs[k].nhit + 1; over |= (outs[k].over != 0); }
   total += 1;
   unsigned long long base = atomicAdd(hit_used,total);
-  if (over || base + total > hit_cap) { hit_range[w] = make_uint2(0u,0x80000000u); return; }
+  if (over || base + total > hit_cap) { hrange[w] = make_uint2(0u,0x80000000u); return; }
   ChainHit *H = hits + base;
   unsigned n = 0;
   bool open = false; long long o_alow = 0; int o_cov = 0, o_mix = 0, o_dmin = 2*BUCK_WIDTH, o_dmax = 0;
@@ -1996,7 +1839,7 @@ __global__ void chain_stitch_kernel(ext_params P, const ChunkPlan *__restrict__ 
     }
   CH_EMIT(last_carry);                                             // the scan's final iteration closes the last chain
 #undef CH_EMIT
-  hit_range[w] = make_uint2((unsigned) base,n);
+  hrange[w] = make_uint2((unsigned) base,n);
 }
 
 //  extend_kernel's side: the tube stepping of every pre-scanned chain of a triple, in order
@@ -2063,41 +1906,61 @@ __global__ void seg_fill2_kernel(const rec128 *__restrict__ seeds, long long n, 
 
 #define PREF_LONG 64
 
+//  The serial chain scan of a triple set up by triple_setup (FastGA.c:3087-3162), up to its first
+//  qualifying chain: does the triple hold one?
+static __device__ bool serial_has_chain(const ext_params &P, const TripleCtx &T, unsigned b, unsigned m, unsigned e)
+{ const rec128 *S = P.seeds;
+  const long long LMAX = 0x7fffffffffffffffll;
+  long long ahgh = -P.chain_break, anti;
+  long long ipost = (long long) get_bits(S[b],P.p_anti,P.anti_bits);
+  long long apost = (e > m) ? (long long) get_bits(S[m],P.p_anti,P.anti_bits) : LMAX;
+  unsigned s = b, t = m;
+  int go = 1, lcp, wch, mix = 0, cov = 0;
+  while (go)
+    { if (apost < ipost)
+        { lcp = (int) (S[t].lo & 63);
+          anti = apost;
+          t += 1;
+          apost = (t >= e) ? LMAX : (long long) get_bits(S[t],P.p_anti,P.anti_bits);
+          wch = 2;
+        }
+      else
+        { lcp = (s < m) ? (int) (S[s].lo & 63) : 0;
+          anti = ipost;
+          s += 1;
+          if (s >= m) { if (s > m) go = 0; else ipost = LMAX; }
+          else ipost = (long long) get_bits(S[s],P.p_anti,P.anti_bits);
+          wch = 1;
+        }
+      lcp <<= 1;
+      if (anti < ahgh + P.chain_break)
+        { long long cps = anti + lcp;
+          if (cps > ahgh)
+            { if (anti >= ahgh) cov += lcp; else cov += (int) (cps - ahgh);
+              ahgh = cps;
+            }
+          mix |= wch;
+        }
+      else
+        { if (cov >= P.chain_min && (mix != 1 || T.isnew)) return true;
+          cov = lcp; ahgh = anti + lcp; mix = wch;
+        }
+    }
+  return false;
+}
+
 __global__ void prefilter_kernel(ext_params P, unsigned *__restrict__ work_long, unsigned *__restrict__ work_short,
                                  unsigned *__restrict__ nwork /* [0] long [1] short */,
                                  unsigned *__restrict__ long_size)
 { unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
   if (j >= (unsigned) P.nseg) return;
-  const rec128 *S = P.seeds;
-  unsigned b = P.seg_start[j], m = P.seg_start[j+1], e = m;
-  unsigned minseeds = (unsigned) ((P.chain_min + 79) / 80);
-  rec128 r0 = S[b];
-  u64 grp = get_bits(r0,P.p_jc,P.jc_bits + P.ic_bits + 1);
-  long long cdiag = (long long) get_bits(r0,P.p_band,P.band_bits);
-  if (j+1 < (unsigned) P.nseg)
-    { rec128 rn = S[m];
-      if (get_bits(rn,P.p_jc,P.jc_bits + P.ic_bits + 1) == grp &&
-          (long long) get_bits(rn,P.p_band,P.band_bits) == cdiag+1)
-        e = P.seg_start[j+2];
-    }
-  if (e - b < minseeds) return;
+  TripleCtx T; unsigned b, m, e;
+  if (!triple_setup(P,j,T,b,m,e) || e - b < (unsigned) ((P.chain_min + 79) / 80)) return;
   if (e - b > PREF_LONG)
-    { bool isnew = true;
-      if (j > 0)
-        { rec128 rp = S[P.seg_start[j-1]];
-          if (get_bits(rp,P.p_jc,P.jc_bits + P.ic_bits + 1) == grp &&
-              (long long) get_bits(rp,P.p_band,P.band_bits) == cdiag-1)
-            isnew = false;
-        }
-      if (isnew || e != m)
-        { unsigned o = atomicAdd(nwork,1u);
-          work_long[o] = j; long_size[o] = e - b;
-        }
-      return;
+    { unsigned o = atomicAdd(nwork,1u);
+      work_long[o] = j; long_size[o] = e - b;
     }
-  Ctx c; u64 nla = 0; unsigned nh = 0;
-  scan_triple<false>(P,c,j,nh,nla,NULL);
-  if (nh > 0)
+  else if (serial_has_chain(P,T,b,m,e))
     work_short[atomicAdd(nwork+1,1u)] = j;
 }
 
@@ -2108,6 +1971,32 @@ __global__ void prefilter_kernel(ext_params P, unsigned *__restrict__ work_long,
 #define EX_NFRONT   (EX_PAIR ? EX_WARPS/EX_TEAM : EX_WARPS)  // warps of a block that take triples
 #define BOX_BYTES   (EX_PAIR ? (EX_WARPS/EX_TEAM)*((int) sizeof(PairBox)) : 0)
 
+//  The Ctx of warp wp (global number gw) in both kernels: wave state in shared memory (W = EX_W) or HBM,
+//  the warp's arenas, the scoring tables, no mailbox, and a 64-pebble read-out window in the warp's scan
+//  buffer (returned: SCAN_SMEM bytes of shared memory)
+template<int W>
+static __device__ __forceinline__ unsigned char *ctx_init(Ctx &c, const ext_params &P, int wp, long long gw)
+{ unsigned char *sb = (W == EX_W) ? (ex_smem + (size_t) wp * STATE_BYTES)
+                                  : (P.bigstate + (size_t) gw * WSTATE_BYTES(EX_WBIG));
+  unsigned char *scan = (W == EX_W) ? (sb + WSTATE_BYTES(EX_W)) : (ex_smem + (size_t) wp * BIG_SMEM_PER_WARP);
+  c.T  = (u64 *) sb;
+  c.V  = (int *) (sb + W*8);
+  c.HA = c.V + W; c.HM = c.HA + W; c.NA = c.HM + W;
+  c.carry = c.NA + W;
+  c.pwin = (Peb *) scan; c.pwin_n = 64;
+  c.ttab = P.table; c.sc15 = TRIM_LEN * P.dscore;
+  c.box = NULL; c.box_off = 0;
+  c.cells = P.cells + gw * P.cells_per_warp;
+  c.cmax  = (int) P.cells_per_warp;
+  c.avail = 0;
+  c.fstage = P.stage + gw * 2ll * P.stage_bytes;
+  c.rstage = c.fstage + P.stage_bytes;
+  c.smax = P.stage_bytes;
+  c.tspace = P.tspace; c.path_ave = P.path_ave; c.score = P.score; c.table = P.table;
+  c.nwaves = 0; c.ncells = 0; c.cyc_wave = 0; c.cyc_extract = 0; c.pwaves = 0; c.npairs = 0; c.fwait = 0; c.ftot = 0; c.bwait = 0; c.btot = 0;
+  return scan;
+}
+
 template<int W>
 __global__ void __launch_bounds__(EX_WARPS*32,EX_MINBLK)
 extend_kernel(ext_params P)
@@ -2115,23 +2004,15 @@ extend_kernel(ext_params P)
   const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
   const long long gw = (long long) blockIdx.x * EX_WARPS + wp;
   const size_t per_warp = (W == EX_W) ? STATE_BYTES : BIG_SMEM_PER_WARP;
-  unsigned char *sb = (W == EX_W) ? (smem + (size_t) wp * STATE_BYTES)
-                                  : (P.bigstate + (size_t) gw * WSTATE_BYTES(EX_WBIG));
   Ctx c;
-  c.T  = (u64 *) sb;
-  c.V  = (int *) (sb + W*8);
-  c.HA = c.V + W; c.HM = c.HA + W; c.NA = c.HM + W;
-  c.carry = c.NA + W;
-  rec128 *stagebuf = (W == EX_W) ? (rec128 *) (sb + WSTATE_BYTES(EX_W))
-                                 : (rec128 *) (smem + (size_t) wp * BIG_SMEM_PER_WARP);
-  c.ttab = P.table; c.sc15 = TRIM_LEN * P.dscore;
+  unsigned char *const scanbuf = ctx_init<W>(c,P,wp,gw);
   //  read-out window: the state slot of the team's T warp (T and P keep their state in registers; the
-  //  front warp's own scan buffer is live while a triple scanned here calls into an alignment)
-  c.pwin = EX_PAIR ? (Peb *) (smem + (size_t) (wp + 1) * per_warp) : (Peb *) stagebuf;
-  c.pwin_n = (EX_PAIR && W == EX_W) ? 256 : 64;
-  c.box = NULL; c.box_off = 0;
+  //  front warp's own scan buffer is live while a triple scanned here calls into an alignment), and the
+  //  team's mailbox
   if (EX_PAIR)
-    { c.box_off = (unsigned) ((size_t) EX_WARPS * per_warp + (size_t) (wp / EX_TEAM) * sizeof(PairBox));
+    { c.pwin = (Peb *) (smem + (size_t) (wp + 1) * per_warp);
+      if (W == EX_W) c.pwin_n = 256;
+      c.box_off = (unsigned) ((size_t) EX_WARPS * per_warp + (size_t) (wp / EX_TEAM) * sizeof(PairBox));
       c.box = (PairBox *) (smem + c.box_off);
       if ((wp % EX_TEAM) == 0 && lane == 0) { c.box->seq = 0; c.box->cmd = 0; c.box->stop = 0; c.box->stopp = 0; }
     }
@@ -2154,52 +2035,29 @@ extend_kernel(ext_params P)
       return;
     }
   long long t_start = clock64();
-  c.cells = P.cells + gw * P.cells_per_warp;
-  c.cmax  = (int) P.cells_per_warp;
-  c.avail = 0;
-  c.fstage = P.stage + gw * 2ll * P.stage_bytes;
-  c.rstage = c.fstage + P.stage_bytes;
-  c.smax = P.stage_bytes;
-  c.tspace = P.tspace; c.path_ave = P.path_ave; c.score = P.score; c.table = P.table;
-  c.nwaves = 0; c.ncells = 0; c.cyc_wave = 0; c.cyc_extract = 0; c.pwaves = 0; c.npairs = 0; c.fwait = 0; c.ftot = 0; c.bwait = 0; c.btot = 0;
   u64 nla = 0, nhits = 0;
 
   while (true)
     { unsigned w = 0;
       if (lane == 0) w = atomicAdd(P.queue,1u);
       w = __shfl_sync(FULL,w,0);
-      if (w >= (unsigned) P.nwork) break;
-      unsigned j, w0, nh = 0;
-      uint2 hr = make_uint2(0u,0x80000000u);
-      unsigned grp = 0; bool spec = false;
-      if (P.items != NULL)
-        { const ExItem it = P.items[w];
-          w0 = it.w; j = P.work[w0]; hr = make_uint2(it.h0,it.hn); grp = it.g; spec = true;
-        }
-      else
-        { j = P.work[w];
-          w0 = P.widx ? P.widx[w] : w;
-          if (P.hit_range != NULL) hr = P.hit_range[w0];
-        }
-      const u64 lg_w = c.nwaves, lg_l = nla; const long long lg_t = clock64();
+      if (w >= (unsigned) P.nitems) break;
+      const ExItem it = P.items[w];
+      const unsigned j = P.work[it.w];
+      const bool scan = (it.hn & 0x80000000u) != 0;
+      unsigned nh = 0;
       int st; long long alast_out = -0x7fffffffffffffffll;
-      if (hr.y & 0x80000000u) st = scan_triple_warp<W>(P,c,j,nh,nla,(unsigned char *) stagebuf);
-      else                    st = run_hits<W>(P,c,j,P.hits + hr.x,hr.y,nh,nla,grp,spec,alast_out);
-      if (P.items != NULL && lane == 0) P.galast[w] = alast_out;
+      if (scan) st = scan_triple_warp<W>(P,c,j,nh,nla,scanbuf);
+      else      st = run_hits<W>(P,c,j,P.hits + it.h0,it.hn,nh,nla,it.g,P.groups != 0,alast_out);
+      if (P.groups && lane == 0) P.galast[w] = alast_out;
       if (st != ST_OK)
         { if (lane == 0)
-            { unsigned o = atomicAdd(P.nfailed,1u);
-              P.failed[o] = j; P.failed_w[o] = w0;
+            { P.failed[atomicAdd(P.nfailed,1u)] = w;
               atomicOr(P.need,1u << st);
             }
         }
-      else if (!spec || (hr.y & 0x80000000u))
+      else if (!P.groups || scan)
         nhits += nh;                                                // (hit groups are counted by the host)
-      if (P.wlog != NULL && lane == 0)
-        { unsigned long long *L = P.wlog + 4ull*w;
-          L[0] = ((u64) gw << 32) | j; L[1] = ((c.nwaves - lg_w) << 24) | ((nla - lg_l) << 8) | (u64) (st & 0xff);
-          L[2] = (u64) (lg_t - t_start); L[3] = (u64) (clock64() - t_start);
-        }
       __syncwarp();
     }
   if (EX_PAIR && lane == 0)
@@ -2243,28 +2101,9 @@ template<int W>
 __global__ void __launch_bounds__(EX_WARPS*32,EX_MINBLK)
 la_batch_kernel(ext_params P, const la_job *__restrict__ jobs, const unsigned *__restrict__ idx, int njobs,
                 int *__restrict__ status)
-{ unsigned char *const smem = ex_smem;
-  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
-  const long long gw = (long long) blockIdx.x * EX_WARPS + wp;
-  unsigned char *sb = (W == EX_W) ? (smem + (size_t) wp * STATE_BYTES)
-                                  : (P.bigstate + (size_t) gw * WSTATE_BYTES(EX_WBIG));
+{ const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
   Ctx c;
-  c.T  = (u64 *) sb;
-  c.V  = (int *) (sb + W*8);
-  c.HA = c.V + W; c.HM = c.HA + W; c.NA = c.HM + W;
-  c.carry = c.NA + W;
-  c.pwin = (W == EX_W) ? (Peb *) (sb + WSTATE_BYTES(EX_W)) : (Peb *) (smem + (size_t) wp * BIG_SMEM_PER_WARP);
-  c.pwin_n = 64;
-  c.ttab = P.table; c.sc15 = TRIM_LEN * P.dscore;
-  c.box = NULL; c.box_off = 0;
-  c.cells = P.cells + gw * P.cells_per_warp;
-  c.cmax  = (int) P.cells_per_warp;
-  c.avail = 0;
-  c.fstage = P.stage + gw * 2ll * P.stage_bytes;
-  c.rstage = c.fstage + P.stage_bytes;
-  c.smax = P.stage_bytes;
-  c.tspace = P.tspace; c.path_ave = P.path_ave; c.score = P.score; c.table = P.table;
-  c.nwaves = 0; c.ncells = 0; c.cyc_wave = 0; c.cyc_extract = 0; c.pwaves = 0; c.npairs = 0; c.fwait = 0; c.ftot = 0; c.bwait = 0; c.btot = 0;
+  ctx_init<W>(c,P,wp,(long long) blockIdx.x * EX_WARPS + wp);
   while (true)
     { unsigned w = 0;
       if (lane == 0) w = atomicAdd(P.queue,1u);
@@ -2305,22 +2144,6 @@ extern "C" void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long 
   out[5] = (unsigned long long) o->nseg; out[6] = (unsigned long long) o->nwork;
 }
 
-
-#include <chrono>
-static long long tr_t0 = 0;
-static void tr_mark(const char *what)
-{ static int on = -1;
-  if (on < 0) on = (getenv("FGB_TRACE") != NULL);
-  if (!on) return;
-  long long t = std::chrono::duration_cast<std::chrono::microseconds>(
-                  std::chrono::steady_clock::now().time_since_epoch()).count();
-  fprintf(stderr,"[fgb_trace] %-28s +%8.3f ms\n",what,tr_t0 ? (t - tr_t0)/1000.0 : 0.0);
-  tr_t0 = t;
-}
-
-static bool tr_on() { static int on = -1; if (on < 0) on = (getenv("FGB_TRACE") != NULL); return on != 0; }
-#define TR_SYNC(what) do { if (tr_on()) { cudaStreamSynchronize(st); tr_mark(what); } } while (0)
-
 struct ev_timer
 { cudaEvent_t a, b; cudaStream_t st; int which;
   ev_timer(int w, cudaStream_t s) : st(s), which(w)
@@ -2335,9 +2158,18 @@ struct ev_timer
 //  tables: 2 x 32768 int16 (score, then table) and ave_path from New_Align_Spec's arithmetic,
 //  computed by the host caller (align.c:222-268 is float/double set-up, kept on the host).
 
-//  Hit groups of the work triples (host): see the comment in fgb_extend.  hrange[w] = (first hit, count |
-//  bit 31: no list) into hh[0..hused); tinfo[w] = ((strand, contig pair) key, band); items come out in launch
-//  order (largest estimated cost first) with, for each, the first hit of the next group of its triple.
+//  Hit groups of the work triples (host).  Inside a triple a hit is clipped or skipped by the end of the
+//  alignments before it (alast, FastGA.c:3262-3318), which chains its hits serially.  In practice a hit is
+//  only ever touched by an alignment of ITS aligned block: the block's seed chains in this band pair and
+//  in the neighbouring ones, overlapping end to end while the path drifts across bands.  Chains of one
+//  (strand, contig pair) within SPEC_BANDS bands whose anti-diagonal intervals (+- SPEC_SLACK) overlap
+//  are joined into components (union-find); a triple's hit list is cut wherever the components before
+//  and after the cut are disjoint.  Every group is a work item of its own that starts with a clear tube;
+//  after the launch the host checks that no group's tube reached the next group's first hit -- else the
+//  triple is re-run in one piece (extend_launches), so a wrong guess costs time, never the result.
+//  hrange[w] = (first hit, count | bit 31: no list) into hh[0..hused); tinfo[w] = ((strand, contig pair)
+//  key, band); items come out in launch order (largest estimated cost first) with, for each, the first
+//  hit of the next group of its triple.
 static void build_hit_groups(unsigned nwork, const uint2 *hrange, const int2 *tinfo, const ChainHit *hh,
                              unsigned long long hused, int SPEC_BANDS, long long SPEC_SLACK, long long SPEC_GAP,
                              std::vector<ExItem> &items, std::vector<long long> &nxt_alow,
@@ -2466,6 +2298,344 @@ static cudaError_t pinned_staging(size_t bytes, unsigned char **buf)
   return cudaSuccess;
 }
 
+//  Blocks of a launch over n work items, per_block items a block: at most `limit`, and no more than keep
+//  the launch's pebble arenas within 24 GB
+static long long launch_blocks(long long n, int per_block, long long limit, long long cells_per_warp)
+{ long long nb = (n + per_block - 1) / per_block;
+  const long long maxb = (24ll << 30) / ((long long) sizeof(Peb) * cells_per_warp * EX_WARPS);
+  if (nb > limit) nb = limit;
+  if (nb > maxb) nb = maxb;
+  return nb < 1 ? 1 : nb;
+}
+
+//  The per-warp arenas of a launch on nwarps warps: pebbles, trace staging and, for the wide-band
+//  kernels, the wave state in HBM.  alloc() points P at them.
+struct Arenas
+{ dblock<Peb> cells; dblock<unsigned char> stage, big;
+  cudaError_t alloc(ext_params &P, long long nwarps, long long cells_per_warp, int stage_bytes, bool wide,
+                    cudaStream_t st)
+  { reset();
+    cudaError_t e = cells.alloc(cells_per_warp*nwarps,st);
+    if (e == cudaSuccess) e = stage.alloc(2ll*stage_bytes*nwarps,st);
+    if (e == cudaSuccess && wide) e = big.alloc((size_t) nwarps * WSTATE_BYTES(EX_WBIG),st);
+    P.cells = cells; P.cells_per_warp = cells_per_warp;
+    P.stage = stage; P.stage_bytes = stage_bytes;
+    P.bigstate = big;
+    return e;
+  }
+  void reset() { cells.reset(); stage.reset(); big.reset(); }
+};
+
+//  What fgb_extend plans for extend_kernel.  Per work triple w: hrange[w] = its hit list (first hit,
+//  count | bit 31: no list, the kernel scans the triple) into hh[0..hused), tinfo[w] = ((strand, contig
+//  pair) key, band); both empty when chain detection did not run.  The items of the first launch; when
+//  they are hit groups, for each the first hit of the next group of its triple, and the hits per triple.
+struct ExtendPlan
+{ std::vector<uint2> hrange; std::vector<int2> tinfo;
+  std::vector<ChainHit> hh; unsigned long long hused = 0;
+  std::vector<ExItem> items; bool groups = false;
+  std::vector<long long> nxt_alow, nxt_ahgh; std::vector<unsigned> hcount;
+};
+
+//  What the launches leave for the read-out
+struct ExtendOut
+{ dblock<unsigned char> buf; u64 cap = 0, used = 0;        // the records, as the device packed them
+  std::vector<std::pair<unsigned,int> > rerun;            // (triple, launch number) of every re-run
+  unsigned long long hits_done = 0;                       // hits of the hit groups, counted by the host
+};
+
+//  Phase 1: the band segments of the sorted seeds (P.seg_start, P.nseg), the prefilter, and the work
+//  triples (P.work, P.nwork): long ones first, largest first (the kernel's makespan is its longest
+//  triple, so it must not start late), then the short ones that hold a chain.  wsize gets the seed
+//  counts of the long triples in work order; it stays empty when there are none, or too many to sort.
+static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, dblock<unsigned> &d_seg,
+                          dblock<unsigned> &d_work, std::vector<unsigned> &wsize, cudaStream_t st)
+{ const long long n = S->n, tmpb = fgb_dev_scan_tmp_bytes(n);
+  dblock<u64> d_total; dblock<unsigned> d_flag; dblock<unsigned char> d_tmp;
+  CUDA_TRY(d_total.alloc(1,st));
+  CUDA_TRY(d_flag.alloc(n+1,st));
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
+  seg_flag_kernel<<<(int) ((n + 255) / 256),256,0,st>>>(S->d_rec,n,P.p_band,d_flag);
+  int rc = fgb_dev_exclusive_scan_u32(d_flag,n,d_total,d_tmp,tmpb,st);
+  if (rc) return rc;
+  u64 tot = 0;
+  CUDA_TRY(cudaMemcpyAsync(&tot,d_total,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  const unsigned nseg = (unsigned) tot;
+  CUDA_TRY(d_seg.alloc(nseg+2,st));
+  CUDA_TRY(d_work.alloc(3ll*nseg+3,st));
+  seg_fill2_kernel<<<(int) ((n + 1 + 255) / 256),256,0,st>>>(S->d_rec,n,P.p_band,d_flag,d_seg,nseg);
+  P.seg_start = d_seg; P.nseg = (int) nseg;
+  prefilter_kernel<<<(nseg + 127)/128,128,0,st>>>(P,d_work,d_work + nseg + 1,d_misc + 6,d_work + 2ll*nseg + 2);
+  fgb_count_launch(3);
+  CUDA_TRY(cudaGetLastError());
+  unsigned nw2[2];
+  CUDA_TRY(cudaMemcpyAsync(nw2,d_misc + 6,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  if (nw2[0] >= 1 && nw2[0] <= (1u << 20))
+    { std::vector<unsigned> lj(nw2[0]), ls(nw2[0]), ord(nw2[0]);
+      CUDA_TRY(cudaMemcpyAsync(lj.data(),d_work,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaMemcpyAsync(ls.data(),d_work + 2ll*nseg + 2,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      for (unsigned q = 0; q < nw2[0]; q++) ord[q] = q;
+      std::sort(ord.begin(),ord.end(),[&](unsigned a, unsigned b)
+                { return ls[a] != ls[b] ? ls[a] > ls[b] : lj[a] < lj[b]; });
+      std::vector<unsigned> sj(nw2[0]);
+      wsize.resize(nw2[0]);
+      for (unsigned q = 0; q < nw2[0]; q++) { sj[q] = lj[ord[q]]; wsize[q] = ls[ord[q]]; }
+      CUDA_TRY(cudaMemcpyAsync(d_work,sj.data(),4ull*nw2[0],cudaMemcpyHostToDevice,st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+    }
+  CUDA_TRY(cudaMemcpyAsync(d_work + nw2[0],d_work + nseg + 1,sizeof(unsigned)*nw2[1],
+                           cudaMemcpyDeviceToDevice,st));
+  P.work = d_work; P.nwork = (int) (nw2[0] + nw2[1]);
+  return FGB_OK;
+}
+
+//  Phase 2: chain detection of the long work triples, chunk-parallel (chain_plan / chain_chunk /
+//  chain_stitch; the short ones are scanned in extend_kernel).  The hit lists stay in d_hits for the
+//  kernel and come to the host (X.hrange, X.tinfo, X.hh) in one staged download.
+static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize, unsigned *d_misc,
+                        dblock<ChainHit> &d_hits, ExtendPlan &X, cudaStream_t st)
+{ const unsigned nwork = (unsigned) P.nwork;
+  std::vector<ChunkPlan> plan;
+  std::vector<unsigned> first(nwork + 1);
+  for (unsigned w = 0; w < nwork; w++)
+    { unsigned nch = 0;
+      if (w < wsize.size())
+        { nch = (unsigned) (((unsigned long long) wsize[w] + CH_SEEDS + CH_SEEDS/2 - 1) / (CH_SEEDS + CH_SEEDS/2));
+          if (nch < 1) nch = 1;
+        }
+      first[w] = (unsigned) plan.size();
+      for (unsigned k = 0; k < nch; k++)
+        { ChunkPlan c; c.w = w; c.j = 0; c.k = k; c.nch = nch; c.sL = c.sU = 0; plan.push_back(c); }
+    }
+  first[nwork] = (unsigned) plan.size();
+  const int nplan = (int) plan.size();
+  const unsigned long long hit_cap = (unsigned long long) nplan * (CH_HCAP + 1) + nwork + 16;
+  dblock<ChunkPlan> d_plan; dblock<ChunkOut> d_couts; dblock<unsigned> d_first;
+  dblock<uint2> d_hrange; dblock<int2> d_tinfo;
+  CUDA_TRY(d_plan.alloc((size_t) nplan,st));
+  CUDA_TRY(d_couts.alloc((size_t) nplan,st));
+  CUDA_TRY(d_first.alloc((size_t) (nwork + 1),st));
+  CUDA_TRY(d_hits.alloc((size_t) hit_cap,st));
+  CUDA_TRY(d_hrange.alloc((size_t) nwork,st));
+  CUDA_TRY(d_tinfo.alloc((size_t) nwork,st));
+  CUDA_TRY(cudaMemcpyAsync(d_plan,plan.data(),sizeof(ChunkPlan)*(size_t) nplan,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(d_first,first.data(),sizeof(unsigned)*(size_t) (nwork + 1),cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemsetAsync(d_misc + 8,0,8,st));
+  chain_plan_kernel<<<(nplan + 127)/128,128,0,st>>>(P,d_plan,nplan);
+  chain_chunk_kernel<<<(nplan + 3)/4,128,0,st>>>(P,d_plan,nplan,d_couts);
+  chain_stitch_kernel<<<(nwork + 127)/128,128,0,st>>>(P,d_plan,d_couts,d_first,(int) nwork,d_hits,
+                                                     (unsigned long long *) (d_misc + 8),hit_cap,d_hrange,d_tinfo);
+  fgb_count_launch(3);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaStreamSynchronize(st));                 // plan / first are host vectors
+  //  the small result arrays come back through the pinned staging buffer: three copies in flight and
+  //  one synchronisation instead of a staged, synchronous copy each
+  X.hrange.resize(nwork); X.tinfo.resize(nwork);
+  { const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork;
+    unsigned char *hp;
+    CUDA_TRY(pinned_staging(o3,&hp));
+    CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
+    CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
+    CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    memcpy(&X.hused,hp,8);
+    memcpy(X.hrange.data(),hp + o1,sizeof(uint2)*(size_t) nwork);
+    memcpy(X.tinfo.data(),hp + o2,sizeof(int2)*(size_t) nwork);
+  }
+  if (X.hused > hit_cap) X.hused = hit_cap;
+  X.hh.resize((size_t) X.hused + 1);
+  if (X.hused > 0)
+    { unsigned char *hp;
+      CUDA_TRY(pinned_staging(sizeof(ChainHit)*(size_t) X.hused,&hp));
+      CUDA_TRY(cudaMemcpyAsync(hp,d_hits,sizeof(ChainHit)*(size_t) X.hused,cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      memcpy(X.hh.data(),hp,sizeof(ChainHit)*(size_t) X.hused);
+    }
+  return FGB_OK;
+}
+
+//  Phase 3: the items of the first launch.  With hit lists, the hit groups of build_hit_groups
+//  (FGB_SPEC_BANDS / FGB_SPEC_SLACK move its joins; FGB_SPEC_GAP >= 0 cuts at every gap of at least that
+//  instead, which tests use to force re-runs); without, one item per work triple, scanned in the kernel.
+static void first_items(unsigned nwork, ExtendPlan &X)
+{ if (X.hrange.empty())
+    { X.items.resize(nwork);
+      for (unsigned w = 0; w < nwork; w++) X.items[w] = { w, 0u, 0x80000000u, 0u };
+      return;
+    }
+  int SPEC_BANDS = 1; long long SPEC_SLACK = 1000, SPEC_GAP = -1;
+  if (getenv("FGB_SPEC_BANDS") != NULL) SPEC_BANDS = atoi(getenv("FGB_SPEC_BANDS"));
+  if (getenv("FGB_SPEC_SLACK") != NULL) SPEC_SLACK = atoll(getenv("FGB_SPEC_SLACK"));
+  if (getenv("FGB_SPEC_GAP") != NULL) SPEC_GAP = atoll(getenv("FGB_SPEC_GAP"));
+  build_hit_groups(nwork,X.hrange.data(),X.tinfo.data(),X.hh.data(),X.hused,SPEC_BANDS,SPEC_SLACK,SPEC_GAP,
+                   X.items,X.nxt_alow,X.nxt_ahgh,X.hcount);
+  X.groups = true;
+}
+
+//  Phase 4: extend_kernel over the first items, then over re-runs until no item fails.  The triples of
+//  the items that failed (an arena overflowed: ST_*) and, after the hit-group launch, of every group whose
+//  tube reached the next group's first hit make the next list: each triple whole, hit after hit, on the
+//  wide-band kernel with larger arenas on fewer warps; collect_records drops what they emitted in
+//  earlier launches.  A launch that overflows the record buffer is repeated with a larger one.
+static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc, ExtendOut &R, cudaStream_t st)
+{ if (X.items.empty()) return FGB_OK;
+  int dev = 0, nsm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
+  const size_t smem = (size_t) EX_WARPS * STATE_BYTES + BOX_BYTES;
+  const size_t smem_big = (size_t) EX_WARPS * BIG_SMEM_PER_WARP + BOX_BYTES;
+  CUDA_TRY(cudaFuncSetAttribute(extend_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
+  CUDA_TRY(cudaFuncSetAttribute(extend_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
+  int bps = 0;
+  CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps,extend_kernel<EX_W>,EX_WARPS*32,smem));
+  if (bps < 1) bps = 1;
+  long long cells_per_warp = 1ll << 17;          // 128 K pebbles = 2 MB per warp
+  int stage_bytes = 1 << 15;
+  long long nblocks = launch_blocks((long long) X.items.size(),EX_NFRONT,(long long) nsm * bps,cells_per_warp);
+
+  //  a re-run list holds one item per triple of the list before it, so no list outgrows the first
+  std::vector<ExItem> items = X.items;
+  bool groups = X.groups;
+  std::vector<long long> ga(items.size());
+  std::vector<unsigned> hwork;                   // the work triples on the host, fetched for the first re-run
+  dblock<ExItem> d_items; dblock<unsigned> d_failed; dblock<long long> d_galast;
+  CUDA_TRY(d_items.alloc(items.size(),st));
+  CUDA_TRY(d_failed.alloc(items.size(),st));
+  if (groups) CUDA_TRY(d_galast.alloc(items.size(),st));
+  CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
+  P.items = d_items; P.failed = d_failed; P.galast = d_galast;
+  P.queue = d_misc + 1; P.nfailed = d_misc + 2; P.out_used = (u64 *) (d_misc + 4); P.need = d_misc + 10;
+  R.cap = (u64) P.nwork * 512 + (64ull << 20);
+  CUDA_TRY(R.buf.alloc(R.cap,st));
+  u64 used_before = 0;
+  for (int attempt = 0; ; attempt++)
+    { Arenas ar;
+      CUDA_TRY(ar.alloc(P,nblocks * EX_WARPS,cells_per_warp,stage_bytes,attempt > 0,st));
+      P.out = R.buf; P.out_cap = R.cap;
+      P.nitems = (int) items.size(); P.groups = groups; P.attempt = attempt;
+      CUDA_TRY(cudaMemsetAsync(d_misc+1,0,8,st));          // queue, nfailed
+      CUDA_TRY(cudaMemsetAsync(d_misc+10,0,4,st));         // reasons of this attempt's failures
+      { ev_timer t(1,st);
+        if (attempt == 0)
+          extend_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P);
+        else                                               // retries: wide-band kernel, state in HBM
+          extend_kernel<EX_WBIG><<<(unsigned) nblocks,EX_WARPS*32,smem_big,st>>>(P);
+      }
+      fgb_count_launch(1);
+      CUDA_TRY(cudaGetLastError());
+      unsigned misc[12];
+      CUDA_TRY(cudaMemcpyAsync(misc,d_misc,48,cudaMemcpyDeviceToHost,st));
+      if (groups) CUDA_TRY(cudaMemcpyAsync(ga.data(),d_galast,sizeof(long long)*items.size(),cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaStreamSynchronize(st));
+      ar.reset();                                          // before the record buffer may grow
+      R.used = ((u64) misc[5] << 32) | misc[4];
+      if (R.used > R.cap)
+        { //  record buffer too small: grow it (keeping earlier attempts' records) and repeat this attempt
+          if (attempt > 12) return FGB_ERR_OVERFLOW;
+          dblock<unsigned char> d_new;
+          const u64 ncap = R.used * 2 + (64ull << 20);
+          CUDA_TRY(d_new.alloc(ncap,st));
+          if (used_before) CUDA_TRY(cudaMemcpyAsync(d_new,R.buf,used_before,cudaMemcpyDeviceToDevice,st));
+          R.buf = std::move(d_new); R.cap = ncap;
+          CUDA_TRY(cudaMemcpyAsync(d_misc+4,&used_before,8,cudaMemcpyHostToDevice,st));
+          R.used = used_before;
+          for (size_t q = 0; q < R.rerun.size(); q++)        // the repeat runs under the next launch number
+            if (R.rerun[q].second == attempt) R.rerun[q].second = attempt + 1;
+          continue;
+        }
+      used_before = R.used;
+      //  the triples to re-run, by work-list position
+      std::vector<unsigned> fw;
+      if (misc[2] > 0)
+        { std::vector<unsigned> f(misc[2]);
+          CUDA_TRY(cudaMemcpyAsync(f.data(),d_failed,sizeof(unsigned)*f.size(),cudaMemcpyDeviceToHost,st));
+          CUDA_TRY(cudaStreamSynchronize(st));
+          for (size_t q = 0; q < f.size(); q++) fw.push_back(items[f[q]].w);
+        }
+      if (groups)                                          // a group's tube must have stopped short of the next group
+        for (size_t q = 0; q < items.size(); q++)
+          if (ga[q] > X.nxt_alow[q] || ga[q] >= X.nxt_ahgh[q]) fw.push_back(items[q].w);
+      std::sort(fw.begin(),fw.end());
+      fw.erase(std::unique(fw.begin(),fw.end()),fw.end());     // several groups of a triple failed: one re-run
+      if (groups)
+        { //  hit count (the -v line, FastGA.c:4371): the groups do not count their hits, a triple
+          //  that completed in this launch contributes its whole list, a re-run counts for itself
+          for (size_t q = 0; q < X.hcount.size(); q++) R.hits_done += X.hcount[q];
+          for (size_t q = 0; q < fw.size(); q++) R.hits_done -= X.hcount[fw[q]];
+          groups = false;
+        }
+      if (fw.empty()) break;
+      if (attempt > 12 || cells_per_warp > (1ll << 27)) return FGB_ERR_OVERFLOW;
+      if (hwork.empty())
+        { hwork.resize((size_t) P.nwork);
+          CUDA_TRY(cudaMemcpyAsync(hwork.data(),P.work,sizeof(unsigned)*hwork.size(),cudaMemcpyDeviceToHost,st));
+          CUDA_TRY(cudaStreamSynchronize(st));
+        }
+      items.resize(fw.size());
+      for (size_t q = 0; q < fw.size(); q++)
+        { const unsigned w = fw[q];
+          const uint2 hr = X.hrange.empty() ? make_uint2(0u,0x80000000u) : X.hrange[w];
+          items[q] = { w, hr.x, hr.y, 0u };
+          R.rerun.push_back(std::make_pair(hwork[w],attempt + 1));
+        }
+      CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
+      //  grow only what overflowed: a band too wide for the register / shared-memory state (ST_BAND)
+      //  just moves to the wide-band kernel with the same arenas
+      if (attempt > 0 || (misc[10] & (1u << ST_CELLS))) cells_per_warp *= 8;
+      if (attempt > 0 || (misc[10] & (1u << ST_STAGE))) stage_bytes *= 4;
+      nblocks = launch_blocks((long long) items.size(),EX_NFRONT,LLONG_MAX,cells_per_warp);
+    }
+  return FGB_OK;
+}
+
+//  Phase 5: the records to the host (when there were launches), less those a re-run triple emitted in
+//  its earlier launches (every record carries its launch number: a triple keeps those of its LAST), and
+//  the counters
+static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, const u64 *d_counters,
+                           cudaStream_t st)
+{ unsigned char *pin = NULL;
+  if (launched)
+    { CUDA_TRY(pinned_staging(R.used + 64,&pin));
+      O->h_buf = (unsigned char *) malloc(R.used + 64);
+      ev_timer t(2,st);
+      CUDA_TRY(cudaMemcpyAsync(pin,R.buf,R.used,cudaMemcpyDeviceToHost,st));
+    }
+  CUDA_TRY(cudaMemcpyAsync(O->counters,d_counters,16*8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  O->counters[0] += R.hits_done;
+  if (launched)
+    { memcpy(O->h_buf,pin,R.used);
+      O->nbytes = (long long) R.used;
+    }
+  if (!R.rerun.empty())
+    { std::vector<std::pair<unsigned,int> > todo(R.rerun), last;
+      std::sort(todo.begin(),todo.end());
+      for (size_t q = 0; q < todo.size(); q++)
+        if (q + 1 == todo.size() || todo[q+1].first != todo[q].first) last.push_back(todo[q]);
+      long long w = 0;
+      for (long long off = 0; off < O->nbytes; )
+        { int *h = (int *) (O->h_buf + off);
+          const long long sz = OUT_HDR + ((h[8] + 7) & ~7);
+          auto it = std::lower_bound(last.begin(),last.end(),std::make_pair((unsigned) h[0],INT_MIN));
+          if (!(it != last.end() && it->first == (unsigned) h[0] && it->second != h[9]))
+            { if (w != off) memmove(O->h_buf + w,O->h_buf + off,sz);
+              w += sz;
+            }
+          off += sz;
+        }
+      O->nbytes = w;
+    }
+  for (long long off = 0; off < O->nbytes; )
+    { int *h = (int *) (O->h_buf + off);
+      off += OUT_HDR + ((h[8] + 7) & ~7);
+      O->nrec += 1;
+    }
+  return FGB_OK;
+}
+
 extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B,
                           int chain_break, int chain_min, int align_min, double align_rate,
                           const short *tables, int ave_path, int tspace,
@@ -2474,12 +2644,10 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   if (A->d_rseq == NULL) return FGB_ERR_ARG;
   if (S->n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
   std::unique_ptr<fgb_overlaps> O(new fgb_overlaps());
-  long long n = S->n;
-  tr_mark("extend: enter");
 
   ext_params P;
   memset(&P,0,sizeof(P));
-  P.seeds = S->d_rec; P.nseeds = n;
+  P.seeds = S->d_rec; P.nseeds = S->n;
   P.p_anti = 12; P.anti_bits = S->anti_bits;
   P.p_band = P.p_anti + S->anti_bits; P.band_bits = S->band_bits;
   P.p_jc = P.p_band + S->band_bits; P.jc_bits = S->jc_bits;
@@ -2494,384 +2662,36 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   P.self_mode = S->self_mode;
   P.dscore = -tables[0] / TRIM_LEN;                     // SCORE[0] = -15 * dscore
 
-  dblock<short> d_tables;
-  dblock<u64> d_counters, d_total;
-  dblock<unsigned> d_flag, d_seg, d_work, d_misc, d_failed;
-  dblock<unsigned char> d_tmp;
+  dblock<short> d_tables; dblock<u64> d_counters; dblock<unsigned> d_misc;
   CUDA_TRY(d_tables.alloc(65536,st));
   CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
   P.score = d_tables; P.table = d_tables + 32768;
   CUDA_TRY(d_counters.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_counters,0,16*8,st));
-  CUDA_TRY(d_total.alloc(1,st));
+  P.counters = d_counters;
+  //  words 1 queue, 2 failed items, 4-5 record bytes, 6-7 prefilter counts, 8-9 hits listed, 10 failure reasons
   CUDA_TRY(d_misc.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
-  P.counters = d_counters;
 
-  unsigned nseg = 0, nwork = 0;
-  std::vector<unsigned> wsize; bool sizes_known = false;
-  dblock<ChunkPlan> d_plan; dblock<ChunkOut> d_couts; dblock<unsigned> d_first, d_failed_w;
-  dblock<ChainHit> d_hits; dblock<uint2> d_hrange; unsigned long long hit_cap = 0;
-  //  hit groups (first launch): items in launch order, and for each the first hit of the NEXT group of
-  //  its triple (what its tube must not have reached for the groups to have been independent)
-  dblock<ExItem> d_items; dblock<long long> d_galast; dblock<int2> d_tinfo;
-  std::vector<ExItem> items; std::vector<long long> nxt_alow, nxt_ahgh;
-  std::vector<unsigned> hwork, hcount;                 // work triples; hits of each pre-scanned one
-  unsigned long long hits_done = 0;                    // hits of the pre-scanned triples the first launch completed
-  if (n > 0)
+  dblock<unsigned> d_seg, d_work; dblock<ChainHit> d_hits;
+  ExtendPlan X;
+  if (S->n > 0)
     { ev_timer t(0,st);
-      long long tmpb = fgb_dev_scan_tmp_bytes(n);
-      CUDA_TRY(d_flag.alloc(n+1,st));
-      CUDA_TRY(d_tmp.alloc(tmpb,st));
-      int nb = (int) ((n + 255) / 256);
-      seg_flag_kernel<<<nb,256,0,st>>>(S->d_rec,n,P.p_band,d_flag);
-      int rc = fgb_dev_exclusive_scan_u32(d_flag,n,d_total,d_tmp,tmpb,st);
+      std::vector<unsigned> wsize;
+      int rc = extend_triples(P,S,d_misc,d_seg,d_work,wsize,st);
       if (rc) return rc;
-      u64 tot = 0;
-      CUDA_TRY(cudaMemcpyAsync(&tot,d_total,8,cudaMemcpyDeviceToHost,st));
-      CUDA_TRY(cudaStreamSynchronize(st));
-      nseg = (unsigned) tot;
-      TR_SYNC("  seg flags + scan");
-      CUDA_TRY(d_seg.alloc(nseg+2,st));
-      CUDA_TRY(d_work.alloc(3ll*nseg+3,st));
-      nb = (int) ((n + 1 + 255) / 256);
-      seg_fill2_kernel<<<nb,256,0,st>>>(S->d_rec,n,P.p_band,d_flag,d_seg,nseg);
-      P.seg_start = d_seg; P.nseg = (int) nseg;
-      prefilter_kernel<<<(nseg + 127)/128,128,0,st>>>(P,d_work,d_work + nseg + 1,d_misc + 6,d_work + 2ll*nseg + 2);
-      fgb_count_launch(3);
-      CUDA_TRY(cudaGetLastError());
-      unsigned nw2[2];
-      CUDA_TRY(cudaMemcpyAsync(nw2,d_misc + 6,8,cudaMemcpyDeviceToHost,st));
-      CUDA_TRY(cudaStreamSynchronize(st));
-      TR_SYNC("  seg fill + prefilter");
-      //  long triples first, largest first (the kernel's makespan is its longest triple, so it
-      //  must not start late), then the exact short hits
-      if (nw2[0] >= 1 && nw2[0] <= (1u << 20))
-        { std::vector<unsigned> lj(nw2[0]), ls(nw2[0]), ord(nw2[0]);
-          CUDA_TRY(cudaMemcpyAsync(lj.data(),d_work,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
-          CUDA_TRY(cudaMemcpyAsync(ls.data(),d_work + 2ll*nseg + 2,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
-          CUDA_TRY(cudaStreamSynchronize(st));
-          for (unsigned q = 0; q < nw2[0]; q++) ord[q] = q;
-          std::sort(ord.begin(),ord.end(),[&](unsigned a, unsigned b)
-                    { return ls[a] != ls[b] ? ls[a] > ls[b] : lj[a] < lj[b]; });
-          std::vector<unsigned> sj(nw2[0]);
-          wsize.resize(nw2[0]);
-          for (unsigned q = 0; q < nw2[0]; q++) { sj[q] = lj[ord[q]]; wsize[q] = ls[ord[q]]; }
-          CUDA_TRY(cudaMemcpyAsync(d_work,sj.data(),4ull*nw2[0],cudaMemcpyHostToDevice,st));
-          CUDA_TRY(cudaStreamSynchronize(st));
-          sizes_known = true;
+      if (!wsize.empty())
+        { rc = chain_detect(P,wsize,d_misc,d_hits,X,st);
+          if (rc) return rc;
+          P.hits = d_hits;
         }
-      else if (nw2[0] == 0) sizes_known = true;
-      CUDA_TRY(cudaMemcpyAsync(d_work + nw2[0],d_work + nseg + 1,sizeof(unsigned)*nw2[1],
-                               cudaMemcpyDeviceToDevice,st));
-      nwork = nw2[0] + nw2[1];
-      TR_SYNC("  work list ordered");
-
-      //  chain detection of every work triple, chunk-parallel (chain_plan / chain_chunk / chain_stitch)
-      if (sizes_known && nwork > 0)
-        { std::vector<ChunkPlan> plan;
-          std::vector<unsigned> first(nwork + 1);
-          for (unsigned w = 0; w < nwork; w++)
-            { unsigned size = w < wsize.size() ? wsize[w] : 0;
-              unsigned nch = (unsigned) (((unsigned long long) size + CH_SEEDS + CH_SEEDS/2 - 1) / (CH_SEEDS + CH_SEEDS/2));
-              if (nch < 1) nch = 1;
-              if (w >= CH_TOPK || w >= wsize.size()) nch = 0;          // scanned inside extend_kernel
-              first[w] = (unsigned) plan.size();
-              for (unsigned k = 0; k < nch; k++)
-                { ChunkPlan c; c.w = w; c.j = 0; c.k = k; c.nch = nch; c.sL = c.sU = 0; plan.push_back(c); }
-            }
-          first[nwork] = (unsigned) plan.size();
-          const int nplan = (int) plan.size();
-          if (nplan > 0) {
-          hit_cap = (unsigned long long) nplan * (CH_HCAP + 1) + nwork + 16;
-          CUDA_TRY(d_plan.alloc((size_t) nplan,st));
-          CUDA_TRY(d_couts.alloc((size_t) nplan,st));
-          CUDA_TRY(d_first.alloc((size_t) (nwork + 1),st));
-          CUDA_TRY(d_hits.alloc((size_t) hit_cap,st));
-          CUDA_TRY(d_hrange.alloc((size_t) nwork,st));
-          CUDA_TRY(d_tinfo.alloc((size_t) nwork,st));
-          CUDA_TRY(cudaMemcpyAsync(d_plan,plan.data(),sizeof(ChunkPlan)*(size_t) nplan,cudaMemcpyHostToDevice,st));
-          CUDA_TRY(cudaMemcpyAsync(d_first,first.data(),sizeof(unsigned)*(size_t) (nwork + 1),cudaMemcpyHostToDevice,st));
-          CUDA_TRY(cudaMemsetAsync(d_misc + 8,0,8,st));
-          P.work = d_work; P.nwork = (int) nwork;
-          TR_SYNC("  chain: plan uploaded");
-          chain_plan_kernel<<<(nplan + 127)/128,128,0,st>>>(P,d_plan,nplan);
-          TR_SYNC("  chain: plan kernel");
-          chain_chunk_kernel<<<(nplan + 3)/4,128,0,st>>>(P,d_plan,nplan,d_couts);
-          if (tr_on()) { cudaStreamSynchronize(st); fprintf(stderr,"[fgb_trace]   nwork %u nplan %d\n",nwork,nplan); tr_mark("  chain: chunk kernel"); }
-          chain_stitch_kernel<<<(nwork + 127)/128,128,0,st>>>(P,d_plan,d_couts,d_first,(int) nwork,d_hits,
-                                                             (unsigned long long *) (d_misc + 8),hit_cap,d_hrange,d_tinfo);
-          fgb_count_launch(3);
-          CUDA_TRY(cudaGetLastError());
-          CUDA_TRY(cudaStreamSynchronize(st));                 // plan / first are host vectors
-          TR_SYNC("  chain: stitch kernel");
-          P.hits = d_hits; P.hit_range = d_hrange;
-
-          //  Hit groups.  Inside a triple a hit is clipped or skipped by the end of the alignments
-          //  before it (alast, FastGA.c:3262-3318), which chains its hits serially.  In practice a hit is
-          //  only ever touched by an alignment of ITS aligned block: the block's seed chains in this band
-          //  pair and in the neighbouring ones, overlapping end to end while the path drifts across
-          //  bands.  Chains of one (strand, contig pair) within SPEC_BANDS bands whose anti-diagonal
-          //  intervals (+- SPEC_SLACK) overlap are joined into components (union-find); a triple's hit list is cut
-          //  wherever the components before and after the cut are disjoint.  Every group is a work
-          //  item of its own that starts with a clear tube; after the launch the host checks that no
-          //  group's tube reached the next group's first hit -- else the triple is re-run in one piece
-          //  (retry ladder below), so a wrong guess costs time, never the result.
-          { int SPEC_BANDS = 1; long long SPEC_SLACK = 1000;
-            if (getenv("FGB_SPEC_BANDS") != NULL) SPEC_BANDS = atoi(getenv("FGB_SPEC_BANDS"));
-            if (getenv("FGB_SPEC_SLACK") != NULL) SPEC_SLACK = atoll(getenv("FGB_SPEC_SLACK"));
-            long long SPEC_GAP = -1;                                   // tests: cut at every gap >= this instead
-            if (getenv("FGB_SPEC_GAP") != NULL) SPEC_GAP = atoll(getenv("FGB_SPEC_GAP"));
-            //  the small result arrays come back through the pinned staging buffer: four copies in flight and
-            //  one synchronisation instead of a staged, synchronous copy each
-            unsigned long long hused = 0;
-            std::vector<uint2> hrange(nwork);
-            std::vector<int2> tinfo(nwork);
-            hwork.resize(nwork); hcount.assign(nwork,0u);
-            { const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork,
-                           o4 = o3 + sizeof(unsigned)*(size_t) nwork;
-              unsigned char *hp;
-              CUDA_TRY(pinned_staging(o4,&hp));
-              CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
-              CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
-              CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
-              CUDA_TRY(cudaMemcpyAsync(hp + o3,d_work,sizeof(unsigned)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
-              CUDA_TRY(cudaStreamSynchronize(st));
-              memcpy(&hused,hp,8);
-              memcpy(hrange.data(),hp + o1,sizeof(uint2)*(size_t) nwork);
-              memcpy(tinfo.data(),hp + o2,sizeof(int2)*(size_t) nwork);
-              memcpy(hwork.data(),hp + o3,sizeof(unsigned)*(size_t) nwork);
-            }
-            if (hused > hit_cap) hused = hit_cap;
-            std::vector<ChainHit> hh((size_t) hused + 1);
-            if (hused > 0)
-              { unsigned char *hp;
-                CUDA_TRY(pinned_staging(sizeof(ChainHit)*(size_t) hused,&hp));
-                CUDA_TRY(cudaMemcpyAsync(hp,d_hits,sizeof(ChainHit)*(size_t) hused,cudaMemcpyDeviceToHost,st));
-                CUDA_TRY(cudaStreamSynchronize(st));
-                memcpy(hh.data(),hp,sizeof(ChainHit)*(size_t) hused);
-              }
-            build_hit_groups(nwork,hrange.data(),tinfo.data(),hh.data(),hused,SPEC_BANDS,SPEC_SLACK,SPEC_GAP,
-                             items,nxt_alow,nxt_ahgh,hcount);
-            if (!items.empty())
-              { CUDA_TRY(d_items.alloc(items.size(),st));
-                CUDA_TRY(d_galast.alloc(items.size(),st));
-                CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
-              }                                                      // (`items` lives until the launches are over)
-            TR_SYNC("  chain: hit groups");
-          }
-          }
-        }
+      first_items((unsigned) P.nwork,X);
     }
-  O->nseg = nseg; O->nwork = nwork;
-  tr_mark("extend: triples+prefilter");
-
-  dblock<unsigned char> d_out;
-  u64 out_cap = 0, out_used = 0;
-  if (nwork > 0)
-    { int dev = 0, nsm = 132;
-      cudaGetDevice(&dev);
-      cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
-      size_t smem = (size_t) EX_WARPS * STATE_BYTES + BOX_BYTES;
-      size_t smem_big = (size_t) EX_WARPS * BIG_SMEM_PER_WARP + BOX_BYTES;
-      CUDA_TRY(cudaFuncSetAttribute(extend_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
-      CUDA_TRY(cudaFuncSetAttribute(extend_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
-      int bps = 0;
-      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps,extend_kernel<EX_W>,EX_WARPS*32,smem));
-      if (bps < 1) bps = 1;
-      long long nblocks = (long long) nsm * bps;
-      bool use_items = (P.hit_range != NULL);              // first launch over hit groups
-      long long want = ((long long) (use_items ? items.size() : nwork) + EX_NFRONT - 1) / EX_NFRONT;
-      if (want < 1) want = 1;
-      if (nblocks > want) nblocks = want;
-      long long nwarps = nblocks * EX_WARPS;
-
-      CUDA_TRY(d_failed.alloc(nwork+1,st));
-      CUDA_TRY(d_failed_w.alloc(nwork+1,st));
-      P.work = d_work; P.nwork = (int) nwork;
-      P.queue = d_misc + 1; P.nfailed = d_misc + 2; P.failed = d_failed; P.failed_w = d_failed_w; P.widx = NULL; P.need = d_misc + 10;
-      P.out_used = (u64 *) (d_misc + 4);
-
-      long long cells_per_warp = 1ll << 17;          // 128 K pebbles = 2 MB per warp
-      int stage_bytes = 1 << 15;
-      out_cap = (u64) nwork * 512 + (64ull << 20);
-      std::vector<std::pair<unsigned,int> > todo;    // (triple, launch number) of every re-run
-      unsigned *d_list = d_work; unsigned nlist = use_items ? (unsigned) items.size() : nwork;
-      dblock<unsigned> d_work2;
-      u64 used_before = 0;
-      for (int attempt = 0; nlist > 0; attempt++)
-        { dblock<Peb> d_cells; dblock<unsigned char> d_stage, d_big;
-          dblock<unsigned long long> d_wlog;
-          CUDA_TRY(d_cells.alloc(cells_per_warp*nwarps,st));
-          CUDA_TRY(d_stage.alloc(2ll*stage_bytes*nwarps,st));
-          if (d_out == NULL) CUDA_TRY(d_out.alloc(out_cap,st));
-          P.cells = d_cells; P.cells_per_warp = cells_per_warp;
-          P.stage = d_stage; P.stage_bytes = stage_bytes;
-          P.out = d_out; P.out_cap = out_cap;
-          P.work = d_list; P.nwork = (int) nlist;
-          P.items = use_items ? (ExItem *) d_items : NULL; P.galast = d_galast; P.attempt = attempt;
-          if (attempt > 0)                                     // retries: wide-band kernel, state in HBM
-            { CUDA_TRY(d_big.alloc((size_t) nwarps * WSTATE_BYTES(EX_WBIG),st));
-              P.bigstate = d_big;
-            }
-          tr_mark("extend: arenas allocated");
-          if (attempt == 0 && getenv("FGB_WLOG") != NULL)
-            { CUDA_TRY(d_wlog.alloc(4ull*(nlist+1),st));
-              CUDA_TRY(cudaMemsetAsync(d_wlog,0,32ull*(nlist+1),st));
-            }
-          P.wlog = d_wlog;
-          CUDA_TRY(cudaMemsetAsync(d_misc+1,0,8,st));          // queue, nfailed
-          CUDA_TRY(cudaMemsetAsync(d_misc+10,0,4,st));         // reasons of this attempt's failures
-          { ev_timer t(1,st);
-            if (attempt == 0)
-              extend_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P);
-            else
-              extend_kernel<EX_WBIG><<<(unsigned) nblocks,EX_WARPS*32,smem_big,st>>>(P);
-          }
-          fgb_count_launch(1);
-          CUDA_TRY(cudaGetLastError());
-          unsigned misc[12];
-          CUDA_TRY(cudaMemcpyAsync(misc,d_misc,48,cudaMemcpyDeviceToHost,st));
-          CUDA_TRY(cudaStreamSynchronize(st));
-          tr_mark("extend: kernel done");
-          if (d_wlog != NULL)
-            { std::vector<unsigned long long> lg(4ull*nlist);
-              CUDA_TRY(cudaMemcpy(lg.data(),d_wlog,32ull*nlist,cudaMemcpyDeviceToHost));
-              FILE *f = fopen(getenv("FGB_WLOG"),"w");
-              if (f != NULL)
-                { for (unsigned q = 0; q < nlist; q++)
-                    fprintf(f,"%u %llu %llu %llu %llu %llu %llu %llu %u %u %u\n",q,lg[4*q] >> 32,lg[4*q] & 0xffffffffull,
-                            lg[4*q+1] >> 24,(lg[4*q+1] >> 8) & 0xffff,lg[4*q+1] & 0xff,lg[4*q+2],lg[4*q+3],
-                            (P.items != NULL ? (items[q].w < wsize.size() ? wsize[items[q].w] : 0u)
-                                             : (q < wsize.size() ? wsize[q] : 0u)),
-                            P.items != NULL ? (items[q].hn & 0x7fffffffu) : 0u,P.items != NULL ? items[q].g : 0u);
-                  fclose(f);
-                }
-              d_wlog.reset();
-            }
-          d_cells.reset(); d_stage.reset(); d_big.reset();     // before the record buffer may grow
-          out_used = ((u64) misc[5] << 32) | misc[4];
-          unsigned nfailed = misc[2];
-          if (out_used > out_cap)
-            { //  record buffer too small: grow it (keeping earlier attempts' records) and
-              //  repeat this attempt
-              if (attempt > 12) return FGB_ERR_OVERFLOW;
-              dblock<unsigned char> d_new;
-              u64 ncap = out_used * 2 + (64ull << 20);
-              CUDA_TRY(d_new.alloc(ncap,st));
-              if (used_before) CUDA_TRY(cudaMemcpy(d_new,d_out,used_before,cudaMemcpyDeviceToDevice));
-              d_out = std::move(d_new); out_cap = ncap;
-              CUDA_TRY(cudaMemcpy(d_misc+4,&used_before,8,cudaMemcpyHostToDevice));
-              out_used = used_before;
-              for (size_t q = 0; q < todo.size(); q++)            // the repeat runs under the next launch number
-                if (todo[q].second == attempt) todo[q].second = attempt + 1;
-              continue;
-            }
-          used_before = out_used;
-          //  failed triples (and their positions in the first list, which index the hit lists)
-          std::vector<unsigned> f(nfailed), fw(nfailed);
-          if (nfailed > 0)
-            { CUDA_TRY(cudaMemcpy(f.data(),d_failed,sizeof(unsigned)*nfailed,cudaMemcpyDeviceToHost));
-              CUDA_TRY(cudaMemcpy(fw.data(),d_failed_w,sizeof(unsigned)*nfailed,cudaMemcpyDeviceToHost));
-            }
-          if (use_items)
-            { //  were the hit groups independent?  a group's tube must have stopped short of the next group's first hit
-              std::vector<long long> ga(items.size());
-              CUDA_TRY(cudaMemcpy(ga.data(),d_galast,sizeof(long long)*items.size(),cudaMemcpyDeviceToHost));
-              for (size_t q = 0; q < items.size(); q++)
-                if (ga[q] > nxt_alow[q] || ga[q] >= nxt_ahgh[q])
-                  { f.push_back(hwork[items[q].w]); fw.push_back(items[q].w); }
-              //  several groups of a triple may have failed: one re-run each
-              std::vector<std::pair<unsigned,unsigned> > u(f.size());
-              for (size_t q = 0; q < f.size(); q++) u[q] = std::make_pair(fw[q],f[q]);
-              std::sort(u.begin(),u.end());
-              u.erase(std::unique(u.begin(),u.end()),u.end());
-              f.resize(u.size()); fw.resize(u.size());
-              for (size_t q = 0; q < u.size(); q++) { fw[q] = u[q].first; f[q] = u[q].second; }
-              if (tr_on()) fprintf(stderr,"[fgb_trace]   hit groups %zu, triples to re-run %zu (%u arena overflows)\n",items.size(),u.size(),nfailed);
-              nfailed = (unsigned) f.size();
-              use_items = false;
-              //  hit count (the -v line, FastGA.c:4371): the groups do not count their hits, a triple
-              //  that completed in this launch contributes its whole list, a re-run counts for itself
-              for (size_t q = 0; q < hcount.size(); q++) hits_done += hcount[q];
-              for (size_t q = 0; q < fw.size(); q++) hits_done -= hcount[fw[q]];
-            }
-          if (nfailed == 0) break;
-          if (attempt > 12 || cells_per_warp > (1ll << 27)) return FGB_ERR_OVERFLOW;
-          //  rerun only the failed triples (whole, hit after hit) with larger arenas on fewer warps; the
-          //  records of their earlier launches are dropped by the host below.
-          for (size_t q = 0; q < f.size(); q++) todo.push_back(std::make_pair(f[q],attempt + 1));
-          if (d_work2 == NULL) CUDA_TRY(d_work2.alloc(2*(nwork+1),st));
-          CUDA_TRY(cudaMemcpy(d_work2,f.data(),sizeof(unsigned)*nfailed,cudaMemcpyHostToDevice));
-          CUDA_TRY(cudaMemcpy(d_work2 + nwork + 1,fw.data(),sizeof(unsigned)*nfailed,cudaMemcpyHostToDevice));
-          P.widx = d_work2 + nwork + 1;
-          d_list = d_work2; nlist = nfailed;
-          //  grow only what overflowed: a band too wide for the register / shared-memory state (ST_BAND)
-          //  just moves to the wide-band kernel below with the same arenas
-          if (attempt > 0 || (misc[10] & (1u << ST_CELLS))) cells_per_warp *= 8;
-          if (attempt > 0 || (misc[10] & (1u << ST_STAGE))) stage_bytes *= 4;
-          long long nb2 = ((long long) nfailed + EX_NFRONT - 1) / EX_NFRONT;
-          long long maxb = (24ll << 30) / ((long long) sizeof(Peb) * cells_per_warp * EX_WARPS);
-          if (maxb < 1) maxb = 1;
-          nblocks = nb2 < maxb ? nb2 : maxb;
-          nwarps = nblocks * EX_WARPS;
-        }
-      d_work2.reset();
-
-      //  bring the records back and drop partial output of triples that were re-run
-      O->nbytes = (long long) out_used;
-      tr_mark("extend: attempts done");
-      unsigned char *pin;
-      CUDA_TRY(pinned_staging(out_used + 64,&pin));
-      O->h_buf = (unsigned char *) malloc(out_used + 64);
-      { ev_timer t(2,st);
-        CUDA_TRY(cudaMemcpyAsync(pin,d_out,out_used,cudaMemcpyDeviceToHost,st));
-      }
-      CUDA_TRY(cudaStreamSynchronize(st));
-      memcpy(O->h_buf,pin,out_used);
-      tr_mark("extend: d2h");
-      if (!todo.empty())
-        { //  a re-run triple may have emitted records in earlier launches: keep only those of its
-          //  LAST launch (every record carries its launch number)
-          std::sort(todo.begin(),todo.end());
-          std::vector<std::pair<unsigned,int> > last;
-          for (size_t q = 0; q < todo.size(); q++)
-            if (q + 1 == todo.size() || todo[q+1].first != todo[q].first) last.push_back(todo[q]);
-          std::vector<long long> offs;
-          for (long long off = 0; off < O->nbytes; )
-            { int *h = (int *) (O->h_buf + off);
-              offs.push_back(off);
-              off += OUT_HDR + ((h[8] + 7) & ~7);
-            }
-          std::vector<char> keep(offs.size(),1);
-          for (size_t i = 0; i < offs.size(); i++)
-            { int *h = (int *) (O->h_buf + offs[i]);
-              auto it = std::lower_bound(last.begin(),last.end(),std::make_pair((unsigned) h[0],INT_MIN));
-              if (it != last.end() && it->first == (unsigned) h[0] && it->second != h[9]) keep[i] = 0;
-            }
-          long long w = 0;
-          for (size_t i = 0; i < offs.size(); i++)
-            { int *h = (int *) (O->h_buf + offs[i]);
-              long long sz = OUT_HDR + ((h[8] + 7) & ~7);
-              if (keep[i])
-                { if (w != offs[i]) memmove(O->h_buf + w,O->h_buf + offs[i],sz);
-                  w += sz;
-                }
-            }
-          O->nbytes = w;
-        }
-    }
-  CUDA_TRY(cudaMemcpy(O->counters,d_counters,16*8,cudaMemcpyDeviceToHost));
-  O->counters[0] += hits_done;
-  { long long cnt = 0;
-    for (long long off = 0; off < O->nbytes; )
-      { int *h = (int *) (O->h_buf + off);
-        off += OUT_HDR + ((h[8] + 7) & ~7);
-        cnt += 1;
-      }
-    O->nrec = cnt;
-  }
-  tr_mark("extend: leave");
+  O->nseg = P.nseg; O->nwork = P.nwork;
+  ExtendOut R;
+  int rc = (P.nwork > 0) ? extend_launches(P,X,d_misc,R,st) : FGB_OK;
+  if (rc == FGB_OK) rc = collect_records(O.get(),R,P.nwork > 0,d_counters,st);
+  if (rc) return rc;
   *out = O.release();                                        // (the device blocks go back as the call returns)
   return FGB_OK;
 }
@@ -2905,15 +2725,13 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
-  long long nblocks = (n + EX_WARPS - 1) / EX_WARPS;
-  if (nblocks > nsm) nblocks = nsm;
-  const long long nwarps = nblocks * EX_WARPS;
-  const long long cells_per_warp = 1ll << 18;
-  const int stage_bytes = 1 << 16;
+  long long cells_per_warp = 1ll << 18;
+  int stage_bytes = 1 << 16;
+  const long long nblocks = launch_blocks(n,EX_WARPS,nsm,cells_per_warp);
   const size_t smem = (size_t) EX_WARPS * STATE_BYTES;
   dblock<short> d_tables; dblock<la_job> d_jobs; dblock<int> d_status; dblock<unsigned> d_misc;
-  dblock<Peb> d_cells; dblock<unsigned char> d_stage, d_out, d_big; dblock<unsigned> d_idx;
-  long long cells_big = cells_per_warp; int stage_big = stage_bytes;
+  dblock<unsigned char> d_out; dblock<unsigned> d_idx;
+  Arenas ar;
   std::vector<unsigned char> h;
   std::vector<int> hs(n);
   u64 out_cap = (u64) n * 256 + (u64) traces_cap + (1ull << 20), out_used = 0;
@@ -2922,15 +2740,12 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   CUDA_TRY(d_jobs.alloc((size_t) n,st));
   CUDA_TRY(d_status.alloc((size_t) n,st));
   CUDA_TRY(d_misc.alloc(16,st));
-  CUDA_TRY(d_cells.alloc(cells_per_warp*nwarps,st));
-  CUDA_TRY(d_stage.alloc(2ll*stage_bytes*nwarps,st));
+  CUDA_TRY(ar.alloc(P,nblocks * EX_WARPS,cells_per_warp,stage_bytes,false,st));
   CUDA_TRY(d_out.alloc(out_cap,st));
   CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_jobs,jobs,sizeof(la_job)*(size_t) n,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
   P.score = d_tables; P.table = d_tables + 32768;
-  P.cells = d_cells; P.cells_per_warp = cells_per_warp;
-  P.stage = d_stage; P.stage_bytes = stage_bytes;
   P.out = d_out; P.out_cap = out_cap; P.out_used = (u64 *) (d_misc + 4);
   P.queue = d_misc + 1;
   la_batch_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P,d_jobs,NULL,(int) n,d_status);
@@ -2949,24 +2764,15 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
         if (hs[i] != ST_OK) redo.push_back((unsigned) i);
       if (redo.empty()) break;
       if (attempt > 4) return FGB_ERR_OVERFLOW;
-      if (attempt > 1) { cells_big *= 8; stage_big *= 4; }
+      if (attempt > 1) { cells_per_warp *= 8; stage_bytes *= 4; }
       const size_t smem_big = (size_t) EX_WARPS * BIG_SMEM_PER_WARP;
-      long long nb2 = ((long long) redo.size() + EX_WARPS - 1) / EX_WARPS;
-      if (nb2 > nsm) nb2 = nsm;
-      long long maxb = (24ll << 30) / ((long long) sizeof(Peb) * cells_big * EX_WARPS);
-      if (nb2 > maxb) nb2 = maxb > 1 ? maxb : 1;
-      const long long nw2 = nb2 * EX_WARPS;
-      d_cells.reset(); d_stage.reset(); d_big.reset(); d_idx.reset();      // all four before the larger ones
-      CUDA_TRY(d_cells.alloc(cells_big*nw2,st));
-      CUDA_TRY(d_stage.alloc(2ll*stage_big*nw2,st));
-      CUDA_TRY(d_big.alloc((size_t) nw2 * WSTATE_BYTES(EX_WBIG),st));
+      const long long nb2 = launch_blocks((long long) redo.size(),EX_WARPS,nsm,cells_per_warp);
+      d_idx.reset();                                               // all four before the larger ones
+      CUDA_TRY(ar.alloc(P,nb2 * EX_WARPS,cells_per_warp,stage_bytes,true,st));
       CUDA_TRY(d_idx.alloc(redo.size(),st));
       CUDA_TRY(cudaMemcpyAsync(d_idx,redo.data(),sizeof(unsigned)*redo.size(),cudaMemcpyHostToDevice,st));
       CUDA_TRY(cudaMemsetAsync(d_misc + 1,0,4,st));                 // queue
       CUDA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
-      P.cells = d_cells; P.cells_per_warp = cells_big;
-      P.stage = d_stage; P.stage_bytes = stage_big;
-      P.bigstate = d_big;
       la_batch_kernel<EX_WBIG><<<(unsigned) nb2,EX_WARPS*32,smem_big,st>>>(P,d_jobs,d_idx,(int) redo.size(),d_status);
       fgb_count_launch(1);
       CUDA_TRY(cudaGetLastError());
@@ -2976,7 +2782,8 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       if (out_used > out_cap) return FGB_ERR_OVERFLOW;
     }
   h.resize((size_t) out_used + 64);
-  CUDA_TRY(cudaMemcpy(h.data(),d_out,out_used,cudaMemcpyDeviceToHost));
+  CUDA_TRY(cudaMemcpyAsync(h.data(),d_out,out_used,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
   long long used = 0;
   for (long long i = 0; i < n; i++)
     { int *p = paths + 7*i;
