@@ -204,7 +204,7 @@ static __device__ __forceinline__ int ld_acquire_smem(const volatile int *p)
 }
 #define IX(k) ((k) & (W-1))
 
-static __device__ __forceinline__ u64 get_bits(const rec128 &r, int pos, int n)
+static __host__ __device__ __forceinline__ u64 get_bits(const rec128 &r, int pos, int n)
 { u64 v;
   if (pos >= 64) v = r.hi >> (pos-64);
   else if (pos == 0) v = r.lo;
@@ -2328,11 +2328,13 @@ struct Arenas
 
 //  What fgb_extend plans for extend_kernel.  Per work triple w: hrange[w] = its hit list (first hit,
 //  count | bit 31: no list, the kernel scans the triple) into hh[0..hused), tinfo[w] = ((strand, contig
-//  pair) key, band); both empty when chain detection did not run.  The items of the first launch; when
-//  they are hit groups, for each the first hit of the next group of its triple, and the hits per triple.
+//  pair) key, band); both empty when chain detection did not run.  hasked: the hit slots the triples
+//  reserved, of hit_cap (a triple past it has no list), in nplan chunks.  The items of the first launch;
+//  when they are hit groups, for each the first hit of the next group of its triple, and the hits per
+//  triple.
 struct ExtendPlan
 { std::vector<uint2> hrange; std::vector<int2> tinfo;
-  std::vector<ChainHit> hh; unsigned long long hused = 0;
+  std::vector<ChainHit> hh; unsigned long long hused = 0, hasked = 0, hit_cap = 0; long long nplan = 0;
   std::vector<ExItem> items; bool groups = false;
   std::vector<long long> nxt_alow, nxt_ahgh; std::vector<unsigned> hcount;
 };
@@ -2393,9 +2395,10 @@ static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, d
 }
 
 //  Phase 2: chain detection of the long work triples, chunk-parallel (chain_plan / chain_chunk /
-//  chain_stitch; the short ones are scanned in extend_kernel).  The hit lists stay in d_hits for the
-//  kernel and come to the host (X.hrange, X.tinfo, X.hh) in one staged download.
-static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize, unsigned *d_misc,
+//  chain_stitch; the short ones are scanned in extend_kernel), `chunk` merged seeds a chunk.  The hit
+//  lists stay in d_hits for the kernel and come to the host (X.hrange, X.tinfo, X.hh) in one staged
+//  download.
+static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize, long long chunk, unsigned *d_misc,
                         dblock<ChainHit> &d_hits, ExtendPlan &X, cudaStream_t st)
 { const unsigned nwork = (unsigned) P.nwork;
   std::vector<ChunkPlan> plan;
@@ -2403,7 +2406,7 @@ static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize,
   for (unsigned w = 0; w < nwork; w++)
     { unsigned nch = 0;
       if (w < wsize.size())
-        { nch = (unsigned) (((unsigned long long) wsize[w] + CH_SEEDS + CH_SEEDS/2 - 1) / (CH_SEEDS + CH_SEEDS/2));
+        { nch = (unsigned) (((unsigned long long) wsize[w] + chunk - 1) / chunk);
           if (nch < 1) nch = 1;
         }
       first[w] = (unsigned) plan.size();
@@ -2445,6 +2448,7 @@ static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize,
     memcpy(X.hrange.data(),hp + o1,sizeof(uint2)*(size_t) nwork);
     memcpy(X.tinfo.data(),hp + o2,sizeof(int2)*(size_t) nwork);
   }
+  X.hasked = X.hused; X.hit_cap = hit_cap; X.nplan = nplan;
   if (X.hused > hit_cap) X.hused = hit_cap;
   X.hh.resize((size_t) X.hused + 1);
   if (X.hused > 0)
@@ -2455,6 +2459,14 @@ static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize,
       memcpy(X.hh.data(),hp,sizeof(ChainHit)*(size_t) X.hused);
     }
   return FGB_OK;
+}
+
+//  Merged seeds per chunk of chain detection: CH_SEEDS x 1.5, or FGB_CHAIN_CHUNK (0 or less: no chain detection,
+//  every work triple is scanned in extend_kernel, as beyond 2^20 long triples)
+static long long chain_chunk_seeds()
+{ long long chunk = CH_SEEDS + CH_SEEDS/2;
+  if (getenv("FGB_CHAIN_CHUNK") != NULL) chunk = atoll(getenv("FGB_CHAIN_CHUNK"));
+  return chunk;
 }
 
 //  Phase 3: the items of the first launch.  With hit lists, the hit groups of build_hit_groups
@@ -2636,6 +2648,21 @@ static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, c
   return FGB_OK;
 }
 
+//  The fields of P that the segments, the prefilter and chain detection read: the seeds' layout and the
+//  chain parameters
+static void seed_params(ext_params &P, const fgb_seeds *S, int chain_break, int chain_min)
+{ memset(&P,0,sizeof(P));
+  P.seeds = S->d_rec; P.nseeds = S->n;
+  P.p_anti = 12; P.anti_bits = S->anti_bits;
+  P.p_band = P.p_anti + S->anti_bits; P.band_bits = S->band_bits;
+  P.p_jc = P.p_band + S->band_bits; P.jc_bits = S->jc_bits;
+  P.p_ic = P.p_jc + S->jc_bits; P.ic_bits = S->ic_bits;
+  P.p_cp = P.p_ic + S->ic_bits;
+  P.amxpos = S->amxpos; P.bmxpos = S->bmxpos;
+  P.chain_break = chain_break; P.chain_min = chain_min;
+  P.self_mode = S->self_mode;
+}
+
 extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B,
                           int chain_break, int chain_min, int align_min, double align_rate,
                           const short *tables, int ave_path, int tspace,
@@ -2646,21 +2673,13 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   std::unique_ptr<fgb_overlaps> O(new fgb_overlaps());
 
   ext_params P;
-  memset(&P,0,sizeof(P));
-  P.seeds = S->d_rec; P.nseeds = S->n;
-  P.p_anti = 12; P.anti_bits = S->anti_bits;
-  P.p_band = P.p_anti + S->anti_bits; P.band_bits = S->band_bits;
-  P.p_jc = P.p_band + S->band_bits; P.jc_bits = S->jc_bits;
-  P.p_ic = P.p_jc + S->jc_bits; P.ic_bits = S->ic_bits;
-  P.p_cp = P.p_ic + S->ic_bits;
-  P.amxpos = S->amxpos; P.bmxpos = S->bmxpos;
+  seed_params(P,S,chain_break,chain_min);
   P.aseq = A->d_seq; P.arseq = A->d_rseq; P.awoff = A->d_woff; P.aclen = A->d_clen; P.aperm = A->d_perm;
   P.bseq = B->d_seq; P.bwoff = B->d_woff; P.bclen = B->d_clen; P.bperm = B->d_perm;
-  P.chain_break = chain_break; P.chain_min = chain_min;
   P.aln_min = align_min - 50; P.aln_rate = align_rate + .05;      // FastGA.c:3013-3014
   P.tspace = tspace; P.path_ave = ave_path;
-  P.self_mode = S->self_mode;
   P.dscore = -tables[0] / TRIM_LEN;                     // SCORE[0] = -15 * dscore
+  const long long chunk = chain_chunk_seeds();
 
   dblock<short> d_tables; dblock<u64> d_counters; dblock<unsigned> d_misc;
   CUDA_TRY(d_tables.alloc(65536,st));
@@ -2680,8 +2699,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
       std::vector<unsigned> wsize;
       int rc = extend_triples(P,S,d_misc,d_seg,d_work,wsize,st);
       if (rc) return rc;
-      if (!wsize.empty())
-        { rc = chain_detect(P,wsize,d_misc,d_hits,X,st);
+      if (!wsize.empty() && chunk > 0)
+        { rc = chain_detect(P,wsize,chunk,d_misc,d_hits,X,st);
           if (rc) return rc;
           P.hits = d_hits;
         }
@@ -2693,6 +2712,64 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   if (rc == FGB_OK) rc = collect_records(O.get(),R,P.nwork > 0,d_counters,st);
   if (rc) return rc;
   *out = O.release();                                        // (the device blocks go back as the call returns)
+  return FGB_OK;
+}
+
+//  Chain detection alone: phases 1 and 2 of fgb_extend at `chunk_seeds` merged seeds a chunk (0: none),
+//  read out per work triple and hit slot (include/fastga_b200.h)
+extern "C" int fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min, long long chunk_seeds,
+                              long long *trip, long long trip_cap, long long *hits, long long hits_cap,
+                              long long *info, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (chunk_seeds < 0 || trip_cap < 0 || hits_cap < 0) return FGB_ERR_ARG;
+  if (S->n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
+  for (int q = 0; q < 6; q++) info[q] = 0;
+  if (S->n == 0) return FGB_OK;
+  ext_params P;
+  seed_params(P,S,chain_break,chain_min);
+  dblock<unsigned> d_misc, d_seg, d_work; dblock<ChainHit> d_hits;
+  CUDA_TRY(d_misc.alloc(16,st));
+  CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
+  std::vector<unsigned> wsize;
+  int rc = extend_triples(P,S,d_misc,d_seg,d_work,wsize,st);
+  if (rc) return rc;
+  ExtendPlan X;
+  if (!wsize.empty() && chunk_seeds > 0)
+    { rc = chain_detect(P,wsize,chunk_seeds,d_misc,d_hits,X,st);
+      if (rc) return rc;
+    }
+  const long long nwork = P.nwork;
+  info[0] = nwork; info[1] = (long long) wsize.size(); info[2] = (long long) X.hused;
+  info[3] = (long long) X.hasked; info[4] = (long long) X.hit_cap; info[5] = X.nplan;
+  if (nwork > trip_cap || (long long) X.hused > hits_cap) return FGB_ERR_OVERFLOW;
+  //  the end of a triple: the next band segment too when it is the band above in the same group
+  //  (triple_setup), read from the seeds on the host
+  std::vector<unsigned> work((size_t) nwork), seg((size_t) P.nseg + 1);
+  std::vector<rec128> rec((size_t) S->n);
+  CUDA_TRY(cudaMemcpyAsync(work.data(),P.work,sizeof(unsigned)*work.size(),cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(seg.data(),P.seg_start,sizeof(unsigned)*seg.size(),cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(rec.data(),S->d_rec,sizeof(rec128)*rec.size(),cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  const int grp_bits = P.jc_bits + P.ic_bits + 1;
+  for (long long w = 0; w < nwork; w++)
+    { const unsigned j = work[(size_t) w];
+      const rec128 &r0 = rec[seg[j]];
+      unsigned e = seg[j+1];
+      if (j + 1 < (unsigned) P.nseg)
+        { const rec128 &r1 = rec[seg[j+1]];
+          if (get_bits(r1,P.p_jc,grp_bits) == get_bits(r0,P.p_jc,grp_bits) &&
+              get_bits(r1,P.p_band,P.band_bits) == get_bits(r0,P.p_band,P.band_bits) + 1)
+            e = seg[j+2];
+        }
+      const uint2 hr = X.hrange.empty() ? make_uint2(0u,0x80000000u) : X.hrange[(size_t) w];
+      const int2 ti = X.tinfo.empty() ? make_int2(-1,0) : X.tinfo[(size_t) w];
+      long long *t = trip + 7*w;
+      t[0] = seg[j]; t[1] = e; t[2] = (w < (long long) wsize.size()); t[3] = ti.x; t[4] = ti.y; t[5] = hr.x; t[6] = hr.y;
+    }
+  for (unsigned long long q = 0; q < X.hused; q++)
+    { const ChainHit &h = X.hh[(size_t) q];
+      hits[4*q] = h.alow; hits[4*q+1] = h.ahgh; hits[4*q+2] = h.dgmin; hits[4*q+3] = h.dgmax;
+    }
   return FGB_OK;
 }
 

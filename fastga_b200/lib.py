@@ -234,6 +234,15 @@ class DeviceSeeds:
         _check(L.fgb_seeds_find(gix1.h, gix2.h, amxpos, bmxpos, freq, C.byref(h), stream), "fgb_seeds_find")
         return cls(h)
 
+    @classmethod
+    def find_self(cls, gix, amxpos, freq=10, stream=None):
+        """SELF mode: the seeds of a genome's table against itself (gix from DeviceGix.build)"""
+        L = load_library()
+        h = c_void_p()
+        L.fgb_seeds_find_self.argtypes = [c_void_p, c_ll, c_int, C.POINTER(c_void_p), c_void_p]
+        _check(L.fgb_seeds_find_self(gix.h, amxpos, freq, C.byref(h), stream), "fgb_seeds_find_self")
+        return cls(h)
+
     @property
     def n(self):
         L = load_library()
@@ -565,6 +574,36 @@ def hit_groups_host(hrange, tinfo, hits, bands=1, slack=1000, gap=-1):
     L.fgb_hit_groups_host.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_ll, c_ll, c_void_p, c_void_p]
     n = L.fgb_hit_groups_host(len(hr), _ptr(hr), _ptr(ti), _ptr(hh), len(hh), bands, slack, gap, _ptr(items), _ptr(nxt))
     return items[:n].copy(), nxt[:n].copy()
+
+
+CHAIN_TRIPLE_DT = np.dtype([("start", "i8"), ("end", "i8"), ("long", "i8"), ("key", "i8"), ("band", "i8"),
+                            ("h0", "i8"), ("hn", "i8")])
+CHAIN_HIT_DT = np.dtype([("alow", "i8"), ("ahgh", "i8"), ("dgmin", "i8"), ("dgmax", "i8")])
+CHAIN_LISTLESS = 0x80000000
+
+
+def chain_hits(seeds, chain_break=2000, chain_min=170, chunk=None, stream=None):
+    """Chain detection alone (fgb_chain_hits): (triples, hits, info).  chunk: merged seeds per chunk (None:
+    fgb_extend's 1536; 0: no detection).  triples: the work triples in work order -- seeds [start, end),
+    long (scanned in chunks), (key, band) of the triple, its hit list hits[h0 : h0 + hn] unless hn has
+    bit 31 (CHAIN_LISTLESS: scanned in the extension kernel); hits: (alow, ahgh, dgmin, dgmax) per slot;
+    info: dict of the counts (work triples, long triples, hit slots, slots reserved, capacity, chunks)."""
+    L = load_library()
+    L.fgb_chain_hits.argtypes = [c_void_p, c_int, c_int, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p]
+    chunk = 1536 if chunk is None else int(chunk)
+    info = np.zeros(6, dtype=np.int64)
+    trip = np.zeros(1, dtype=CHAIN_TRIPLE_DT)
+    hits = np.zeros(1, dtype=CHAIN_HIT_DT)
+    for _ in range(2):
+        rc = L.fgb_chain_hits(seeds.h, chain_break, chain_min, chunk, _ptr(trip), len(trip), _ptr(hits), len(hits),
+                              _ptr(info), stream)
+        if rc != -4:
+            break
+        trip = np.zeros(max(int(info[0]), 1), dtype=CHAIN_TRIPLE_DT)
+        hits = np.zeros(max(int(info[2]), 1), dtype=CHAIN_HIT_DT)
+    _check(rc, "fgb_chain_hits")
+    names = ("work", "long", "slots", "reserved", "capacity", "chunks")
+    return trip[:int(info[0])].copy(), hits[:int(info[2])].copy(), dict(zip(names, (int(v) for v in info)))
 
 
 def device_free(ptr):

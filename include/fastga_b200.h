@@ -243,6 +243,21 @@ long long fgb_hit_groups_host(int nwork, const unsigned *hrange, const int *tinf
                               long long nhits, int bands, long long slack, long long gap,
                               unsigned *items_out, long long *next_out);
 
+/* ---- diagnostics: chain detection alone, the stage of fgb_extend before its first launch (band
+ *      segments, prefilter, chain_plan / chain_chunk / chain_stitch) on `stream`.  chunk_seeds: merged
+ *      seeds per chunk (fgb_extend: 1536, or FGB_CHAIN_CHUNK); 0 skips detection, as fgb_extend does past
+ *      2^20 long triples.  trip: 7 words per work triple, in work order: first seed, end of the triple
+ *      (seeds [first, end) of its two bands), 1 if long (scanned in chunks) else 0, (strand, contig pair)
+ *      key and band (-1, 0: not pre-scanned), first hit slot, hits | bit 31 (no list: scanned in the
+ *      extension kernel).  hits: 4 words per hit slot (alow, ahgh, dgmin, dgmax; anti-diagonals and
+ *      band-relative diagonals of the triple's seeds), indexed by a triple's (first hit slot, hits).
+ *      info: work triples, long triples, hit slots (what hits holds), slots the triples reserved, slot
+ *      capacity (a triple that reserves past it gets bit 31 too), chunks.  FGB_ERR_OVERFLOW with info set:
+ *      call again with trip_cap >= info[0] and hits_cap >= info[2]. ---- */
+int  fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min, long long chunk_seeds,
+                    long long *trip, long long trip_cap, long long *hits, long long hits_cap,
+                    long long *info /* 6 */, void *stream);
+
 /* ---- housekeeping ---- */
 int  fgb_device_ready(void);
 void fgb_release_cache(void);      /* return cached device blocks to the driver */

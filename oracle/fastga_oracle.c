@@ -8,7 +8,8 @@
  *   - orc_local_alignment   vs  Local_Alignment of libfastga_ref.so (align.c:1423) on the same
  *                               sequences / tubes, Path + trace bytes bit-exact
  *   - orc_gix_build         vs  the .gix/.ktab files written by oracle/_ref/GIXmake
- *   - orc_merge + orc_search vs the .1aln written by oracle/_ref/FastGA (through ONEview)
+ *   - orc_merge + orc_search vs the .1aln written by oracle/_ref/FastGA (through ONEview); orc_chains
+ *                               lists the chains of orc_search's own scan (one function serves both)
  *
  * Each function cites the reference lines it restates.  It is a restatement, not a copy: the two
  * wave routines of align.c are folded into one direction-normalised routine, M is derived from T
@@ -900,17 +901,22 @@ void orc_set_self(int on) { g_self = on; }
 /* aseq[c], bseq[c]: contig c (ORIGINAL numbering), one base per byte with a sentinel 4 at [-1]
    and [len]; acseq[c]: reverse complement of A contig c, same framing (Complement_Seq). */
 
-int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
-                   const orc_spec *spec, const int *perm1, const int *perm2,
-                   const char **aseq, const char **acseq, const int64_t *alens,
-                   const char **bseq, const int64_t *blens, orc_result *R)
+/*  The chain scan of every band-pair triple (FastGA.c:3087-3162), shared by orc_search, which
+    extends each chain, and orc_chains, which only lists them.  For every scanned triple tri() is
+    called first, then hit() for every chain that qualifies, in discovery order, with the values
+    the scan holds at the reference's hit count (FastGA.c:3160): anti-diagonals and band-relative
+    diagonals of the triple's own seeds, before any strand or offset adjustment -- the coordinates
+    of the device's ChainHit -- and the number of seeds of the chain.  */
+typedef struct
+  { int64_t b, m, e, cdiag; uint64_t key; int isnew; } orc_triple;
+
+typedef void (*orc_tri_fn)(void *ctx, const orc_triple *T);
+typedef void (*orc_hit_fn)(void *ctx, const orc_triple *T, int64_t alow, int64_t ahgh, int dgmin, int dgmax,
+                           int64_t nseed);
+
+static void chain_scan(const rec128 *seeds, int64_t n, const orc_layout *L, int chain_break, int chain_min,
+                       orc_tri_fn tri, orc_hit_fn hit, void *ctx)
 { int p_anti = 12, p_band = p_anti + L->anti_bits, p_jc = p_band + L->band_bits;
-  int p_ic = p_jc + L->jc_bits, p_cp = p_ic + L->ic_bits;
-  int64_t amxpos = L->amxpos, bmxpos = L->bmxpos, maxdag = amxpos + bmxpos;
-  int alnMin = P->align_min - 50;
-  double alnRate = P->align_rate + .05;
-  orc_work *work = orc_new_work();
-  orc_path path; memset(&path,0,sizeof(path));
   int64_t g0 = 0;
 
 #define ANTI(i) ((int64_t) get_bits(seeds+(i),p_anti,L->anti_bits))
@@ -921,13 +927,7 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
     { int64_t g1 = g0;
       uint64_t gk = GRP(g0);
       while (g1 < n && GRP(g1) == gk) g1 += 1;
-      { int comp = (int) get_bits(seeds+g0,p_cp,1);
-        int ctg1 = perm1[get_bits(seeds+g0,p_ic,L->ic_bits)];
-        int ctg2 = perm2[get_bits(seeds+g0,p_jc,L->jc_bits)];
-        int64_t alen = alens[ctg1], blen = blens[ctg2], mlen = alen+blen;
-        int64_t doffset = alen - maxdag, aoffset = alen - amxpos;
-        const char *as = comp ? acseq[ctg1] : aseq[ctg1];
-        const char *bs = bseq[ctg2];
+      { orc_triple T;
         int64_t b, m, e, cdiag;
         int     isnew, aux;
 
@@ -941,16 +941,17 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
 
             if (isnew || aux)
               { int     go, lcp, wch, mix, cov, dgmin, dgmax, dg;
-                int64_t ahgh, alow, amid, alast, anti, eant, ipost, apost, s, t;
+                int64_t ahgh, alow, anti, ipost, apost, s, t, nseed;
 
-                alast = -1;
+                T.b = b; T.m = m; T.e = e; T.cdiag = cdiag; T.key = gk; T.isnew = isnew;
+                tri(ctx,&T);
                 s = b; t = m;
                 ipost = ANTI(s);
                 apost = aux ? ANTI(t) : INT64_MAX;
                 dgmin = 2*BUCK_WIDTH; dgmax = 0;
-                ahgh  = -P->chain_break;
+                ahgh  = -chain_break;
                 alow  = (apost < ipost) ? apost : ipost;
-                cov = 0; go = 1; mix = 0;
+                cov = 0; go = 1; mix = 0; nseed = 0;
                 while (go)
                   { if (apost < ipost)
                       { lcp  = (int) get_bits(seeds+t,0,6);
@@ -977,7 +978,7 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
                       }
                     lcp <<= 1;
 
-                    if (anti < ahgh + P->chain_break)
+                    if (anti < ahgh + chain_break)
                       { int64_t cps = anti + lcp;
                         if (cps > ahgh)
                           { if (anti >= ahgh) cov += lcp; else cov += (int) (cps-ahgh);
@@ -985,65 +986,14 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
                           }
                         mix |= wch;
                         if (dg < dgmin) dgmin = dg; else if (dg > dgmax) dgmax = dg;
+                        nseed += 1;
                       }
                     else
-                      { if (cov >= P->chain_min && (mix != 1 || isnew))
-                          { R->nhit += 1;
-                            dgmin += (int) (cdiag<<BUCK_SHIFT);
-                            dgmax += (int) (cdiag<<BUCK_SHIFT);
-                            if (comp)
-                              { dgmin += (int) doffset; dgmax += (int) doffset;
-                                alow += aoffset; ahgh += aoffset;
-                              }
-                            else
-                              { dgmin -= (int) bmxpos; dgmax -= (int) bmxpos; }
-
-                            if (ahgh > alast)
-                              { if (alow < alast) alow = alast;
-                                ahgh -= BUCK_ANTI;
-                                do
-                                  { int rlen;
-                                    amid = alow + BUCK_ANTI;
-                                    if (amid > ahgh)
-                                      { amid = ahgh;
-                                        if (amid + dgmin < 0)
-                                          { dgmin = (int) -amid;
-                                            if (dgmin > dgmax) break;
-                                          }
-                                      }
-                                    if (g_self && ctg1 == ctg2 && !comp)
-                                      { if (dgmin > 0)
-                                          orc_local_alignment(work,spec,as,(int) alen,bs,(int) blen,comp,
-                                                              dgmin,dgmax,(int) amid,dgmin-1,-1,&path);
-                                        else if (dgmax < 0)
-                                          orc_local_alignment(work,spec,as,(int) alen,bs,(int) blen,comp,
-                                                              dgmin,dgmax,(int) amid,-1,-(dgmax+1),&path);
-                                        else
-                                          path.abpos = path.aepos = 0;
-                                      }
-                                    else
-                                      orc_local_alignment(work,spec,as,(int) alen,bs,(int) blen,comp,
-                                                          dgmin,dgmax,(int) amid,-1,-1,&path);
-                                    rlen = path.aepos - path.abpos;
-                                    if (rlen >= alnMin && alnRate*rlen >= path.diffs)
-                                      { orc_ovl o;
-                                        o.comp = comp; o.aread = ctg1; o.bread = ctg2;
-                                        o.abpos = path.abpos; o.bbpos = path.bbpos;
-                                        o.aepos = path.aepos; o.bepos = path.bepos;
-                                        o.diffs = path.diffs; o.tlen = path.tlen; o.toff = 0;
-                                        res_push(R,&o,path.trace);
-                                      }
-                                    if (comp) eant = mlen - (path.abpos + path.bbpos);
-                                    else      eant = path.aepos + path.bepos;
-                                    if (eant <= alow) alow = amid; else alow = eant;
-                                  }
-                                while (alow < ahgh);
-                                alast = alow;
-                              }
-                          }
+                      { if (cov >= chain_min && (mix != 1 || isnew))
+                          hit(ctx,&T,alow,ahgh,dgmin,dgmax,nseed);
                         if (go)
                           { cov = lcp; ahgh = anti + lcp; mix = wch; alow = anti;
-                            dgmin = dgmax = dg;
+                            dgmin = dgmax = dg; nseed = 1;
                           }
                       }
                   }
@@ -1065,7 +1015,143 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
 #undef ANTI
 #undef BAND
 #undef GRP
+}
+
+/*  orc_search: every chain goes through the tube stepping and Local_Alignment calls of
+    FastGA.c:3157-3340 as soon as the scan closes it; alast blocks within a triple.  */
+typedef struct
+  { const rec128 *seeds; const orc_layout *L; const orc_params *P; const orc_spec *spec;
+    const int *perm1, *perm2; const char **aseq, **acseq, **bseq; const int64_t *alens, *blens;
+    orc_result *R; orc_work *work; orc_path *path; int alnMin; double alnRate;
+    int comp, ctg1, ctg2; int64_t alen, blen, mlen, doffset, aoffset, alast; const char *as, *bs;
+  } search_ctx;
+
+static void search_triple(void *v, const orc_triple *T)
+{ search_ctx *S = (search_ctx *) v;
+  const orc_layout *L = S->L;
+  int p_jc = 12 + L->anti_bits + L->band_bits, p_ic = p_jc + L->jc_bits, p_cp = p_ic + L->ic_bits;
+  const rec128 *r = S->seeds + T->b;
+  S->comp = (int) get_bits(r,p_cp,1);
+  S->ctg1 = S->perm1[get_bits(r,p_ic,L->ic_bits)];
+  S->ctg2 = S->perm2[get_bits(r,p_jc,L->jc_bits)];
+  S->alen = S->alens[S->ctg1]; S->blen = S->blens[S->ctg2]; S->mlen = S->alen + S->blen;
+  S->doffset = S->alen - (L->amxpos + L->bmxpos); S->aoffset = S->alen - L->amxpos;
+  S->as = S->comp ? S->acseq[S->ctg1] : S->aseq[S->ctg1];
+  S->bs = S->bseq[S->ctg2];
+  S->alast = -1;
+}
+
+static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh, int dgmin, int dgmax,
+                       int64_t nseed)
+{ search_ctx *S = (search_ctx *) v;
+  orc_path *path = S->path;
+  int comp = S->comp, ctg1 = S->ctg1, ctg2 = S->ctg2, alen = (int) S->alen, blen = (int) S->blen;
+  int64_t amid, eant;
+  (void) nseed;
+  S->R->nhit += 1;
+  dgmin += (int) (T->cdiag<<BUCK_SHIFT);
+  dgmax += (int) (T->cdiag<<BUCK_SHIFT);
+  if (comp)
+    { dgmin += (int) S->doffset; dgmax += (int) S->doffset;
+      alow += S->aoffset; ahgh += S->aoffset;
+    }
+  else
+    { dgmin -= (int) S->L->bmxpos; dgmax -= (int) S->L->bmxpos; }
+
+  if (ahgh > S->alast)
+    { if (alow < S->alast) alow = S->alast;
+      ahgh -= BUCK_ANTI;
+      do
+        { int rlen;
+          amid = alow + BUCK_ANTI;
+          if (amid > ahgh)
+            { amid = ahgh;
+              if (amid + dgmin < 0)
+                { dgmin = (int) -amid;
+                  if (dgmin > dgmax) break;
+                }
+            }
+          if (g_self && ctg1 == ctg2 && !comp)
+            { if (dgmin > 0)
+                orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
+                                    dgmin,dgmax,(int) amid,dgmin-1,-1,path);
+              else if (dgmax < 0)
+                orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
+                                    dgmin,dgmax,(int) amid,-1,-(dgmax+1),path);
+              else
+                path->abpos = path->aepos = 0;
+            }
+          else
+            orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
+                                dgmin,dgmax,(int) amid,-1,-1,path);
+          rlen = path->aepos - path->abpos;
+          if (rlen >= S->alnMin && S->alnRate*rlen >= path->diffs)
+            { orc_ovl o;
+              o.comp = comp; o.aread = ctg1; o.bread = ctg2;
+              o.abpos = path->abpos; o.bbpos = path->bbpos;
+              o.aepos = path->aepos; o.bepos = path->bepos;
+              o.diffs = path->diffs; o.tlen = path->tlen; o.toff = 0;
+              res_push(S->R,&o,path->trace);
+            }
+          if (comp) eant = S->mlen - (path->abpos + path->bbpos);
+          else      eant = path->aepos + path->bepos;
+          if (eant <= alow) alow = amid; else alow = eant;
+        }
+      while (alow < ahgh);
+      S->alast = alow;
+    }
+}
+
+int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
+                   const orc_spec *spec, const int *perm1, const int *perm2,
+                   const char **aseq, const char **acseq, const int64_t *alens,
+                   const char **bseq, const int64_t *blens, orc_result *R)
+{ search_ctx S;
+  orc_path path; memset(&path,0,sizeof(path));
+  memset(&S,0,sizeof(S));
+  S.seeds = seeds; S.L = L; S.P = P; S.spec = spec; S.perm1 = perm1; S.perm2 = perm2;
+  S.aseq = aseq; S.acseq = acseq; S.bseq = bseq; S.alens = alens; S.blens = blens;
+  S.R = R; S.work = orc_new_work(); S.path = &path;
+  S.alnMin = P->align_min - 50;
+  S.alnRate = P->align_rate + .05;
+  chain_scan(seeds,n,L,P->chain_break,P->chain_min,search_triple,search_hit,&S);
   free(path.trace);
-  orc_free_work(work);
+  orc_free_work(S.work);
   return R->novl;
+}
+
+/*  orc_chains: the chains alone.  trip gets 8 words per scanned triple (b, m, e, isnew, (strand,
+    contig pair) key, cdiag, first hit, hits), hits 5 words per chain (alow, ahgh, dgmin, dgmax,
+    seeds); counts = (triples, chains).  With trip or hits NULL only the counts are made.  */
+typedef struct { int64_t *trip, *hits, ntrip, nhit; } chains_ctx;
+
+static void chains_triple(void *v, const orc_triple *T)
+{ chains_ctx *C = (chains_ctx *) v;
+  if (C->trip != NULL)
+    { int64_t *t = C->trip + 8*C->ntrip;
+      t[0] = T->b; t[1] = T->m; t[2] = T->e; t[3] = T->isnew; t[4] = (int64_t) T->key; t[5] = T->cdiag;
+      t[6] = C->nhit; t[7] = 0;
+    }
+  C->ntrip += 1;
+}
+
+static void chains_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh, int dgmin, int dgmax,
+                       int64_t nseed)
+{ chains_ctx *C = (chains_ctx *) v;
+  (void) T;
+  if (C->hits != NULL && C->trip != NULL)
+    { int64_t *h = C->hits + 5*C->nhit;
+      h[0] = alow; h[1] = ahgh; h[2] = dgmin; h[3] = dgmax; h[4] = nseed;
+      C->trip[8*(C->ntrip-1) + 7] += 1;
+    }
+  C->nhit += 1;
+}
+
+void orc_chains(const rec128 *seeds, int64_t n, const orc_layout *L, int chain_break, int chain_min,
+                int64_t *trip, int64_t *hits, int64_t *counts)
+{ chains_ctx C;
+  C.trip = trip; C.hits = hits; C.ntrip = 0; C.nhit = 0;
+  if (trip == NULL || hits == NULL) C.trip = C.hits = NULL;
+  chain_scan(seeds,n,L,chain_break,chain_min,chains_triple,chains_hit,&C);
+  counts[0] = C.ntrip; counts[1] = C.nhit;
 }

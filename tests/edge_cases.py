@@ -180,19 +180,46 @@ def max_contigs():
     return A, B, 8, lambda al, hits: len(al) > 100
 
 
+def chain_islands():
+    """one contig pair of 200 homologous islands of 100-130 bp between unrelated spacers of 1100-1500 bp,
+    equal in A and B (longer than chain_break / 2, so every island is a chain of its own).  An island of B
+    is its A island with every 18th base substituted: no indels, so all its seeds lie on one diagonal
+    inside one 64-wide band, and a substitution every 18 bases leaves about 15 seeds per chain.  So one
+    band-pair triple holds 180-odd chains in two chunks of chain detection, far more than the 48 a chunk
+    records, and is scanned in the extension kernel instead.  Eight more pairs, diverged copies with
+    indels, hold few chains each in band pairs of thousands of seeds."""
+    rng = np.random.default_rng(77)
+    a, b = [], []
+    for _ in range(200):
+        isl = rng.integers(0, 4, int(rng.integers(100, 131)), dtype=np.uint8)
+        sub = np.arange(len(isl)) % 18 == 17
+        mut = isl.copy()
+        mut[sub] = (mut[sub] + rng.integers(1, 4, int(sub.sum()))) % 4
+        n = int(rng.integers(1_100, 1_501))
+        a += [isl, rng.integers(0, 4, n, dtype=np.uint8)]
+        b += [mut, rng.integers(0, 4, n, dtype=np.uint8)]
+    A = [np.concatenate(a)] + [rng.integers(0, 4, int(rng.integers(40_000, 60_000)), dtype=np.uint8) for _ in range(8)]
+    B = [np.concatenate(b)] + [synth.diverged_copy(rng, c, 0.05, sv_every=0, inversions=False) for c in A[1:]]
+    return _distinct(A), _distinct(B), 4, lambda al, hits: hits >= 180 and len(al) >= 180
+
+
 CASES = {"ragged": ragged, "unrelated": unrelated, "identical_and_revcomp": identical_and_revcomp,
          "tandem_repeats": tandem_repeats, "many_small_contigs": many_small_contigs,
          "seed_key_64": seed_key_64, "seed_key_65": seed_key_65, "icont_straddles": icont_straddles,
-         "long_contigs": long_contigs, "long_and_many": long_and_many, "max_contigs": max_contigs}
+         "long_contigs": long_contigs, "long_and_many": long_and_many, "max_contigs": max_contigs,
+         "chain_islands": chain_islands}
 
 #  what each width case must reach: seed key bits, (post_bytes, cont_bytes) of A and of B, and for
-#  the long cases the least longest-contig length
+#  the long cases the least longest-contig length; chunk_overflow: a chunk of chain detection holds more
+#  chains than it records (tests/test_gpu_chains.py checks it)
 REGIMES = {"seed_key_64": dict(key=64, gixA=(3, 2), gixB=(3, 1)),
            "seed_key_65": dict(key=65, gixA=(3, 2), gixB=(3, 2)),
            "icont_straddles": dict(key=66, gixA=(3, 2), gixB=(3, 2)),
            "long_contigs": dict(key=63, gixA=(4, 1), gixB=(4, 1), maxlen=1 << 24),
            "long_and_many": dict(key=69, gixA=(4, 1), gixB=(4, 2), maxlen=1 << 24),
-           "max_contigs": dict(key=62, gixA=(2, 2), gixB=(2, 2), ncontigA=MAX_CONTIGS)}
+           "max_contigs": dict(key=62, gixA=(2, 2), gixB=(2, 2), ncontigA=MAX_CONTIGS),
+           # a chunk of chain detection with more than 48 chains: its triple has no hit list
+           "chain_islands": dict(key=55, gixA=(3, 1), gixB=(3, 1), chunk_overflow=True)}
 
 
 def reference_run(name):

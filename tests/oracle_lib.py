@@ -364,6 +364,32 @@ def search(recs, layout, gA, gB, perm1, perm2, freq, chain_break=2000, chain_min
     return ov, tp, nhit
 
 
+CHAIN_TRIPLE_DT = np.dtype([("b", "i8"), ("m", "i8"), ("e", "i8"), ("isnew", "i8"), ("key", "i8"), ("cdiag", "i8"),
+                            ("h0", "i8"), ("nh", "i8")])
+CHAIN_HIT_DT = np.dtype([("alow", "i8"), ("ahgh", "i8"), ("dgmin", "i8"), ("dgmax", "i8"), ("nseed", "i8")])
+
+
+def chains(recs, layout, chain_break=2000, chain_min=170):
+    """the oracle's chain scan alone (orc_chains, the scan orc_search extends from): (triples, hits).
+    triples: every scanned band-pair triple in scan order -- seeds [b, m) of band cdiag, [m, e) of band
+    cdiag + 1, isnew, (strand, contig pair) key, its chains hits[h0 : h0 + nh]; hits: every chain that
+    qualifies, in discovery order -- alow, ahgh, dgmin, dgmax as the scan holds them when it counts the
+    hit (the coordinates of the device's ChainHit) and the number of seeds of the chain."""
+    o = orc()
+    o.orc_chains.restype = None
+    recs = np.ascontiguousarray(recs, dtype=np.uint64)
+    L = OrcLayout(*layout)
+    counts = np.zeros(2, dtype=np.int64)
+    args = [recs.ctypes.data_as(C.c_void_p), C.c_int64(len(recs)), C.byref(L), C.c_int(chain_break),
+            C.c_int(chain_min)]
+    o.orc_chains(*args, None, None, counts.ctypes.data_as(C.c_void_p))
+    trip = np.zeros(int(counts[0]), dtype=CHAIN_TRIPLE_DT)
+    hits = np.zeros(int(counts[1]), dtype=CHAIN_HIT_DT)
+    o.orc_chains(*args, trip.ctypes.data_as(C.c_void_p), hits.ctypes.data_as(C.c_void_p),
+                 counts.ctypes.data_as(C.c_void_p))
+    return trip, hits
+
+
 def pack_overlaps(ov, tp, rank1, rank2, jb, ib):
     """oracle alignments (discovery order) -> the packed record buffer the device stage emits, so the
     product's host filter can be run on them"""
@@ -405,10 +431,12 @@ def oracle_pipeline(gA, gB, rank=None, **kw):
     recs = seed_records(seeds, layout)
     skw = {k: v for k, v in kw.items() if k in ("chain_break", "chain_min", "align_min", "align_rate")}
     ov, tp, nhit = search(recs, layout, gA, gB, pa, pb, gA.freq, **skw)
+    ckw = {k: v for k, v in skw.items() if k in ("chain_break", "chain_min")}
     O = pack_overlaps(ov, tp, ra, rb, layout[2], layout[3])
     al = lib.filter_overlaps(O.h, pa, pb, layout[2], layout[3])
     return dict(tabA=tA, tabB=tB, pstartA=sA, pstartB=sB, nseeds=len(seeds), sumlen=sumlen, seedrecs=recs,
-                nhit=nhit, nraw=len(ov), alns=al, lines=al.canonical_lines(), perm1=pa, perm2=pb)
+                nhit=nhit, nchain=len(chains(recs, layout, **ckw)[1]), nraw=len(ov), alns=al,
+                lines=al.canonical_lines(), perm1=pa, perm2=pb)
 
 
 def oracle_pipeline_self(g, **kw):

@@ -72,7 +72,8 @@ CASES = {
     "loose": (["-i.55", "-l50"], lambda: composed_pair(72, 350_000, 3, 0.18, 30_000),
               "ave_path 33: wide bands, the +.05 acceptance slack (slow on the CPU: kept small)"),
     "short_chains": (["-c20", "-s100"], lambda: composed_pair(73, 1_000_000, 3, 0.08, 50_000),
-                     "many chain breaks and hits per triple, the CH_HCAP overflow scan"),
+                     "many chain breaks and hits per triple (a dozen chains at most in one chunk of chain "
+                     "detection: the 48-chain overflow is edge_cases.chain_islands)"),
     "long_break": (["-c500", "-s20000"], lambda: composed_pair(74, 1_500_000, 3, 0.05, 20_000),
                    "chains bridging SV gaps, 13 seeds before a triple is scanned"),
     "freq3": (["-f3"], _tandem, "frequency cutoff 3 on tandem repeats"),

@@ -195,5 +195,7 @@ def test_edge_case_bit_exact_vs_reference(name):
     st = edge_cases.reference_run(name)
     alns, stats = lib.fastga(formats.genome_from_arrays(A), formats.genome_from_arrays(B))
     assert stats["nseeds"] == st.get("seeds", 0)
+    assert stats["nhits"] == st.get("hits", 0)
+    assert alns.nraw == st.get("alns", 0)
     assert len(alns) == st["records"] and ol.md5_lines(alns.canonical_lines()) == st["aln_md5"]
     check(alns, stats["nhits"])

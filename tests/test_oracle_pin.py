@@ -31,7 +31,7 @@ def test_oracle_reproduces_reference_golden(name):
     cnt = g["counters"]
     assert r["nseeds"] == cnt["seeds"]
     assert abs(r["sumlen"] / r["nseeds"] - cnt["avelen"]) < 0.051
-    assert r["nhit"] == cnt["hits"]
+    assert r["nhit"] == cnt["hits"] == r["nchain"]
     assert r["nraw"] == cnt["alns"]
     assert len(r["lines"]) == cnt["kept"] == g["aln_records"]
     assert r["lines"][:3] == g["first_records"]
@@ -204,6 +204,7 @@ def test_oracle_edge_cases_vs_live_reference(name):
     st = edge_cases.reference_run(name)
     r = ol.oracle_pipeline(formats.genome_from_arrays(A), formats.genome_from_arrays(B))
     assert r["nseeds"] == st.get("seeds", 0)
+    assert r["nhit"] == st.get("hits", 0) == r["nchain"] and r["nraw"] == st.get("alns", 0)
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
     check(r["alns"], r["nhit"])
 

@@ -164,6 +164,7 @@ def test_oracle_at_parameters_vs_reference(name):
     r = ol.oracle_pipeline(formats.genome_from_arrays(A), formats.genome_from_arrays(B), **pc.params(flags))
     assert (r["nseeds"], r["nhit"], r["nraw"], len(r["lines"])) == \
         (st.get("seeds", 0), st["hits"], st["alns"], st["kept"])
+    assert r["nchain"] == r["nhit"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
     assert st["records"] >= 5
 
