@@ -11,9 +11,10 @@
 // furthest point depends on its neighbour of the SAME wave -- so the unit of parallel work is one
 // THREAD per tile: millions of tiles, each a few thousand instructions.  A tile keeps its waves
 // (furthest B-index per diagonal, int16) and move codes (int8) in a private slab of HBM sized from
-// the tile's own difference count (the optimum never needs more waves than the trace point
-// recorded differences), reads the 2-bit staged contigs through L1, and leaves its indel positions
-// in a per-tile slot; the host strings the slots of an alignment together in order.
+// the tile's own recorded difference count, reads the 2-bit staged contigs through L1, and leaves
+// its indel positions in a per-tile slot; the host strings the slots of an alignment together in
+// order.  A tile whose recorded count understates its optimum runs once more with the record's
+// wave limit, the one Compute_Trace_PTS applies (see fgb_compute_trace_pts).
 //
 // What must be reproduced exactly (it decides WHERE an indel is placed among equal-cost scripts):
 // the order in which a wave is filled (above the end diagonal downwards, below it upwards, the end
@@ -29,7 +30,7 @@ struct TileJob                      // one trace-point tile
 { unsigned aln;                     // alignment it belongs to
   int a0, m;                        // A interval [a0,a0+m) in contig coordinates
   int b0, n;                        // B interval (complemented-B coordinates for strand C)
-  int dcap;                         // waves available: recorded differences - |m-n|
+  int dcap;                         // waves available: recorded differences - |m-n|, or the record's limit
   unsigned out;                     // first slot of its script entries
   u64 slab;                         // byte offset of its wave slab
 };
@@ -149,11 +150,53 @@ extern "C" int fgb_scripts_get(const fgb_scripts *s, long long *soff, int *scrip
   return FGB_OK;
 }
 
+//  Place a tile with `dcap` waves at the end of a launch's slab and script slots.
+static void tile_layout(TileJob &J, int dcap, u64 &slab, unsigned long long &slots)
+{ int del = J.m - J.n; if (del < 0) del = -del;
+  J.dcap = dcap;
+  J.out = (unsigned) slots; J.slab = slab;
+  slots += (unsigned long long) (dcap + del);
+  slab += tile_slab_bytes(J.m,J.n,dcap);
+}
+
+//  One launch of trace_tiles_kernel over `jobs`, whose slabs and slots tile_layout placed from 0:
+//  per tile its script entry count (-1: more than dcap waves needed), its differences and its slots.
+static int run_tiles(const fgb_genome *A, const fgb_genome *B, const std::vector<TileJob> &jobs, u64 slab,
+                     unsigned long long slots, const AlnSeq *d_seqs, const unsigned char *d_comp,
+                     std::vector<int> &cnt, std::vector<int> &td, std::vector<int> &scr, cudaStream_t st)
+{ if (slots >= 0xfffffff0ull || jobs.size() >= 0x7ffffff0ull) return FGB_ERR_LIMIT;
+  const int nj = (int) jobs.size();
+  dblock<TileJob> d_jobs; dblock<unsigned char> d_slab;
+  dblock<int> d_script, d_count, d_td;
+  cnt.resize(nj); td.resize(nj); scr.resize((size_t) slots + 1);
+  CUDA_TRY(d_jobs.alloc((size_t) nj,st));
+  CUDA_TRY(d_slab.alloc((size_t) slab + 16,st));
+  CUDA_TRY(d_script.alloc((size_t) slots + 1,st));
+  CUDA_TRY(d_count.alloc((size_t) nj,st));
+  CUDA_TRY(d_td.alloc((size_t) nj,st));
+  CUDA_TRY(cudaMemcpyAsync(d_jobs,jobs.data(),sizeof(TileJob)*(size_t) nj,cudaMemcpyHostToDevice,st));
+  trace_tiles_kernel<<<(nj + 127)/128,128,0,st>>>(d_jobs,nj,d_seqs,A->d_seq,B->d_seq,B->d_rseq,d_comp,d_slab,
+                                                  d_script,d_count,d_td);
+  fgb_count_launch(1);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(cudaMemcpyAsync(cnt.data(),d_count,sizeof(int)*(size_t) nj,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(td.data(),d_td,sizeof(int)*(size_t) nj,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(scr.data(),d_script,sizeof(int)*(size_t) slots,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  return FGB_OK;
+}
+
 //  fields / toff / pool: alignments as fgb_alns_get returns them (n x 9 ints: comp aread bread abpos
 //  bbpos aepos bepos diffs tlen; B coordinates of strand-C records in complemented B, as in the
 //  .1aln).  B must have been created with its reverse complement when any record is strand C.
 //  The script of alignment i is script[soff[i] .. soff[i+1]): what Compute_Trace_PTS leaves in
 //  path->trace (align.h:330-349), diffs[i] what it leaves in path->diffs (-1: bad trace points).
+//
+//  Compute_Trace_PTS gives every tile of a record the same wave limit: the record's largest tile
+//  difference count rounded up to even (0 when tlen < 2, align.c:6210-6221).  A tile here first gets
+//  only its own recorded count, which keeps its slab small and is always enough when the record is
+//  consistent; the tiles that run out are launched once more with the record's limit, and a record
+//  is bad exactly when one of its tiles runs out of that too.
 extern "C" int fgb_compute_trace_pts(const fgb_genome *A, const fgb_genome *B, long long n, const int *fields,
                                      const long long *toff, const unsigned char *pool, int tspace,
                                      fgb_scripts **out, void *stream)
@@ -168,6 +211,7 @@ extern "C" int fgb_compute_trace_pts(const fgb_genome *A, const fgb_genome *B, l
   std::vector<TileJob> jobs;
   std::vector<AlnSeq> seqs(n);
   std::vector<unsigned char> comp(n);
+  std::vector<int> dmax(n);                     // the wave limit Compute_Trace_PTS gives every tile
   std::vector<long long> first(n+1);            // first tile of every alignment
   u64 slab = 0; unsigned long long slots = 0;
   for (long long i = 0; i < n; i++)
@@ -181,49 +225,63 @@ extern "C" int fgb_compute_trace_pts(const fgb_genome *A, const fgb_genome *B, l
       seqs[i].alen = (int) A->clen[ar]; seqs[i].blen = (int) B->clen[br];
       first[i] = (long long) jobs.size();
       const int ntile = tlen >= 2 ? tlen/2 : 1;
+      dmax[i] = 0;
+      for (int t = 0; t < ntile && tlen >= 2; t++)
+        if (tr[2*t] > dmax[i]) dmax[i] = tr[2*t];
+      dmax[i] += dmax[i] & 1;
       int a = f[3], b = f[4];
       for (int t = 0; t < ntile; t++)
         { const bool last = (t == ntile-1);
           const int ae = last ? f[5] : (f[3]/tspace)*tspace + (t+1)*tspace;
           const int be = last ? f[6] : b + tr[2*t+1];
-          const int d  = tlen >= 2 ? tr[2*t] : f[7];
+          const int d  = tlen >= 2 ? tr[2*t] : 0;
           TileJob J;
           J.aln = (unsigned) i; J.a0 = a; J.m = ae - a; J.b0 = b; J.n = be - b;
           if (J.m < 0 || J.n < 0 || ae > seqs[i].alen || be > seqs[i].blen) return FGB_ERR_ARG;
+          if (J.m > 32767 || J.n > 32767) return FGB_ERR_LIMIT;     // furthest points are int16
           int del = J.m - J.n; if (del < 0) del = -del;
-          J.dcap = d > del ? d - del : 0;
-          J.out = (unsigned) slots; J.slab = slab;
-          slots += (unsigned long long) (J.dcap + del);
-          slab += tile_slab_bytes(J.m,J.n,J.dcap);
+          tile_layout(J,d > del ? d - del : 0,slab,slots);
           jobs.push_back(J);
           a = ae; b = be;
         }
     }
   first[n] = (long long) jobs.size();
-  if (slots >= 0xfffffff0ull || jobs.size() >= 0x7ffffff0ull) return FGB_ERR_LIMIT;
 
   const int nj = (int) jobs.size();
-  dblock<TileJob> d_jobs; dblock<AlnSeq> d_seqs; dblock<unsigned char> d_comp, d_slab;
-  dblock<int> d_script, d_count, d_td;
-  std::vector<int> cnt(nj), td(nj), scr((size_t) slots + 1);
-  CUDA_TRY(d_jobs.alloc((size_t) nj,st));
+  dblock<AlnSeq> d_seqs; dblock<unsigned char> d_comp;
+  std::vector<int> cnt, td, scr;
   CUDA_TRY(d_seqs.alloc((size_t) n,st));
   CUDA_TRY(d_comp.alloc((size_t) n,st));
-  CUDA_TRY(d_slab.alloc((size_t) slab + 16,st));
-  CUDA_TRY(d_script.alloc((size_t) slots + 1,st));
-  CUDA_TRY(d_count.alloc((size_t) nj,st));
-  CUDA_TRY(d_td.alloc((size_t) nj,st));
-  CUDA_TRY(cudaMemcpyAsync(d_jobs,jobs.data(),sizeof(TileJob)*(size_t) nj,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_seqs,seqs.data(),sizeof(AlnSeq)*(size_t) n,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_comp,comp.data(),(size_t) n,cudaMemcpyHostToDevice,st));
-  trace_tiles_kernel<<<(nj + 127)/128,128,0,st>>>(d_jobs,nj,d_seqs,A->d_seq,B->d_seq,B->d_rseq,d_comp,d_slab,
-                                                  d_script,d_count,d_td);
-  fgb_count_launch(1);
-  CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(cnt.data(),d_count,sizeof(int)*(size_t) nj,cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaMemcpyAsync(td.data(),d_td,sizeof(int)*(size_t) nj,cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaMemcpyAsync(scr.data(),d_script,sizeof(int)*(size_t) slots,cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaStreamSynchronize(st));
+  int rc = run_tiles(A,B,jobs,slab,slots,d_seqs,d_comp,cnt,td,scr,st);
+  if (rc) return rc;
+  std::vector<size_t> from(nj);                 // where each tile's entries are in scr
+  for (int t = 0; t < nj; t++) from[t] = jobs[t].out;
+
+  //  the tiles that ran out of their own count, again with the record's limit
+  std::vector<TileJob> again;
+  std::vector<int> which;
+  u64 slab2 = 0; unsigned long long slots2 = 0;
+  for (int t = 0; t < nj; t++)
+    if (cnt[t] < 0 && dmax[jobs[t].aln] > jobs[t].dcap)
+      { TileJob J = jobs[t];
+        tile_layout(J,dmax[J.aln],slab2,slots2);
+        again.push_back(J);
+        which.push_back(t);
+      }
+  if (!again.empty())
+    { std::vector<int> cnt2, td2, scr2;
+      rc = run_tiles(A,B,again,slab2,slots2,d_seqs,d_comp,cnt2,td2,scr2,st);
+      if (rc) return rc;
+      const size_t base = scr.size();
+      scr.insert(scr.end(),scr2.begin(),scr2.end());
+      for (size_t r = 0; r < again.size(); r++)
+        { const int t = which[r];
+          cnt[t] = cnt2[r]; td[t] = td2[r]; from[t] = base + again[r].out;
+        }
+    }
+
   //  string the tiles of every alignment together
   R->script.reserve((size_t) slots);
   for (long long i = 0; i < n; i++)
@@ -231,7 +289,7 @@ extern "C" int fgb_compute_trace_pts(const fgb_genome *A, const fgb_genome *B, l
       R->soff[i] = (long long) R->script.size();
       for (long long t = first[i]; t < first[i+1]; t++)
         { if (cnt[t] < 0) { bad = true; break; }
-          R->script.insert(R->script.end(),scr.begin() + jobs[t].out,scr.begin() + jobs[t].out + cnt[t]);
+          R->script.insert(R->script.end(),scr.begin() + from[t],scr.begin() + from[t] + cnt[t]);
           diffs += td[t];
         }
       if (bad) { R->script.resize((size_t) R->soff[i]); diffs = -1; R->bad += 1; }

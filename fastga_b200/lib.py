@@ -529,11 +529,12 @@ def fastga(gA, gB, stream=None, **kw):
     return _alns_out(h), st.asdict()
 
 
-def compute_trace_pts(dA, dB, alns, tspace=100, stream=None):
+def compute_trace_pts(dA, dB, alns, tspace=100, stream=None, with_bad=False):
     """Compute_Trace_PTS for every alignment of `alns` (an Alignments): returns (soff, script, diffs) --
     script[soff[i]:soff[i+1]] is the edit script the reference leaves in path->trace, diffs[i] its
-    path->diffs (-1: trace points inconsistent with the sequences).  dB needs want_revcomp=True when
-    strand-C records are present."""
+    path->diffs (-1: trace points inconsistent with the sequences).  with_bad: (soff, script, diffs,
+    bad), bad the library's count of such alignments (fgb_scripts_bad).  dB needs want_revcomp=True
+    when strand-C records are present."""
     L = load_library()
     h = c_void_p()
     fields = np.ascontiguousarray(alns.fields, dtype=np.int32)
@@ -551,9 +552,12 @@ def compute_trace_pts(dA, dB, alns, tspace=100, stream=None):
     diffs = np.zeros(max(n, 1), dtype=np.int32)
     L.fgb_scripts_get.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
     _check(L.fgb_scripts_get(h, _ptr(soff), _ptr(script), _ptr(diffs)), "fgb_scripts_get")
+    L.fgb_scripts_bad.restype = c_ll
+    L.fgb_scripts_bad.argtypes = [c_void_p]
+    bad = L.fgb_scripts_bad(h)
     L.fgb_scripts_free.argtypes = [c_void_p]
     L.fgb_scripts_free(h)
-    return soff, script[:tot], diffs[:n]
+    return (soff, script[:tot], diffs[:n]) + ((bad,) if with_bad else ())
 
 
 # ---- building blocks of the k-mer-space sharded path (several GPUs; orchestrated by shard.py) ----

@@ -204,6 +204,61 @@ def ref_local_alignments(calls, freq, ave_corr=0.7):
     return out
 
 
+def script_key(script, diffs):
+    """short digest of one edit script (int entries as Compute_Trace_PTS leaves them) and its diffs"""
+    return hashlib.md5(np.asarray(script, dtype=np.int32).tobytes() + b"%d" % diffs).hexdigest()[:12]
+
+
+_ref_trace = None
+
+
+def _ref_trace_lib():
+    """libfastga_ref.so with its Error_Buffer pointed at a buffer, so that a record the reference rejects
+    makes the call return 1 instead of exiting the process; plus one Work_Data for every call"""
+    global _ref_trace
+    if _ref_trace is None:
+        ref = C.CDLL(REF_SO)
+        buf = C.create_string_buffer(1 << 16)
+        C.c_void_p.in_dll(ref, "Error_Buffer").value = C.addressof(buf)
+        ref.New_Work_Data.restype = C.c_void_p
+        ref.Compute_Trace_PTS.argtypes = [C.POINTER(Alignment), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
+        _ref_trace = (ref, buf, ref.New_Work_Data())
+    return _ref_trace
+
+
+def ref_trace_pts_raw(records, gA, gB):
+    """Compute_Trace_PTS(aln, work, 100, GREEDIEST, 1, -1) on every record of `records` (fields (n, 9),
+    toff and pool as lib.Alignments holds them) as ALNtoPAF.c:251-278 calls it: A and B in separate
+    buffers (so the band is unbounded), strand-C records against the complement of their B contig.
+    Per record (script, diffs), or None where the reference rejects the trace points."""
+    ref, _, work = _ref_trace_lib()
+    A, B, BC = {}, {}, {}
+    out = []
+    for i in range(len(records)):
+        comp, ar, br, ab, bb, ae, be, df, tl = (int(x) for x in records.fields[i])
+        if ar not in A:
+            A[ar] = _framed(gA.contig(ar))
+        if comp and br not in BC:
+            BC[br] = _framed(3 - gB.contig(br)[::-1])
+        elif not comp and br not in B:
+            B[br] = _framed(gB.contig(br))
+        pts = records.pool[int(records.toff[i]):int(records.toff[i]) + tl].astype(np.uint16)  # Decompress_TraceTo16
+        p = Path(pts.ctypes.data, tl, df, ab, bb, ae, be)
+        a, b = A[ar], (BC[br] if comp else B[br])
+        al = Alignment(C.pointer(p), 2 if comp else 0, a.ctypes.data + 1, b.ctypes.data + 1, len(a) - 2, len(b) - 2)
+        if ref.Compute_Trace_PTS(C.byref(al), work, 100, 0, 1, -1) != 0:
+            out.append(None)
+            continue
+        sc = np.ctypeslib.as_array(C.cast(p.trace, C.POINTER(C.c_int32)), shape=(max(p.tlen, 1),))[:p.tlen].copy()
+        out.append((sc, p.diffs))
+    return out
+
+
+def ref_trace_pts(records, gA, gB):
+    """ref_trace_pts_raw as JSON data: per record script_key(script, diffs), or "fail" """
+    return [("fail" if r is None else script_key(*r)) for r in ref_trace_pts_raw(records, gA, gB)]
+
+
 def ref_env():
     env = dict(os.environ)
     env["PATH"] = REF_DIR + os.pathsep + env.get("PATH", "")

@@ -2,7 +2,6 @@
 UNMODIFIED reference's Compute_Trace_PTS (oracle/_ref/libfastga_ref.so; its results stored in
 tests/golden/reference_runs.json) on the alignments the path emits: same int script, same diffs,
 for every record."""
-import ctypes as C
 import hashlib
 
 import numpy as np
@@ -19,33 +18,6 @@ def _aln_key(alns, i):
     return hashlib.md5(alns.fields[i].astype(np.int32).tobytes() + alns.trace(i).tobytes()).hexdigest()[:12]
 
 
-def _script_key(script, diffs):
-    return hashlib.md5(np.asarray(script, dtype=np.int32).tobytes() + b"%d" % diffs).hexdigest()[:12]
-
-
-def _reference_scripts(gA, gB, alns, limit=None):
-    """Compute_Trace_PTS(aln, work, 100, GREEDIEST, 1, -1) as ALNtoPAF.c:251-272 calls it"""
-    ref = C.CDLL(ol.REF_SO)
-    ref.New_Work_Data.restype = C.c_void_p
-    ref.Compute_Trace_PTS.argtypes = [C.POINTER(ol.Alignment), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int]
-    work = ref.New_Work_Data()
-    A = [ol._framed(gA.contig(c)) for c in range(gA.ncontig)]
-    B = [ol._framed(gB.contig(c)) for c in range(gB.ncontig)]
-    BC = [ol._framed(3 - gB.contig(c)[::-1]) for c in range(gB.ncontig)]
-    out = []
-    n = len(alns) if limit is None else min(limit, len(alns))
-    for i in range(n):
-        comp, ar, br, ab, bb, ae, be, df, tl = (int(x) for x in alns.fields[i])
-        pts = alns.trace(i).astype(np.uint16)            # Decompress_TraceTo16
-        p = ol.Path(pts.ctypes.data, tl, df, ab, bb, ae, be)
-        a, b = A[ar], (BC[br] if comp else B[br])
-        al = ol.Alignment(C.pointer(p), 2 if comp else 0, a.ctypes.data + 1, b.ctypes.data + 1, len(a) - 2, len(b) - 2)
-        assert ref.Compute_Trace_PTS(C.byref(al), work, 100, 0, 1, -1) == 0
-        sc = np.ctypeslib.as_array(C.cast(p.trace, C.POINTER(C.c_int32)), shape=(max(p.tlen, 1),))[:p.tlen].copy()
-        out.append((sc, p.diffs))
-    return out
-
-
 def _check_pair(name, seed, total, ncontig, div, sv, flip=()):
     A, B = synth.make_pair(seed, total, ncontig, div, sv_every=sv)
     for i in flip:                                   # whole contigs on the opposite strand
@@ -60,8 +32,7 @@ def reference_scripts(name, A, B):
 
     def run():
         ralns = ol.oracle_pipeline(gA, gB)["alns"]
-        return {_aln_key(ralns, i): _script_key(sc, df)
-                for i, (sc, df) in enumerate(_reference_scripts(gA, gB, ralns))}
+        return {_aln_key(ralns, i): key for i, key in enumerate(ol.ref_trace_pts(ralns, gA, gB))}
     return ol.reference("trace_pts/" + name, ol.digest(A, B), run)
 
 
@@ -71,12 +42,12 @@ def _check_contigs(name, A, B):
     alns, _ = lib.fastga(gA, gB)
     assert len(alns) > 0 and len(alns) == len(want)
     dA, dB = lib.DeviceGenome(gA), lib.DeviceGenome(gB, want_revcomp=True)
-    soff, script, diffs = lib.compute_trace_pts(dA, dB, alns)
-    assert (diffs >= 0).all()
+    soff, script, diffs, bad = lib.compute_trace_pts(dA, dB, alns, with_bad=True)
+    assert (diffs >= 0).all() and bad == 0
     ncomp = 0
     for i in range(len(alns)):
         got = script[soff[i]:soff[i + 1]]
-        assert _script_key(got, int(diffs[i])) == want[_aln_key(alns, i)], (i, got[:8], int(diffs[i]))
+        assert ol.script_key(got, int(diffs[i])) == want[_aln_key(alns, i)], (i, got[:8], int(diffs[i]))
         ncomp += int(alns.fields[i, 0])
     return len(alns), ncomp, alns
 
@@ -99,16 +70,31 @@ def test_scripts_match_reference_past_2_24():
     assert past.any() and 0 < int(alns.fields[past, 0].sum()) < int(past.sum())
 
 
+def _understate(alns):
+    """the longest record with zero differences claimed for three of its tiles that have some"""
+    i = int(np.argmax(alns.fields[:, 8]))
+    for k in (2, 4, 6):
+        alns.pool[int(alns.toff[i]) + k] = 0
+    return i
+
+
 def test_inconsistent_trace_points_are_flagged_not_fatal():
+    """Understated tile counts do not make a record bad by themselves: the reference gives every tile
+    the record's largest count as its wave limit (align.c:6210-6221), so it still computes this
+    record's script, and so must the device."""
     A, B = synth.make_pair(23, 600_000, 2, 0.05, sv_every=50_000)
     gA, gB = formats.genome_from_arrays(A), formats.genome_from_arrays(B)
+
+    def run():
+        ralns = ol.oracle_pipeline(gA, gB)["alns"]
+        i = _understate(ralns)
+        return dict(record=_aln_key(ralns, i), script=ol.ref_trace_pts(ralns, gA, gB)[i])
+    want = ol.reference("trace_pts/understated_tiles", ol.digest(A, B), run)
+    assert want["script"] != "fail"
     alns, _ = lib.fastga(gA, gB)
+    i = _understate(alns)
+    assert _aln_key(alns, i) == want["record"]
     dA, dB = lib.DeviceGenome(gA), lib.DeviceGenome(gB, want_revcomp=True)
-    i = int(np.argmax(alns.fields[:, 8]))
-    alns.pool[int(alns.toff[i]) + 2] = 0          # claim zero differences in a tile that has some
-    alns.pool[int(alns.toff[i]) + 4] = 0
-    alns.pool[int(alns.toff[i]) + 6] = 0
-    soff, script, diffs = lib.compute_trace_pts(dA, dB, alns)
-    good = [k for k in range(len(alns)) if k != i]
-    assert (diffs[good] >= 0).all()
-    assert diffs[i] == -1 or diffs[i] >= 0        # only flagged when a tile really cannot be aligned
+    soff, script, diffs, bad = lib.compute_trace_pts(dA, dB, alns, with_bad=True)
+    assert bad == 0 and (diffs >= 0).all()
+    assert ol.script_key(script[soff[i]:soff[i + 1]], int(diffs[i])) == want["script"]
