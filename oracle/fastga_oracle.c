@@ -431,6 +431,48 @@ int orc_align_spec(double ave_corr, const float *freq, int16_t *tables, int *ave
   return 0;
 }
 
+/*  What one wave pass went through (orc_search_calls): the regimes a device wave routine branches on.
+    Coordinates are the pass's own (direction-normalised); `call` is the Local_Alignment call's number.  */
+typedef struct
+  { int call, s;
+    int waves;                   /* waves after wave 0 */
+    int maxband;                 /* widest band a wave ran over (hghk-lowk+1 after the band grew) */
+    int narrowspan;              /* most A bases the best point advanced over consecutive waves of <= 17 diagonals */
+    int maxsnake;                /* longest slide of one diagonal in one wave after wave 0 */
+    int aend, bend;              /* a slide met the end of A (ca == 4) / of B (cb == 4) */
+    int stall;                   /* a wave after wave 0 did not raise besta: never, see wave() */
+    int endempty;                /* a wave stopped by a contig end left no diagonal after the end clip and trim */
+    int aspan;                   /* A bases from the start point to the trim point */
+    int da0, da1, db0, db1;      /* the start point's distance to A's start, A's end, B's start, B's end */
+    int maxhop;                  /* largest cell-index gap between consecutive pebbles of the read-out path */
+  } orc_pass;
+
+/*  Every Local_Alignment call of orc_search_calls in discovery order: its arguments (original contig
+    numbers), whether it produced a record, its path (trace bytes at toff in tpool), its passes.  */
+typedef struct
+  { int comp, ctg1, ctg2, low, hgh, anti, lbord, hbord, rec;
+    int abpos, bbpos, aepos, bepos, diffs, tlen, pass0, npass, pad;
+    int64_t toff;
+  } orc_call;
+
+typedef struct
+  { orc_call *call; int64_t ncall, maxcall;
+    uint8_t  *tpool; int64_t tlen, tmax;
+    orc_pass *pass; int64_t npass, maxpass;
+  } orc_calllog;
+
+static orc_pass *pass_new(orc_calllog *g)
+{ if (g == NULL) return NULL;
+  if (g->npass >= g->maxpass)
+    { g->maxpass = g->maxpass*2 + 256;
+      g->pass = (orc_pass *) realloc(g->pass,sizeof(orc_pass)*g->maxpass);
+    }
+  orc_pass *p = g->pass + g->npass++;
+  memset(p,0,sizeof(orc_pass));
+  p->call = (int) g->ncall;
+  return p;
+}
+
 typedef struct
   { const char *aseq, *bseq;     /* one base per byte, sentinel 4 at [-1] and [len] */
     int   alen, blen;
@@ -439,6 +481,7 @@ typedef struct
     uint64_t *T;
     Peb  *cells;
     int   cmax, avail;
+    orc_calllog *log;            /* NULL, or where orc_local_alignment records its passes */
   } orc_work;
 
 static inline int a_at(const orc_work *w, int s, int xn)
@@ -485,13 +528,14 @@ typedef struct
 #define IX(k) ((k) & Wm)
 
 static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int mida,
-                 int minp, int maxp, int aoff, wave_out *out)
+                 int minp, int maxp, int aoff, wave_out *out, orc_pass *st)
 { int tspace = spec->tspace, PATH_AVE = spec->path_ave;
   const int16_t *SCORE = spec->score, *TABLE = spec->table;
   int FRESH = (s > 0) ? -1 : -INT32_MAX;
   int lowk, hghk, minpn, maxpn, dif;
   int besta, bestx, lasta, trima, trimx, trimd, trimha;
   int more, aclip, bclip, Wm, kk;
+  int nx0 = 0, nrun = 0;                               /* pass statistics: start of the current narrow stretch */
 
   if (s > 0) { lowk = low;  hghk = hgh;  minpn = minp;  maxpn = maxp; }
   else       { lowk = -hgh; hghk = -low; minpn = -maxp; maxpn = -minp; }
@@ -506,6 +550,12 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
   besta = trima = lasta = s*mida;
   bestx = trimx = s*((mida+hgh)>>1);
   trimd = 0; trimha = 0;
+  if (st != NULL)
+    { int xm = (mida + ((low+hgh)>>1))>>1, ym = mida - xm;
+      st->s = s;
+      st->da0 = xm; st->da1 = w->alen - xm; st->db0 = ym; st->db1 = w->blen - ym;
+      st->maxband = hghk - lowk + 1;
+    }
 
   for (kk = hghk; kk >= lowk; kk--)                    /* wave 0 (align.c:426-507 / :956-1036) */
     { int k = s*kk, x = (mida+k)>>1, xn, na, nan, ha, c;
@@ -525,11 +575,12 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
           if (cb == 4)
             { more = 0;
               if (bclip < kk) bclip = kk;
+              if (st != NULL) st->bend = 1;
               break;
             }
           ca = a_at(w,s,xn);
           if (cb != ca)
-            { if (ca == 4) { more = 0; aclip = kk; }
+            { if (ca == 4) { more = 0; aclip = kk; if (st != NULL) st->aend = 1; }
               break;
             }
           xn += 1;
@@ -555,7 +606,7 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
     }
 
   while (more && lasta >= besta - TRIM_MLAG)           /* align.c:546-800 / :1077-1330 */
-    { int am, ac, ap, ua, n;
+    { int am, ac, ap, ua, n, besta0 = besta;
       uint64_t t;
 
       grow_state(w,lowk-1,hghk+1);
@@ -571,6 +622,16 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
       else
         hghk -= 1;
       dif += 1;
+      if (st != NULL)
+        { st->waves += 1;
+          if (hghk - lowk + 1 > st->maxband) st->maxband = hghk - lowk + 1;
+          if (hghk - lowk + 1 > 17)
+            nrun = 0;
+          else
+            { if (!nrun) { nrun = 1; nx0 = bestx; }
+              if (bestx - nx0 > st->narrowspan) st->narrowspan = bestx - nx0;
+            }
+        }
 
       w->V[IX(hghk+1)] = w->V[IX(lowk-1)] = FRESH;
       ac = FRESH;
@@ -578,7 +639,7 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
       t  = PATH_INT;
       ua = -1;
       for (kk = hghk; kk >= lowk; kk--)
-        { int xn, c, ha, k = s*kk;
+        { int xn, x0, c, ha, k = s*kk;
           uint64_t b;
 
           ap = ac; ac = am; am = w->V[IX(kk-1)];
@@ -591,22 +652,24 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
               else         { c = ac+2; b = w->T[IX(kk)]; ha = w->HA[IX(kk)]; }
             }
           b <<= 1;
-          xn = (c+kk)>>1;
+          xn = x0 = (c+kk)>>1;
           while (1)
             { int cb = b_at(w,s,xn-kk), ca;
               if (cb == 4)
                 { more = 0;
                   if (bclip < kk) bclip = kk;
+                  if (st != NULL) st->bend = 1;
                   break;
                 }
               ca = a_at(w,s,xn);
               if (cb != ca)
-                { if (ca == 4) { more = 0; aclip = kk; }
+                { if (ca == 4) { more = 0; aclip = kk; if (st != NULL) st->aend = 1; }
                   break;
                 }
               xn += 1;
               b = (b << 1) | 1;
             }
+          if (st != NULL && xn - x0 > st->maxsnake) st->maxsnake = xn - x0;
           c = 2*xn - kk;
 
           while (xn >= w->NA[IX(kk)])
@@ -630,6 +693,12 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
           w->V[IX(kk)] = c; w->T[IX(kk)] = b; w->HA[IX(kk)] = ha;
         }
 
+      /* besta cannot stall: the diagonal holding it gains at least 2 each wave while it is in the band, the
+         WAVE_LAG trim never drops it, and an end clip drops it only when it slid into that end itself (a
+         diagonal at or above aclip with as large a value lies as far along A; at or below bclip, along B),
+         which leaves more == 0.  The device's "no advance" bail-out is reached the other way: the wave
+         that meets an end leaves no diagonal within WAVE_LAG once the clipped ones are gone (endempty). */
+      if (st != NULL && besta == besta0) st->stall = 1;
       if (more == 0)
         { if (b_at(w,s,besta-bestx) != 4 && a_at(w,s,bestx) != 4) more = 1;
           if (hghk >= aclip) hghk = aclip-1;
@@ -645,12 +714,19 @@ static void wave(orc_work *w, const orc_spec *spec, int s, int low, int hgh, int
           { while (w->V[IX(lowk)] < n) lowk += 1;
             break;
           }
+      if (st != NULL && more == 0 && hghk < lowk) st->endempty = 1;
     }
 
   out->endx   = s*trimx;
   out->endy   = s*(trima - trimx);
   out->diffs  = trimd;
   out->trimha = trimha;
+  if (st != NULL)
+    { int h;
+      st->aspan = trimx - s*((mida+hgh)>>1);
+      for (h = trimha; w->cells[h].ptr >= 0; h = w->cells[h].ptr)
+        if (h - w->cells[h].ptr > st->maxhop) st->maxhop = h - w->cells[h].ptr;
+    }
   { int h = trimha;
     while (w->cells[h].ptr >= 0) h = w->cells[h].ptr;
     out->root_diag = w->cells[h].diag;
@@ -796,12 +872,12 @@ int orc_local_alignment(orc_work *w, const orc_spec *spec, const char *aseq, int
   aoff = acomp ? alen % spec->tspace : 0;
 
   p->tlen = 0; p->diffs = 0;
-  wave(w,spec,+1,low,hgh,anti,minp,maxp,aoff,&f);
+  wave(w,spec,+1,low,hgh,anti,minp,maxp,aoff,&f,pass_new(w->log));
   fwd_trace(w,&f,anti,p);
   low = f.root_diag;
   fshort = ((p->aepos + p->bepos) - anti < DUB_TRIM);
 
-  wave(w,spec,-1,low,low,anti,minp,maxp,aoff,&r);
+  wave(w,spec,-1,low,low,anti,minp,maxp,aoff,&r,pass_new(w->log));
   rev_trace(w,&r,spec->tspace,aoff,p);
   rshort = (anti - (p->abpos + p->bbpos) < DUB_TRIM);
 
@@ -815,7 +891,7 @@ int orc_local_alignment(orc_work *w, const orc_spec *spec, const char *aseq, int
         { low  = p->abpos - p->bbpos;
           anti = p->abpos + p->bbpos;
           p->tlen = 0;
-          wave(w,spec,+1,low,low,anti,minp,maxp,aoff,&f);
+          wave(w,spec,+1,low,low,anti,minp,maxp,aoff,&f,pass_new(w->log));
           fwd_trace(w,&f,anti,p);
         }
     }
@@ -823,7 +899,7 @@ int orc_local_alignment(orc_work *w, const orc_spec *spec, const char *aseq, int
     { low  = p->aepos - p->bepos;
       anti = p->aepos + p->bepos;
       p->tlen = 0; p->diffs = 0;
-      wave(w,spec,-1,low,low,anti,minp,maxp,aoff,&r);
+      wave(w,spec,-1,low,low,anti,minp,maxp,aoff,&r,pass_new(w->log));
       rev_trace(w,&r,spec->tspace,aoff,p);
     }
 
@@ -1023,6 +1099,7 @@ typedef struct
   { const rec128 *seeds; const orc_layout *L; const orc_params *P; const orc_spec *spec;
     const int *perm1, *perm2; const char **aseq, **acseq, **bseq; const int64_t *alens, *blens;
     orc_result *R; orc_work *work; orc_path *path; int alnMin; double alnRate;
+    orc_calllog *log;                       /* NULL (orc_search), or the call list of orc_search_calls */
     int comp, ctg1, ctg2; int64_t alen, blen, mlen, doffset, aoffset, alast; const char *as, *bs;
   } search_ctx;
 
@@ -1039,6 +1116,31 @@ static void search_triple(void *v, const orc_triple *T)
   S->as = S->comp ? S->acseq[S->ctg1] : S->aseq[S->ctg1];
   S->bs = S->bseq[S->ctg2];
   S->alast = -1;
+}
+
+static void log_call(orc_calllog *g, int comp, int ctg1, int ctg2, int low, int hgh, int anti, int lbord,
+                     int hbord, int rec, const orc_path *p)
+{ orc_call *c;
+  if (g->ncall >= g->maxcall)
+    { g->maxcall = g->maxcall*2 + 256;
+      g->call = (orc_call *) realloc(g->call,sizeof(orc_call)*g->maxcall);
+    }
+  if (g->tlen + p->tlen > g->tmax)
+    { g->tmax = (g->tlen + p->tlen)*2 + 4096;
+      g->tpool = (uint8_t *) realloc(g->tpool,g->tmax);
+    }
+  c = g->call + g->ncall;
+  c->comp = comp; c->ctg1 = ctg1; c->ctg2 = ctg2; c->low = low; c->hgh = hgh; c->anti = anti;
+  c->lbord = lbord; c->hbord = hbord; c->rec = rec;
+  c->abpos = p->abpos; c->bbpos = p->bbpos; c->aepos = p->aepos; c->bepos = p->bepos;
+  c->diffs = p->diffs; c->tlen = p->tlen; c->pad = 0;
+  c->pass0 = (int) g->npass; c->npass = 0;
+  while (c->pass0 > 0 && g->pass[c->pass0-1].call == g->ncall) c->pass0 -= 1;
+  c->npass = (int) g->npass - c->pass0;
+  c->toff = g->tlen;
+  memcpy(g->tpool+g->tlen,p->trace,p->tlen);
+  g->tlen += p->tlen;
+  g->ncall += 1;
 }
 
 static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh, int dgmin, int dgmax,
@@ -1071,20 +1173,22 @@ static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh,
                   if (dgmin > dgmax) break;
                 }
             }
+          int lbord = -1, hbord = -1, called = 1;
           if (g_self && ctg1 == ctg2 && !comp)
             { if (dgmin > 0)
-                orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
-                                    dgmin,dgmax,(int) amid,dgmin-1,-1,path);
+                lbord = dgmin-1;
               else if (dgmax < 0)
-                orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
-                                    dgmin,dgmax,(int) amid,-1,-(dgmax+1),path);
+                hbord = -(dgmax+1);
               else
-                path->abpos = path->aepos = 0;
+                { path->abpos = path->aepos = 0; called = 0; }
             }
-          else
+          if (called)
             orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
-                                dgmin,dgmax,(int) amid,-1,-1,path);
+                                dgmin,dgmax,(int) amid,lbord,hbord,path);
           rlen = path->aepos - path->abpos;
+          if (called && S->log != NULL)
+            log_call(S->log,comp,ctg1,ctg2,dgmin,dgmax,(int) amid,lbord,hbord,
+                     rlen >= S->alnMin && S->alnRate*rlen >= path->diffs,path);
           if (rlen >= S->alnMin && S->alnRate*rlen >= path->diffs)
             { orc_ovl o;
               o.comp = comp; o.aread = ctg1; o.bread = ctg2;
@@ -1102,16 +1206,17 @@ static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh,
     }
 }
 
-int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
-                   const orc_spec *spec, const int *perm1, const int *perm2,
-                   const char **aseq, const char **acseq, const int64_t *alens,
-                   const char **bseq, const int64_t *blens, orc_result *R)
+static int64_t search(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
+                      const orc_spec *spec, const int *perm1, const int *perm2,
+                      const char **aseq, const char **acseq, const int64_t *alens,
+                      const char **bseq, const int64_t *blens, orc_result *R, orc_calllog *log)
 { search_ctx S;
   orc_path path; memset(&path,0,sizeof(path));
   memset(&S,0,sizeof(S));
   S.seeds = seeds; S.L = L; S.P = P; S.spec = spec; S.perm1 = perm1; S.perm2 = perm2;
   S.aseq = aseq; S.acseq = acseq; S.bseq = bseq; S.alens = alens; S.blens = blens;
   S.R = R; S.work = orc_new_work(); S.path = &path;
+  S.log = log; S.work->log = log;
   S.alnMin = P->align_min - 50;
   S.alnRate = P->align_rate + .05;
   chain_scan(seeds,n,L,P->chain_break,P->chain_min,search_triple,search_hit,&S);
@@ -1119,6 +1224,28 @@ int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const or
   orc_free_work(S.work);
   return R->novl;
 }
+
+int64_t orc_search(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
+                   const orc_spec *spec, const int *perm1, const int *perm2,
+                   const char **aseq, const char **acseq, const int64_t *alens,
+                   const char **bseq, const int64_t *blens, orc_result *R)
+{ return search(seeds,n,L,P,spec,perm1,perm2,aseq,acseq,alens,bseq,blens,R,NULL); }
+
+/*  orc_search_calls: orc_search, and the list of its Local_Alignment calls with the passes of each
+    (orc_calllog_* read it out; orc_free_calllog releases it).  */
+orc_calllog *orc_new_calllog(void) { return (orc_calllog *) calloc(1,sizeof(orc_calllog)); }
+void     orc_free_calllog(orc_calllog *g) { free(g->call); free(g->tpool); free(g->pass); free(g); }
+int64_t  orc_calllog_calls(orc_calllog *g) { return g->ncall; }
+int64_t  orc_calllog_passes(orc_calllog *g) { return g->npass; }
+orc_call *orc_calllog_call(orc_calllog *g) { return g->call; }
+orc_pass *orc_calllog_pass(orc_calllog *g) { return g->pass; }
+uint8_t  *orc_calllog_traces(orc_calllog *g) { return g->tpool; }
+
+int64_t orc_search_calls(const rec128 *seeds, int64_t n, const orc_layout *L, const orc_params *P,
+                         const orc_spec *spec, const int *perm1, const int *perm2,
+                         const char **aseq, const char **acseq, const int64_t *alens,
+                         const char **bseq, const int64_t *blens, orc_result *R, orc_calllog *log)
+{ return search(seeds,n,L,P,spec,perm1,perm2,aseq,acseq,alens,bseq,blens,R,log); }
 
 /*  orc_chains: the chains alone.  trip gets 8 words per scanned triple (b, m, e, isnew, (strand,
     contig pair) key, cdiag, first hit, hits), hits 5 words per chain (alow, ahgh, dgmin, dgmax,

@@ -203,11 +203,20 @@ def chain_islands():
     return _distinct(A), _distinct(B), 4, lambda al, hits: hits >= 180 and len(al) >= 180
 
 
+def wave_regimes():
+    """the crafted wave tubes of wave_cases.py, the `ends` family on strand N and the `runs` family on strand
+    C, as one genome pair, aligned from natural seeds: anchors near every contig end, tails, short and
+    4 kbp-boundary contigs, exact runs of 31..500 bases and homopolymer runs"""
+    import wave_cases as wc
+    e, r = wc.case("ends", 0), wc.case("runs", 1)
+    return _distinct(e.A + r.A), _distinct(e.B + r.B), 4, lambda al, hits: len(al) >= 600
+
+
 CASES = {"ragged": ragged, "unrelated": unrelated, "identical_and_revcomp": identical_and_revcomp,
          "tandem_repeats": tandem_repeats, "many_small_contigs": many_small_contigs,
          "seed_key_64": seed_key_64, "seed_key_65": seed_key_65, "icont_straddles": icont_straddles,
          "long_contigs": long_contigs, "long_and_many": long_and_many, "max_contigs": max_contigs,
-         "chain_islands": chain_islands}
+         "chain_islands": chain_islands, "wave_regimes": wave_regimes}
 
 #  what each width case must reach: seed key bits, (post_bytes, cont_bytes) of A and of B, and for
 #  the long cases the least longest-contig length; chunk_overflow: a chunk of chain detection holds more

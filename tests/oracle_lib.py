@@ -380,9 +380,37 @@ def _framed(a):
     return b
 
 
+CALL_DT = np.dtype([("comp", "i4"), ("ctg1", "i4"), ("ctg2", "i4"), ("low", "i4"), ("hgh", "i4"), ("anti", "i4"),
+                    ("lbord", "i4"), ("hbord", "i4"), ("rec", "i4"), ("abpos", "i4"), ("bbpos", "i4"),
+                    ("aepos", "i4"), ("bepos", "i4"), ("diffs", "i4"), ("tlen", "i4"), ("pass0", "i4"),
+                    ("npass", "i4"), ("pad", "i4"), ("toff", "i8")])
+PASS_DT = np.dtype([(n, "i4") for n in ("call", "s", "waves", "maxband", "narrowspan", "maxsnake", "aend", "bend",
+                                        "stall", "endempty", "aspan", "da0", "da1", "db0", "db1", "maxhop")])
+
+
 def search(recs, layout, gA, gB, perm1, perm2, freq, chain_break=2000, chain_min=170, align_min=100,
            align_rate=0.3):
     """oracle alignments in reference discovery order: (records, trace pool, nhit)"""
+    return _search(recs, layout, gA, gB, perm1, perm2, freq, chain_break, chain_min, align_min, align_rate,
+                   False)[:3]
+
+
+def search_calls(recs, layout, gA, gB, perm1, perm2, freq, chain_break=2000, chain_min=170, align_min=100,
+                 align_rate=0.3):
+    """search(), and every Local_Alignment call it made, in discovery order: (records, trace pool, nhit,
+    calls, passes).  calls: CALL_DT rows -- the call's arguments (original contig numbers), rec = 1 where
+    it produced a record, its path (trace bytes "trace") and its passes [pass0, pass0+npass); passes:
+    PASS_DT rows, what every wave pass went through (oracle/fastga_oracle.c orc_pass)."""
+    return _search(recs, layout, gA, gB, perm1, perm2, freq, chain_break, chain_min, align_min, align_rate,
+                   True)
+
+
+def call_key(c):
+    """path_key of one logged call (a CALL_DT row and its trace bytes)"""
+    return path_key(c["abpos"], c["bbpos"], c["aepos"], c["bepos"], c["diffs"], c["tlen"], c["trace"])
+
+
+def _search(recs, layout, gA, gB, perm1, perm2, freq, chain_break, chain_min, align_min, align_rate, logged):
     o = orc()
     spec, tabs, _ = make_spec(freq, 1.0 - align_rate)
     A = [_framed(gA.contig(c)) for c in range(gA.ncontig)]
@@ -398,9 +426,35 @@ def search(recs, layout, gA, gB, perm1, perm2, freq, chain_break=2000, chain_min
     recs = np.ascontiguousarray(recs, dtype=np.uint64)
     p1 = np.ascontiguousarray(perm1, dtype=np.int32)
     p2 = np.ascontiguousarray(perm2, dtype=np.int32)
-    n = o.orc_search(recs.ctypes.data_as(C.c_void_p), C.c_int64(len(recs)), C.byref(L), C.byref(P),
-                     C.byref(spec), p1.ctypes.data_as(C.c_void_p), p2.ctypes.data_as(C.c_void_p),
-                     pa, pac, gA.clen.ctypes.data_as(C.c_void_p), pb, gB.clen.ctypes.data_as(C.c_void_p), R)
+    args = [recs.ctypes.data_as(C.c_void_p), C.c_int64(len(recs)), C.byref(L), C.byref(P), C.byref(spec),
+            p1.ctypes.data_as(C.c_void_p), p2.ctypes.data_as(C.c_void_p), pa, pac,
+            gA.clen.ctypes.data_as(C.c_void_p), pb, gB.clen.ctypes.data_as(C.c_void_p), R]
+    calls = passes = None
+    if logged:
+        for f in ("orc_new_calllog", "orc_calllog_call", "orc_calllog_pass", "orc_calllog_traces"):
+            getattr(o, f).restype = C.c_void_p
+        for f in ("orc_calllog_calls", "orc_calllog_passes", "orc_search_calls"):
+            getattr(o, f).restype = C.c_int64
+        for f in ("orc_calllog_calls", "orc_calllog_passes", "orc_calllog_call", "orc_calllog_pass",
+                  "orc_calllog_traces", "orc_free_calllog"):
+            getattr(o, f).argtypes = [C.c_void_p]
+        G = C.c_void_p(o.orc_new_calllog())
+        n = o.orc_search_calls(*args, G)
+        nc, npas = o.orc_calllog_calls(G), o.orc_calllog_passes(G)
+
+        def take(ptr, dt, count):
+            if count == 0:
+                return np.zeros(0, dtype=dt)
+            return np.ctypeslib.as_array(C.cast(ptr, C.POINTER(C.c_uint8)), shape=(count * dt.itemsize,)).view(dt).copy()
+        raw = take(o.orc_calllog_call(G), CALL_DT, nc)
+        passes = take(o.orc_calllog_pass(G), PASS_DT, npas)
+        tl = int((raw["toff"] + raw["tlen"]).max()) if nc else 0
+        pool = take(o.orc_calllog_traces(G), np.dtype(np.uint8), tl)
+        o.orc_free_calllog(G)
+        calls = [dict({f: int(c[f]) for f in CALL_DT.names},
+                      trace=pool[int(c["toff"]):int(c["toff"]) + int(c["tlen"])]) for c in raw]
+    else:
+        n = o.orc_search(*args)
     o.orc_result_ovls.restype = C.c_void_p
     o.orc_result_traces.restype = C.c_void_p
     o.orc_result_hits.restype = C.c_int64
@@ -416,7 +470,7 @@ def search(recs, layout, gA, gB, perm1, perm2, freq, chain_break=2000, chain_min
         tp = np.zeros(0, dtype=np.uint8)
     o.orc_free_result.argtypes = [C.c_void_p]
     o.orc_free_result(R)
-    return ov, tp, nhit
+    return ov, tp, nhit, calls, passes
 
 
 CHAIN_TRIPLE_DT = np.dtype([("b", "i8"), ("m", "i8"), ("e", "i8"), ("isnew", "i8"), ("key", "i8"), ("cdiag", "i8"),
