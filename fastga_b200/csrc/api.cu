@@ -1,7 +1,7 @@
 // C-ABI of libfastga_b200.so: opaque handles (genome / GIX / seed set) over device memory and the
 // host-buffer entry points the reference-side host code binds (see include/fastga_b200.h and
 // INTEGRATION.md).  No torch types, no CPU fallback: every call runs the sm_90a kernels.
-#include "common.cuh"
+#include "stages.h"
 #include "handles.h"
 #include <vector>
 #include <algorithm>
@@ -12,65 +12,6 @@ typedef unsigned long long u64;
 
 static inline long long now_us()
 { return std::chrono::duration_cast<std::chrono::microseconds>(std::chrono::steady_clock::now().time_since_epoch()).count(); }
-
-extern "C" {
-int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                               void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                            void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
-                       void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-long long fgb_sort128_tmp_bytes(long long n);
-int fgb_sort_seeds64_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                            void *d_tmp, long long tmp_bytes, unsigned long long *d_flag, void *stream);
-int fgb_stage_genome_device(const void *d_bps, const long long *d_boff, const long long *d_clen,
-                            const long long *d_woff, int ncontig, long long total_words,
-                            void *d_seq, void *d_rseq, void *stream);
-int fgb_syncmer_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                             const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                             int ntiles, unsigned *d_tile_count, unsigned long long *d_buck1024,
-                             unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                             unsigned plo, unsigned phi, void *stream);
-int fgb_syncmer_emit_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                            const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                            int ntiles, unsigned *d_tile_offset, void *d_records, unsigned plo,
-                            unsigned phi, void *stream);
-int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
-int fgb_syncmer_bin_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                                 const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                                 int ntiles, unsigned long long *d_buck1024, unsigned *d_bin_start, long long nf,
-                                 int fsh, unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                                 unsigned plo, unsigned phi, void *stream);
-int fgb_syncmer_scatter_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                               const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                               int ntiles, const unsigned *d_bin_start, unsigned *d_cursor, long long nf, int fsh,
-                               long long n, void *d_records, unsigned *d_bad, unsigned plo, unsigned phi,
-                               void *stream);
-int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                                     const unsigned *fstart, long long nf, int fsh, int *result_in_b, void *stream);
-int fgb_kix_index_device(const void *d_tab, long long n, unsigned *d_pstart, unsigned char *d_adj, void *stream);
-int fgb_ktab_export_device(const void *d_tab, long long n, int pbytes, int cbytes,
-                           const long long *d_part_first, int nparts, void *d_out, void *stream);
-int fgb_ktab_import_device(const void *d_ent, long long n, int pbytes, int cbytes,
-                           const long long *d_index, void *d_tab, void *stream);
-int fgb_sc_tile();
-int fgb_owner_count_device(const void *d_seeds, long long n, int p_ic, int ic_bits, const int *d_owner, int nrc,
-                           int world, unsigned long long *d_cnt, void *stream);
-int fgb_owner_scatter_device(const void *d_seeds, long long n, int p_ic, int ic_bits, const int *d_owner, int nrc,
-                             int world, unsigned long long *d_base, void *d_out, void *stream);
-int fgb_kmer_bins_device(const void *d_tab, long long n, int binshift, unsigned *d_bins, void *stream);
-int fgb_self_merge_device(const void *d_T, long long n, const unsigned *d_pstart, int freq,
-                          int anti_bits, int band_bits, int jc_bits, int ic_bits,
-                          long long amxpos, void *d_seeds, long long capacity,
-                          unsigned long long *d_counters, unsigned long long *h_nseeds,
-                          unsigned long long *h_sumlen, void *stream);
-int fgb_forward_view_device(const void *d_T, long long n, void *d_out, long long *h_nfwd, void *stream);
-int fgb_merge_device(const void *d_T1, long long n1, const void *d_T2, long long n2, const unsigned *d_pstart2,
-                     const unsigned char *d_adj2, int freq, int anti_bits, int band_bits, int jc_bits, int ic_bits,
-                     long long amxpos, long long bmxpos, void *d_seeds, long long capacity,
-                     unsigned long long *d_counters, unsigned long long *h_nseeds,
-                     unsigned long long *h_sumlen, void *stream);
-}
 
 static fgb_timings g_timings;
 
@@ -454,29 +395,6 @@ extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, in
   return FGB_OK;
 }
 
-//  records grouped by the top byte of the k-mer (its first four bases): d_out[bounds[b] .. bounds[b+1])
-//  holds those with top byte b, b = 0..255.  One Onesweep pass; the owner of a record is any
-//  monotone function of that byte, so the send blocks of an all-to-all are contiguous.
-extern "C" int fgb_records_group_by_top_byte(void *d_recs, long long n, void *d_out, long long *bounds257,
-                                             void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  for (int b = 0; b <= 256; b++) bounds257[b] = 0;
-  if (n <= 0) return FGB_OK;
-  dblock<unsigned char> d_tmp; dblock<unsigned> d_bins;
-  long long tmpb = fgb_sort128_tmp_bytes(n);
-  int rc, inb = 0;
-  std::vector<unsigned> bins(65537);
-  CUDA_TRY(d_tmp.alloc(tmpb,st));
-  CUDA_TRY(d_bins.alloc(65537,st));
-  if ((rc = fgb_sort128_device(d_recs,d_out,n,15,16,d_tmp,tmpb,&inb,st))) return rc;
-  if (!inb) CUDA_TRY(cudaMemcpyAsync(d_out,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-  if ((rc = fgb_kmer_bins_device(d_out,n,56,d_bins,st))) return rc;
-  CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*65537,cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  for (int b = 0; b <= 256; b++) bounds257[b] = bins[b];
-  return FGB_OK;
-}
-
 //  a table over n unsorted device records (copied) whose 12-base prefixes lie in [plo,phi): one
 //  rank's slice of a k-mer-space sharded table
 extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned plo, unsigned phi, int fwd_only,
@@ -679,16 +597,11 @@ static int seeds_sort_impl(dblock<rec128> d_a, long long n, const seed_bits &L, 
   const bool narrow = L.key <= 64 && !(wide_env != NULL && atoi(wide_env) != 0);
   u64 hiflag = 0, *d_hiflag = NULL;
   CUDA_TRY(d_b.alloc(n+1,st));
-  CUDA_TRY(d_tmp.alloc(tmpb + 8,st));
+  CUDA_TRY(d_tmp.alloc(tmpb,st));
   { stage_timer t(&g_timings.ssort_ms,st);
     //  from bit 6: the lcp field (bits 0..5) cannot break a tie -- two seeds that agree on strand,
     //  contigs, band, anti-diagonal and diagonal remainder are the same pair of positions
-    if (narrow)
-      { d_hiflag = (u64 *) (d_tmp + tmpb);
-        rc = fgb_sort_seeds64_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,d_hiflag,st);
-      }
-    else
-      rc = fgb_sort128_bits_device(d_a,d_b,n,6,L.key,d_tmp,tmpb,&inb,st);
+    rc = fgb_radix_sort_device(d_a,d_b,n,6,L.key,narrow,d_tmp,tmpb,&inb,&d_hiflag,st);
   }
   if (rc) return rc;
   if (d_hiflag) CUDA_TRY(cudaMemcpyAsync(&hiflag,d_hiflag,8,cudaMemcpyDeviceToHost,st));
@@ -762,7 +675,6 @@ extern "C" int fgb_seeds_group_by_owner(const void *d_seeds, long long n, const 
 }
 
 //  k-mer records grouped by the rank that owns their first four bases: owner256[b] for top byte b
-//  (cheaper than the radix pass of fgb_records_group_by_top_byte when only the destination matters)
 extern "C" int fgb_records_group_by_owner(const void *d_recs, long long n, const int *owner256, int world,
                                           void *d_out, long long *bounds, void *stream)
 { return group_by_owner(d_recs,n,120,8,owner256,256,world,d_out,bounds,(cudaStream_t) stream); }
@@ -817,30 +729,11 @@ extern "C" int fgb_device_ready()
  *  Read_GDB and la_merge (FastGA.c:4927-5205), GIX construction included.
  **********************************************************************************************/
 
-struct fgb_alns;
-extern "C" {
-int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B, int chain_break,
-               int chain_min, int align_min, double align_rate, const short *tables, int ave_path,
-               int tspace, fgb_overlaps **out, void *stream);
-int fgb_align_spec(double ave_corr, const float *freq, short *tables, int *ave_path);
-long long fgb_overlaps_bytes(const fgb_overlaps *o);
-void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out);
-int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *perm2, int jc_bits, int ic_bits,
-               int do_filter, fgb_alns **out);
-}
-
 struct fgb_run_stats
 { long long nkmers1, nkmers2, nseeds, sumlen, nhits, nla, nwaves, ncells, nraw, h2d_bytes, d2h_bytes,
             nseg, nwork, warp_cycles, wave_cycles, extract_cycles,
             us_gix, us_seeds, us_extend, us_filter, nkmers1_fwd,
             slow_cycles, slow_waves, paired_waves, pairings; };
-
-//  Merge + seed sort + extension + filter from prebuilt tables (x2 may have been assembled from
-//  shares built on several ranks).
-extern "C" int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1,
-                                const fgb_gix *x2, const float *freqA,
-                                int freq, int chain_break, int chain_min, int align_min,
-                                double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream);
 
 static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
                              std::unique_ptr<fgb_gix> *own, const float *freqA, int freq, int chain_break,
@@ -869,6 +762,8 @@ extern "C" int fgb_align_resident(const fgb_genome *A, const fgb_genome *B, cons
   return rc;
 }
 
+//  Merge + seed sort + extension + filter from prebuilt tables (x2 may have been assembled from
+//  shares built on several ranks).
 extern "C" int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1,
                                 const fgb_gix *x2, const float *freqA,
                                 int freq, int chain_break, int chain_min, int align_min,

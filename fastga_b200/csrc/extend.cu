@@ -25,7 +25,7 @@
 //   * SELF mode (a genome against itself): band borders for a contig against itself (handle_hit).
 // Sequences are the 2-bit staged contigs (gix.cu); a snake step compares 32 bases per 64-bit XOR.
 // Integer / branch work: no tensor cores.
-#include "common.cuh"
+#include "stages.h"
 #include "handles.h"
 #include <limits.h>
 #include <string.h>

@@ -8,7 +8,7 @@
 //   entwine                         FastGA.c:2818-2941
 //   redundancy filter               FastGA.c:3407-3685   (per (A-contig, B-contig, strand) call)
 //   la_sort / SORT_MAP order        FastGA.c:3800-3900
-#include "common.cuh"
+#include "stages.h"
 #include "handles.h"
 #include <stdlib.h>
 #include <string.h>
@@ -18,10 +18,6 @@
 #define OUT_HDR   40
 #define TSPACE    100
 #define BOX_FUZZ  10
-
-struct fgb_overlaps;
-extern "C" long long fgb_overlaps_bytes(const fgb_overlaps *o);
-extern "C" const unsigned char *fgb_overlaps_data(const fgb_overlaps *o);
 
 //  The rules below are the reference's (their result is part of the .1aln contract, libc qsort tie
 //  order and the `diffs < aepos` comparison of FastGA.c:3456 included); the implementation is this

@@ -8,7 +8,7 @@
 //   msd_sort                         MSDsort.c:404                 -> sort128.cu (10 byte passes)
 //   compress_thread / k_sort writer  GIXmake.c:1211-1278,1300-1596 -> kix_index/ktab_export kernels
 //   Kmer_Stream reader               libfastk.c:785-1313           -> ktab_import_kernel
-#include "common.cuh"
+#include "stages.h"
 
 // 4-mer hash map of the syncmer sampler.  This is data, not code: it defines which positions
 // are indexed, so it must be value-identical to GIXmake.c:92-109 (TMap) for on-disk parity.
@@ -506,10 +506,6 @@ __global__ void ktab_import_kernel(const unsigned char *__restrict__ ent, long l
 /***********************************************************************************************
  *  Host-callable pieces (device pointers in, device pointers out).
  **********************************************************************************************/
-
-extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
-                                  void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-extern "C" long long fgb_sort128_tmp_bytes(long long n);
 
 extern "C" int fgb_stage_genome_device(const void *d_bps, const long long *d_boff,
                                        const long long *d_clen, const long long *d_woff,

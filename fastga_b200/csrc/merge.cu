@@ -19,7 +19,7 @@
 // Seeds are expanded load-balanced: each entry drops one 32-bit descriptor per seed into shared
 // memory, then every thread builds one 128-bit seed record per step and the stores of the CTA are
 // one contiguous run reserved with ONE atomic.
-#include "common.cuh"
+#include "stages.h"
 
 typedef unsigned long long u64;
 

@@ -11,12 +11,8 @@
 // words (panel | key | ...), sorted with the radix sort of sort128.cu and narrowed again.
 // Equal keys keep their input order here (the reference's in-place sort leaves them in an
 // unspecified order; its consumers do not depend on it).
-#include "common.cuh"
+#include "stages.h"
 #include <string.h>
-
-extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
-                                  void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-extern "C" long long fgb_sort128_tmp_bytes(long long n);
 
 typedef unsigned long long u64;
 

@@ -1,4 +1,4 @@
-// LSD radix sort of 128-bit records on a byte range of the key, hand-written for sm_90a (H100).
+// LSD radix sort of 128-bit records on a bit range of the key, hand-written for sm_90a (H100).
 //
 // Replaces the reference's two CPU sorts on the hot path:
 //   msd_sort   (MSDsort.c:404)  -- k-mer records of the GIX build, key = 40-mer (80 bits)
@@ -6,11 +6,18 @@
 // Both are in-place American-flag MSD sorts on byte-packed records (MSDsort.c:211-360); on the
 // device every record is widened to one 16-byte word so each pass is a perfectly coalesced
 // stream (read 16 B, write 16 B per record).  One pass = one Onesweep kernel: a stable scatter
-// that ranks records inside a 4096-record tile with a warp multi-split (ballots), finds the tile's
-// bases by decoupled look-back, stages the tile in shared memory in digit order and writes digit
-// runs back coalesced, while counting the next pass's histogram.  HBM-bound integer work: no
-// tensor cores.
-#include "common.cuh"
+// that ranks records inside a tile with a warp multi-split (ballots), finds the tile's bases by
+// decoupled look-back, stages the tile in shared memory in digit order and writes digit runs back
+// coalesced, while counting the next pass's histogram.  HBM-bound integer work: no tensor cores.
+//
+// Pass plans (fgb_radix_sort_device):
+//   128-bit  every pass reads and writes 16-byte records; the result lands in d_a or d_b.
+//   narrow   for records whose hi word is zero (keys of <= 64 bits, two passes or more): the first pass
+//            reads the 16-byte records and writes only their lo words (ORing every dropped hi word into
+//            a flag), the middle passes run on 8-byte words and the last pass writes 16-byte records
+//            again (hi = 0) into d_a: per record 16 + 24 + 16·(passes−2) + 24 bytes instead of
+//            16 + 32·passes.
+#include "stages.h"
 #include <stdlib.h>
 #include <vector>
 
@@ -18,11 +25,19 @@
 #ifndef SORT_ITEMS
 #define SORT_ITEMS   8
 #endif
+//  items per thread of a pass on 8-byte input: the staging buffer holds one tile of INPUT records,
+//  64 KB for both widths, so two CTAs still share an SM
+#ifndef SORT64_ITEMS
+#define SORT64_ITEMS 16
+#endif
 #ifndef SORT_MINBLK
 #define SORT_MINBLK  2
 #endif
 #define SORT_TILE    (SORT_THREADS*SORT_ITEMS)
 #define SORT_WARPS   (SORT_THREADS/32)
+static_assert(SORT_THREADS*SORT64_ITEMS >= SORT_TILE, "fgb_sort128_tmp_bytes sizes the look-back status for SORT_TILE");
+
+typedef unsigned long long u64;
 
 static __device__ __forceinline__ unsigned warp_incl_scan(unsigned v, int lane)
 {
@@ -34,11 +49,17 @@ static __device__ __forceinline__ unsigned warp_incl_scan(unsigned v, int lane)
   return v;
 }
 
+//  the 8-bit digit at bit offset sh of an 8-byte word, and the word's loads and stores, beside the
+//  rec128 forms of common.cuh
+static __device__ __forceinline__ unsigned rec_dig(u64 v, int sh) { return (unsigned) (v >> sh) & 0xff; }
+static __device__ __forceinline__ u64 ld_rec(const u64 *p) { return *p; }
+static __device__ __forceinline__ void st_rec(u64 *p, u64 v) { *p = v; }
+
 
 /***********************************************************************************************
- *  Onesweep pass: one kernel per key byte reads every record once and writes it once.
+ *  Onesweep pass: one kernel per digit reads every record once and writes it once.
  *   - the GLOBAL digit histogram of a pass is produced by the previous pass (each tile counts
- *     the next byte while it holds the records; the first pass has a small histogram kernel);
+ *     the next digit while it holds the records; the first pass has a small histogram kernel);
  *   - the tile's base inside each digit bucket comes from a decoupled look-back over the
  *     per-tile digit counts (status word = count | flag<<62; 1 = tile aggregate, 2 = inclusive
  *     prefix), tiles being handed out by an atomic ticket so every predecessor is running.
@@ -58,10 +79,80 @@ static __device__ __forceinline__ unsigned match_digit(unsigned d, bool valid)
   return peers;
 }
 
+//  Rank of this lane's item among the items of digit d its warp has ranked so far: myc is the warp's
+//  count column (myc[d] = items of digit d in earlier rounds), bumped by the round's leader.
+static __device__ __forceinline__ unsigned warp_rank(unsigned *myc, unsigned d, bool valid)
+{ const int lane = threadIdx.x & 31;
+  unsigned peers = match_digit(d,valid);
+  int leader = valid ? __ffs(peers)-1 : lane;
+  unsigned b = 0;
+  if (valid && lane == leader)
+    { b = myc[d];
+      myc[d] = b + __popc(peers);
+    }
+  b = __shfl_sync(0xffffffffu,b,leader);
+  __syncwarp();
+  return b + __popc(peers & lanemask_lt());
+}
+
+//  Once every warp has ranked its items: wcount[w][d] (the count columns, SORT_WARPS x 256) becomes the
+//  count of digit d in the warps before w, and bexcl[d] the tile's count of the digits below d.  Thread
+//  d < 256 returns the tile's count of digit d and hands it to publish before the scan.  Ends on a barrier.
+template <class F>
+static __device__ __forceinline__ unsigned digit_offsets(unsigned *wcount, unsigned *bexcl, unsigned *wtot, F publish)
+{ const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  unsigned c = 0, inc = 0;
+  __syncthreads();
+  if (tid < 256)
+    {
+#pragma unroll
+      for (int ww = 0; ww < SORT_WARPS; ww++)
+        { unsigned t = wcount[ww*256+tid];
+          wcount[ww*256+tid] = c;
+          c += t;
+        }
+      publish(c);
+      inc = warp_incl_scan(c,lane);
+      if (lane == 31) wtot[w] = inc;
+    }
+  __syncthreads();
+  if (tid < 256)
+    { unsigned pre = 0;
+      for (int i = 0; i < w; i++) pre += wtot[i];
+      bexcl[tid] = pre + inc - c;
+    }
+  __syncthreads();
+  return c;
+}
 
 #define ST_AGG  (1ull << 62)
 #define ST_INC  (2ull << 62)
 #define ST_MASK ((1ull << 62) - 1)
+
+//  Records of digit d (d = tid < 256) in the tiles before tileid.  Four predecessors per round trip:
+//  the status words of consecutive tiles are independent loads, a serial walk pays one L2 latency per
+//  tile, and the walk is as deep as the tiles in flight.  A tile that has published nothing yet is
+//  read again from there on.
+static __device__ __forceinline__ u64 lookback(const u64 *status, unsigned tileid, int tid)
+{ volatile const u64 *stt = status;
+  u64 excl = 0;
+  for (long long t = (long long) tileid - 1; t >= 0; )
+    { u64 v[4];
+#pragma unroll
+      for (int q = 0; q < 4; q++)
+        v[q] = (t - q >= 0) ? stt[(u64) (t - q)*256 + tid] : ST_INC;
+      bool done = false;
+#pragma unroll
+      for (int q = 0; q < 4; q++)
+        { if (done || (v[q] >> 62) == 0) break;
+          excl += v[q] & ST_MASK;
+          t -= 1;
+          if (v[q] & ST_INC) done = true;
+        }
+      if (done) break;
+    }
+  return excl;
+}
 
 __global__ void __launch_bounds__(SORT_THREADS)
 sort_ghist_kernel(const rec128 *__restrict__ in, long long n, int dsh /* digit = bits [dsh,dsh+8) */, unsigned long long *__restrict__ ghist)
@@ -109,252 +200,41 @@ __global__ void sort_bins_kernel(const unsigned long long *__restrict__ ghist, u
   if (tid == 0) *ticket = 0;
 }
 
-__global__ void __launch_bounds__(SORT_THREADS,SORT_MINBLK)
-sort_onesweep_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out, long long n, int byte /* bit offset of the digit */,
-                     int next_byte /* bit offset of the next pass's digit, -1: none */, const unsigned long long *__restrict__ binbase,
-                     unsigned long long *__restrict__ nexthist, unsigned long long *status /* [ntiles][256] */,
-                     unsigned *__restrict__ ticket)
-{ extern __shared__ __align__(16) unsigned char smem_raw[];
-  rec128   *tile   = reinterpret_cast<rec128 *>(smem_raw);
-  unsigned *wcount = reinterpret_cast<unsigned *>(tile + SORT_TILE);   // [SORT_WARPS][256]
-  unsigned *bexcl  = wcount + SORT_WARPS*256;                           // [256]
-  unsigned *nhist  = bexcl + 256;                                       // [256] next byte
-  unsigned *wtot   = nhist + 256;                                       // [8]
-  unsigned long long *gbase = reinterpret_cast<unsigned long long *>(wtot + 8);   // [256]
-  __shared__ unsigned tile_s;
-  __shared__ __align__(8) unsigned long long tbar;
-
-  int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  if (tid == 0)
-    { unsigned t = atomicAdd(ticket,1u);
-      tile_s = t;
-      //  the tile is 4096 consecutive 128-bit records: fetched by one TMA bulk copy (UBLKCP)
-      //  into the staging buffer while the block zeroes its counters
-      long long t0 = (long long) t * SORT_TILE, rm = n - t0;
-      unsigned nb = (unsigned) (rm < SORT_TILE ? rm : SORT_TILE) * 16u;
-      mbar_init(&tbar,1);
-      tma_load_1d(tile,in + t0,nb,&tbar);
-    }
-  for (int i = tid; i < SORT_WARPS*256; i += SORT_THREADS) wcount[i] = 0;
-  if (tid < 256) nhist[tid] = 0;
-  __syncthreads();
-  const unsigned tileid = tile_s;
-  long long tile0 = (long long) tileid * SORT_TILE;
-  long long rem = n - tile0;
-  int cnt = rem < SORT_TILE ? (int) rem : SORT_TILE;
-
-  rec128   r[SORT_ITEMS];
-  unsigned rank[SORT_ITEMS];
-  int base = w*(32*SORT_ITEMS);
-  unsigned *myc = wcount + w*256;
-  mbar_wait(&tbar,0);
-#pragma unroll
-  for (int it = 0; it < SORT_ITEMS; it++)
-    { int idx = base + it*32 + lane;
-      bool valid = idx < cnt;
-      unsigned d = 0;
-      if (valid)
-        { r[it] = ld_rec(tile + idx);
-          d = rec_dig(r[it],byte);
-        }
-      unsigned peers = match_digit(d,valid);
-      int leader = valid ? __ffs(peers)-1 : lane;
-      unsigned b = 0;
-      if (valid && lane == leader)
-        { b = myc[d];
-          myc[d] = b + __popc(peers);
-        }
-      b = __shfl_sync(0xffffffffu,b,leader);
-      rank[it] = b + __popc(peers & lanemask_lt());
-      if (next_byte >= 0 && valid) atomicAdd(&nhist[rec_dig(r[it],next_byte)],1u);
-      __syncwarp();
-    }
-  __syncthreads();
-
-  //  Order of the rest: publish the tile's digit counts at once (the tiles after this one add them up
-  //  while it works on), place the records in digit order inside the tile, and only THEN look back for
-  //  this tile's own bases -- by which time the tiles before it have had the whole placement phase to
-  //  publish theirs, so the walk is short and rarely spins.
-  unsigned c = 0, inc = 0;
-  unsigned long long *mine = status + (unsigned long long) tileid*256 + tid;
-  if (tid < 256)
-    { unsigned sum = 0;
-#pragma unroll
-      for (int ww = 0; ww < SORT_WARPS; ww++)
-        { unsigned t = wcount[ww*256+tid];
-          wcount[ww*256+tid] = sum;
-          sum += t;
-        }
-      c = sum;
-      if (tileid == 0)
-        atomicExch(mine,ST_INC | c);
-      else
-        atomicExch(mine,ST_AGG | c);
-      inc = warp_incl_scan(c,lane);
-      if (lane == 31) wtot[w] = inc;
-    }
-  __syncthreads();
-  if (tid < 256)
-    { unsigned pre = 0;
-      for (int i = 0; i < w; i++) pre += wtot[i];
-      bexcl[tid] = pre + inc - c;
-    }
-  __syncthreads();
-
-#pragma unroll
-  for (int it = 0; it < SORT_ITEMS; it++)
-    { int idx = base + it*32 + lane;
-      if (idx < cnt)
-        { unsigned d = rec_dig(r[it],byte);
-          st_rec(tile + (bexcl[d] + myc[d] + rank[it]),r[it]);
-        }
-    }
-  if (tid < 256)
-    { //  four predecessors per round trip (the status words of consecutive tiles are independent loads;
-      //  a serial walk pays one L2 latency per tile, and the walk is as deep as the tiles in flight)
-      volatile unsigned long long *stt = status;
-      unsigned long long excl = 0;
-      for (long long t = (long long) tileid - 1; t >= 0; )
-        { unsigned long long v[4];
-#pragma unroll
-          for (int q = 0; q < 4; q++)
-            v[q] = (t - q >= 0) ? stt[(unsigned long long) (t - q)*256 + tid] : ST_INC;
-          bool done = false;
-#pragma unroll
-          for (int q = 0; q < 4; q++)
-            { if (done || (v[q] >> 62) == 0) break;            // not there yet: spin from this tile on
-              excl += v[q] & ST_MASK;
-              t -= 1;
-              if (v[q] & ST_INC) done = true;
-            }
-          if (done) break;
-        }
-      if (tileid != 0) atomicExch(mine,ST_INC | (excl + c));
-      gbase[tid] = binbase[tid] + excl - bexcl[tid];
-      if (next_byte >= 0 && nhist[tid]) atomicAdd(&nexthist[tid],(unsigned long long) nhist[tid]);
-    }
-  __syncthreads();
-
-  for (int p = tid; p < cnt; p += SORT_THREADS)
-    { rec128 v = ld_rec(tile + p);
-      unsigned d = rec_dig(v,byte);
-      st_rec(out + (gbase[d] + p),v);
-    }
-}
-
-static const size_t ONESWEEP_SMEM = SORT_TILE*sizeof(rec128) + (SORT_WARPS*256 + 256 + 256 + 8)*sizeof(unsigned)
-                                    + 256*sizeof(unsigned long long);
-
-extern "C" long long fgb_sort128_tmp_bytes(long long n)
-{ long long ntiles = (n + SORT_TILE - 1) / SORT_TILE;
-  if (ntiles < 1) ntiles = 1;
-  return 256*ntiles*8 + (3*256 + 16)*8;          // look-back status + 2 histograms + bin bases + ticket
-}
-
-//  Sorts n records on key bytes [byte_lo,byte_hi) of the 128-bit little-endian value, stable.
-//  d_a holds the input; d_b is a same-size scratch.  Returns via *result_in_b where the sorted
-//  data landed (0 = d_a, 1 = d_b).  All pointers are device pointers.
-
-//  LSD passes on the 8-bit digits at bit offsets bit_lo, bit_lo+8, ... below bit_hi (the last digit may
-//  reach past bit_hi: the bits above a key are part of the order, zero in every record sorted here)
-extern "C" int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                                       void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  if (n < 0 || bit_lo < 0 || bit_hi > 128 || bit_lo > bit_hi) return FGB_ERR_ARG;
-  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
-  *result_in_b = 0;
-  if (n <= 1 || bit_lo == bit_hi) return FGB_OK;
-  if (tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
-
-  int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE);
-  unsigned long long *status = (unsigned long long *) d_tmp;
-  unsigned long long *hist[2] = { status + 256ull*ntiles, status + 256ull*ntiles + 256 };
-  unsigned long long *binbase = status + 256ull*ntiles + 512;
-  unsigned *ticket = (unsigned *) (binbase + 256);
-
-  static bool attr_set = false;
-  if (!attr_set)
-    { CUDA_TRY(cudaFuncSetAttribute(sort_onesweep_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int) ONESWEEP_SMEM));
-      attr_set = true;
-    }
-
-  rec128 *src = (rec128 *) d_a, *dst = (rec128 *) d_b;
-  CUDA_TRY(cudaMemsetAsync(hist[0],0,256*8,st));
-  { int nb = ntiles < 1184 ? ntiles : 1184;
-    sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>(src,n,bit_lo,hist[0]);
-    fgb_count_launch(1);
-  }
-  int cur = 0;
-  for (int b = bit_lo; b < bit_hi; b += 8)
-    { sort_bins_kernel<<<1,256,0,st>>>(hist[cur],binbase,hist[cur^1],ticket);
-      CUDA_TRY(cudaMemsetAsync(status,0,256ull*ntiles*8,st));
-      sort_onesweep_kernel<<<ntiles,SORT_THREADS,ONESWEEP_SMEM,st>>>(src,dst,n,b,(b+8 < bit_hi) ? b+8 : -1,
-                                                                   binbase,hist[cur^1],status,ticket);
-      fgb_count_launch(2);
-      cur ^= 1;
-      rec128 *t = src; src = dst; dst = t;
-      *result_in_b ^= 1;
-    }
-  CUDA_TRY(cudaGetLastError());
-  return FGB_OK;
-}
-
-extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
-                                  void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
-{ if (byte_lo < 0 || byte_hi > 16 || byte_lo > byte_hi) return FGB_ERR_ARG;
-  return fgb_sort128_bits_device(d_a,d_b,n,8*byte_lo,8*byte_hi,d_tmp,tmp_bytes,result_in_b,stream);
-}
-
-/***********************************************************************************************
- *  Seed sort on 64-bit words.  When the seed key fits in 64 bits (every 100 Mbp-class pair) the
- *  merge leaves hi = 0 in every record, yet the 128-bit passes above read and write all 16 bytes.
- *  Here the first pass reads the 16-byte records and writes only their lo words, the middle passes
- *  run on 8-byte words and the last pass writes 16-byte records again (hi = 0): per record
- *  16 + 24 + 16·(passes−2) + 24 bytes instead of 16 + 32·passes.  Same Onesweep method as
- *  sort_onesweep_kernel (TMA tile, nine-ballot multi-split, counts published first, look-back last,
- *  next histogram counted while the tile is resident), stable.
- **********************************************************************************************/
-
-//  records per tile of a pass on 8-byte input (the 16-byte first pass keeps SORT_TILE: the staging
-//  buffer holds one tile of INPUT records, 64 KB either way, so two CTAs still share an SM)
-#ifndef SORT64_ITEMS
-#define SORT64_ITEMS 16
-#endif
-static_assert(SORT_THREADS*SORT64_ITEMS >= SORT_TILE, "fgb_sort128_tmp_bytes sizes the look-back status for SORT_TILE");
-
-template <int IW> struct os64_tile
+//  IW: bytes per input record; a tile holds SORT_ITEMS 16-byte records or SORT64_ITEMS 8-byte words per thread
+template <int IW> struct os_tile
 { static constexpr int ITEMS = (IW == 16) ? SORT_ITEMS : SORT64_ITEMS;
   static constexpr int TILE  = SORT_THREADS*ITEMS;
   static constexpr size_t SMEM = (size_t) TILE*IW + (SORT_WARPS*256 + 256 + 256 + 8)*sizeof(unsigned)
-                                 + 256*sizeof(unsigned long long);
+                                 + 256*sizeof(u64);
 };
 
-//  IW / OW: bytes per input / output record.  16: a rec128 whose hi word must be zero (the pass ORs
-//  every hi word it drops into *hiflag); 8: its lo word alone; 16 out: lo, hi = 0.
-template <int IW, int OW>
+//  One pass on the digit at bit dsh.  Key: the word ranked and held in registers, a rec128 or the lo
+//  word of a record whose hi word must be zero.  IW / OW: bytes per input / output record.  A 16-byte
+//  record read into a u64 Key ORs its hi word into *hiflag; a u64 Key written as 16 bytes gets hi = 0.
+template <class Key, int IW, int OW>
 __global__ void __launch_bounds__(SORT_THREADS,SORT_MINBLK)
-sort_onesweep64_kernel(const void *__restrict__ in, void *__restrict__ out, long long n, int dsh /* bit offset of the digit */,
-                       int next_dsh /* of the next pass's digit, -1: none */, const unsigned long long *__restrict__ binbase,
-                       unsigned long long *__restrict__ nexthist, unsigned long long *status /* [ntiles][256] */,
-                       unsigned *__restrict__ ticket, unsigned long long *__restrict__ hiflag)
-{ constexpr int ITEMS = os64_tile<IW>::ITEMS, TILE = os64_tile<IW>::TILE;
+sort_onesweep_kernel(const void *__restrict__ in, void *__restrict__ out, long long n, int dsh /* bit offset of the digit */,
+                     int next_dsh /* of the next pass's digit, -1: none */, const u64 *__restrict__ binbase,
+                     u64 *__restrict__ nexthist, u64 *status /* [ntiles][256] */, unsigned *__restrict__ ticket,
+                     u64 *__restrict__ hiflag)
+{ constexpr int ITEMS = os_tile<IW>::ITEMS, TILE = os_tile<IW>::TILE;
   extern __shared__ __align__(16) unsigned char smem_raw[];
-  unsigned long long *tile = reinterpret_cast<unsigned long long *>(smem_raw);   // input tile, then the words in digit order
+  Key      *tile   = reinterpret_cast<Key *>(smem_raw);                  // input tile, then the keys in digit order
   unsigned *wcount = reinterpret_cast<unsigned *>(smem_raw + (size_t) TILE*IW); // [SORT_WARPS][256]
-  unsigned *bexcl  = wcount + SORT_WARPS*256;                                   // [256]
-  unsigned *nhist  = bexcl + 256;                                               // [256] next digit
-  unsigned *wtot   = nhist + 256;                                               // [8]
-  unsigned long long *gbase = reinterpret_cast<unsigned long long *>(wtot + 8); // [256]
+  unsigned *bexcl  = wcount + SORT_WARPS*256;                           // [256]
+  unsigned *nhist  = bexcl + 256;                                       // [256] next digit
+  unsigned *wtot   = nhist + 256;                                       // [8]
+  u64      *gbase  = reinterpret_cast<u64 *>(wtot + 8);                 // [256]
   __shared__ unsigned tile_s;
-  __shared__ __align__(8) unsigned long long tbar;
+  __shared__ __align__(8) u64 tbar;
 
   int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
   if (tid == 0)
     { unsigned t = atomicAdd(ticket,1u);
       tile_s = t;
-      //  an odd count of 8-byte words is rounded up to the 16 bytes a bulk copy moves (the caller's
-      //  buffers have room for that word; it is never ranked)
+      //  the tile's consecutive input records: fetched by one TMA bulk copy (UBLKCP) into the staging
+      //  buffer while the block zeroes its counters.  An odd count of 8-byte words is rounded up to the
+      //  16 bytes a bulk copy moves (the caller's buffers have room for that word; it is never ranked).
       long long t0 = (long long) t * TILE, rm = n - t0;
       unsigned nb = ((unsigned) (rm < TILE ? rm : TILE) * IW + 15u) & ~15u;
       mbar_init(&tbar,1);
@@ -368,8 +248,9 @@ sort_onesweep64_kernel(const void *__restrict__ in, void *__restrict__ out, long
   long long rem = n - tile0;
   int cnt = rem < TILE ? (int) rem : TILE;
 
-  unsigned long long r[ITEMS], hi_or = 0;
+  Key      r[ITEMS];
   unsigned rank[ITEMS];
+  u64      hi_or = 0;
   int base = w*(32*ITEMS);
   unsigned *myc = wcount + w*256;
   mbar_wait(&tbar,0);
@@ -379,166 +260,161 @@ sort_onesweep64_kernel(const void *__restrict__ in, void *__restrict__ out, long
       bool valid = idx < cnt;
       unsigned d = 0;
       if (valid)
-        { if (IW == 16)
-            { rec128 v = ld_rec(reinterpret_cast<const rec128 *>(tile) + idx);
+        { if constexpr (sizeof(Key) < IW)
+            { rec128 v = ld_rec(reinterpret_cast<const rec128 *>(smem_raw) + idx);
               r[it] = v.lo;
               hi_or |= v.hi;
             }
           else
-            r[it] = tile[idx];
-          d = (unsigned) (r[it] >> dsh) & 0xff;
+            r[it] = ld_rec(tile + idx);
+          d = rec_dig(r[it],dsh);
         }
-      unsigned peers = match_digit(d,valid);
-      int leader = valid ? __ffs(peers)-1 : lane;
-      unsigned b = 0;
-      if (valid && lane == leader)
-        { b = myc[d];
-          myc[d] = b + __popc(peers);
-        }
-      b = __shfl_sync(0xffffffffu,b,leader);
-      rank[it] = b + __popc(peers & lanemask_lt());
-      if (next_dsh >= 0 && valid) atomicAdd(&nhist[(unsigned) (r[it] >> next_dsh) & 0xff],1u);
-      __syncwarp();
+      rank[it] = warp_rank(myc,d,valid);
+      if (next_dsh >= 0 && valid) atomicAdd(&nhist[rec_dig(r[it],next_dsh)],1u);
     }
-  if (IW == 16 && hi_or) atomicOr(hiflag,hi_or);
-  __syncthreads();
+  if (sizeof(Key) < IW && hi_or) atomicOr(hiflag,hi_or);
 
-  unsigned c = 0, inc = 0;
-  unsigned long long *mine = status + (unsigned long long) tileid*256 + tid;
-  if (tid < 256)
-    { unsigned sum = 0;
-#pragma unroll
-      for (int ww = 0; ww < SORT_WARPS; ww++)
-        { unsigned t = wcount[ww*256+tid];
-          wcount[ww*256+tid] = sum;
-          sum += t;
-        }
-      c = sum;
-      if (tileid == 0)
-        atomicExch(mine,ST_INC | c);
+  //  Order of the rest: publish the tile's digit counts at once (the tiles after this one add them up
+  //  while it works on), place the records in digit order inside the tile, and only THEN look back for
+  //  this tile's own bases -- by which time the tiles before it have had the whole placement phase to
+  //  publish theirs, so the walk is short and rarely spins.
+  u64 *mine = status + (u64) tileid*256 + tid;
+  const unsigned c = digit_offsets(wcount,bexcl,wtot,[&](unsigned total)
+    { if (tileid == 0)
+        atomicExch(mine,ST_INC | total);
       else
-        atomicExch(mine,ST_AGG | c);
-      inc = warp_incl_scan(c,lane);
-      if (lane == 31) wtot[w] = inc;
-    }
-  __syncthreads();
-  if (tid < 256)
-    { unsigned pre = 0;
-      for (int i = 0; i < w; i++) pre += wtot[i];
-      bexcl[tid] = pre + inc - c;
-    }
-  __syncthreads();
+        atomicExch(mine,ST_AGG | total);
+    });
 
 #pragma unroll
   for (int it = 0; it < ITEMS; it++)
     { int idx = base + it*32 + lane;
       if (idx < cnt)
-        { unsigned d = (unsigned) (r[it] >> dsh) & 0xff;
-          tile[bexcl[d] + myc[d] + rank[it]] = r[it];
+        { unsigned d = rec_dig(r[it],dsh);
+          st_rec(tile + (bexcl[d] + myc[d] + rank[it]),r[it]);
         }
     }
   if (tid < 256)
-    { volatile unsigned long long *stt = status;
-      unsigned long long excl = 0;
-      for (long long t = (long long) tileid - 1; t >= 0; )
-        { unsigned long long v[4];
-#pragma unroll
-          for (int q = 0; q < 4; q++)
-            v[q] = (t - q >= 0) ? stt[(unsigned long long) (t - q)*256 + tid] : ST_INC;
-          bool done = false;
-#pragma unroll
-          for (int q = 0; q < 4; q++)
-            { if (done || (v[q] >> 62) == 0) break;
-              excl += v[q] & ST_MASK;
-              t -= 1;
-              if (v[q] & ST_INC) done = true;
-            }
-          if (done) break;
-        }
+    { u64 excl = lookback(status,tileid,tid);
       if (tileid != 0) atomicExch(mine,ST_INC | (excl + c));
       gbase[tid] = binbase[tid] + excl - bexcl[tid];
-      if (next_dsh >= 0 && nhist[tid]) atomicAdd(&nexthist[tid],(unsigned long long) nhist[tid]);
+      if (next_dsh >= 0 && nhist[tid]) atomicAdd(&nexthist[tid],(u64) nhist[tid]);
     }
   __syncthreads();
 
   for (int p = tid; p < cnt; p += SORT_THREADS)
-    { unsigned long long v = tile[p];
-      unsigned long long o = gbase[(unsigned) (v >> dsh) & 0xff] + p;
-      if (OW == 8)
-        reinterpret_cast<unsigned long long *>(out)[o] = v;
-      else
+    { Key v = ld_rec(tile + p);
+      u64 o = gbase[rec_dig(v,dsh)] + p;
+      if constexpr (sizeof(Key) < OW)
         { rec128 R; R.lo = v; R.hi = 0;
           st_rec(reinterpret_cast<rec128 *>(out) + o,R);
         }
+      else
+        st_rec(reinterpret_cast<Key *>(out) + o,v);
     }
 }
 
-template <int IW, int OW>
-static int onesweep64_pass(const void *in, void *out, long long n, int dsh, int next_dsh, const unsigned long long *binbase,
-                           unsigned long long *nexthist, unsigned long long *status, unsigned *ticket,
-                           unsigned long long *hiflag, cudaStream_t st)
-{ typedef os64_tile<IW> T;
+//  The tmp block of a sort (fgb_sort128_tmp_bytes): the look-back status words of a pass (256 per tile
+//  of SORT_TILE records, the smallest tile), the histograms of this pass's digit and the next one, the
+//  bin bases, and a 16-word slot that holds the tile ticket (word 0) and the flag of dropped hi words
+//  (word 1).
+struct sort_tmp
+{ u64 *status, *hist[2], *binbase, *hiflag;
+  unsigned *ticket;
+  sort_tmp(void *d_tmp, long long n)
+    { long long ntiles = (n + SORT_TILE - 1) / SORT_TILE;
+      if (ntiles < 1) ntiles = 1;
+      status  = (u64 *) d_tmp;
+      hist[0] = status + 256ull*ntiles;
+      hist[1] = hist[0] + 256;
+      binbase = hist[1] + 256;
+      ticket  = (unsigned *) (binbase + 256);
+      hiflag  = binbase + 256 + 1;
+    }
+};
+
+extern "C" long long fgb_sort128_tmp_bytes(long long n)
+{ long long ntiles = (n + SORT_TILE - 1) / SORT_TILE;
+  if (ntiles < 1) ntiles = 1;
+  return 256*ntiles*8 + (3*256 + 16)*8;
+}
+
+//  One pass: the bin bases of this pass's histogram (cur), the status words zeroed, the Onesweep kernel.
+template <class Key, int IW, int OW>
+static int onesweep_pass(const void *in, void *out, long long n, int dsh, int next_dsh, const sort_tmp &T, int cur,
+                         cudaStream_t st)
+{ typedef os_tile<IW> O;
   static bool attr_set = false;
   if (!attr_set)
-    { CUDA_TRY(cudaFuncSetAttribute(sort_onesweep64_kernel<IW,OW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) T::SMEM));
+    { CUDA_TRY(cudaFuncSetAttribute(sort_onesweep_kernel<Key,IW,OW>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) O::SMEM));
       attr_set = true;
     }
-  int ntiles = (int) ((n + T::TILE - 1) / T::TILE);
-  CUDA_TRY(cudaMemsetAsync(status,0,256ull*ntiles*8,st));
-  sort_onesweep64_kernel<IW,OW><<<ntiles,SORT_THREADS,T::SMEM,st>>>(in,out,n,dsh,next_dsh,binbase,nexthist,status,ticket,hiflag);
-  fgb_count_launch(1);
+  int ntiles = (int) ((n + O::TILE - 1) / O::TILE);
+  sort_bins_kernel<<<1,256,0,st>>>(T.hist[cur],T.binbase,T.hist[cur^1],T.ticket);
+  CUDA_TRY(cudaMemsetAsync(T.status,0,256ull*ntiles*8,st));
+  sort_onesweep_kernel<Key,IW,OW><<<ntiles,SORT_THREADS,O::SMEM,st>>>(in,out,n,dsh,next_dsh,T.binbase,T.hist[cur^1],
+                                                                     T.status,T.ticket,T.hiflag);
+  fgb_count_launch(2);
   return FGB_OK;
 }
 
-//  Sorts n 16-byte records in d_a on bits [bit_lo,bit_hi) like fgb_sort128_bits_device, for records
-//  whose hi word is zero (bit_hi <= 64).  The two 8-byte ping-pong buffers are the two halves of d_b
-//  (16(n+1) bytes), the result lands in d_a.  *d_flag (device) gets the OR of every hi word the first
-//  pass dropped: non-zero means the records broke the contract and d_a is not sorted.
-extern "C" int fgb_sort_seeds64_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                                       void *d_tmp, long long tmp_bytes, unsigned long long *d_flag, void *stream)
+extern "C" int fgb_radix_sort_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi, int narrow,
+                                     void *d_tmp, long long tmp_bytes, int *result_in_b, u64 **d_hiflag, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  if (n < 0 || bit_lo < 0 || bit_hi > 64 || bit_lo > bit_hi) return FGB_ERR_ARG;
+  if (n < 0 || bit_lo < 0 || bit_hi > (narrow ? 64 : 128) || bit_lo > bit_hi) return FGB_ERR_ARG;
   if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
-  CUDA_TRY(cudaMemsetAsync(d_flag,0,8,st));
+  *result_in_b = 0;
+  const sort_tmp T(d_tmp,n);
+  if (narrow)                                 // the caller reads the flag whether or not anything is sorted
+    { if (tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
+      CUDA_TRY(cudaMemsetAsync(T.hiflag,0,8,st));
+      *d_hiflag = T.hiflag;
+    }
   if (n <= 1 || bit_lo == bit_hi) return FGB_OK;
   if (tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
-  if (bit_hi - bit_lo <= 8)                   // one pass: nothing to narrow
-    { int inb = 0;
-      int rc = fgb_sort128_bits_device(d_a,d_b,n,bit_lo,bit_hi,d_tmp,tmp_bytes,&inb,stream);
-      if (rc) return rc;
-      if (inb) CUDA_TRY(cudaMemcpyAsync(d_a,d_b,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-      return FGB_OK;
-    }
 
-  int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE);       // the carve-up of fgb_sort128_bits_device
-  unsigned long long *status = (unsigned long long *) d_tmp;
-  unsigned long long *hist[2] = { status + 256ull*ntiles, status + 256ull*ntiles + 256 };
-  unsigned long long *binbase = status + 256ull*ntiles + 512;
-  unsigned *ticket = (unsigned *) (binbase + 256);
-  //  the second half starts 16-byte aligned; both halves may be read one word past their end
-  unsigned char *half[2] = { (unsigned char *) d_b, (unsigned char *) d_b + ((8*n + 15) & ~15ll) };
+  const int npass = (bit_hi - bit_lo + 7) / 8;
+  const bool words = narrow && npass >= 2;    // one pass: nothing to narrow, the 128-bit pass runs
+  //  the two 8-byte ping-pong buffers of the narrow plan are the two halves of d_b (16(n+1) bytes); the
+  //  second half starts 16-byte aligned, and both may be read one word past their end
+  void *half[2] = { d_b, (unsigned char *) d_b + ((8*n + 15) & ~15ll) };
 
-  CUDA_TRY(cudaMemsetAsync(hist[0],0,256*8,st));
-  { int nb = ntiles < 1184 ? ntiles : 1184;
-    sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>((const rec128 *) d_a,n,bit_lo,hist[0]);
+  CUDA_TRY(cudaMemsetAsync(T.hist[0],0,256*8,st));
+  { int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE), nb = ntiles < 1184 ? ntiles : 1184;
+    sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>((const rec128 *) d_a,n,bit_lo,T.hist[0]);
     fgb_count_launch(1);
   }
-  int cur = 0, rc = FGB_OK;
-  for (int p = 0, b = bit_lo; b < bit_hi && rc == FGB_OK; p++, b += 8)
-    { const int nd = (b+8 < bit_hi) ? b+8 : -1;
-      sort_bins_kernel<<<1,256,0,st>>>(hist[cur],binbase,hist[cur^1],ticket);
-      fgb_count_launch(1);
-      if (p == 0)
-        rc = onesweep64_pass<16,8>(d_a,half[0],n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
+  int rc = FGB_OK;
+  for (int p = 0; p < npass && rc == FGB_OK; p++)
+    { const int b = bit_lo + 8*p, nd = (p + 1 < npass) ? b + 8 : -1, cur = p & 1;
+      if (!words)
+        rc = onesweep_pass<rec128,16,16>(cur ? d_b : d_a,cur ? d_a : d_b,n,b,nd,T,cur,st);
+      else if (p == 0)
+        rc = onesweep_pass<u64,16,8>(d_a,half[0],n,b,nd,T,cur,st);
       else if (nd >= 0)
-        rc = onesweep64_pass<8,8>(half[(p-1)&1],half[p&1],n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
+        rc = onesweep_pass<u64,8,8>(half[cur^1],half[cur],n,b,nd,T,cur,st);
       else
-        rc = onesweep64_pass<8,16>(half[(p-1)&1],d_a,n,b,nd,binbase,hist[cur^1],status,ticket,d_flag,st);
-      cur ^= 1;
+        rc = onesweep_pass<u64,8,16>(half[cur^1],d_a,n,b,nd,T,cur,st);
     }
   if (rc) return rc;
   CUDA_TRY(cudaGetLastError());
+  if (!words && (npass & 1))
+    { if (narrow)
+        CUDA_TRY(cudaMemcpyAsync(d_a,d_b,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+      else
+        *result_in_b = 1;
+    }
   return FGB_OK;
+}
+
+extern "C" int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
+                                       void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
+{ return fgb_radix_sort_device(d_a,d_b,n,bit_lo,bit_hi,0,d_tmp,tmp_bytes,result_in_b,NULL,stream); }
+
+extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
+                                  void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
+{ if (byte_lo < 0 || byte_hi > 16 || byte_lo > byte_hi) return FGB_ERR_ARG;
+  return fgb_radix_sort_device(d_a,d_b,n,8*byte_lo,8*byte_hi,0,d_tmp,tmp_bytes,result_in_b,NULL,stream);
 }
 
 /***********************************************************************************************
@@ -579,15 +455,6 @@ __global__ void kmer_bins_kernel(const rec128 *__restrict__ tab, long long n, in
   long long hi = (i == n) ? nbins : (long long) ((tab[i].hi >> binshift) - base);
   if (hi > nbins) hi = nbins;
   for (long long p = lo+1; p <= hi; p++) bin_start[p] = (unsigned) i;
-}
-
-//  bin_start[p], p = 0..65536, for bins = hi >> binshift (host-callable)
-extern "C" int fgb_kmer_bins_device(const void *d_tab, long long n, int binshift, unsigned *d_bins, void *stream)
-{ int nb = (int) ((n + 1 + 255) / 256);
-  kmer_bins_kernel<<<nb,256,0,(cudaStream_t) stream>>>((const rec128 *) d_tab,n,binshift,0ull,d_bins,65536ll);
-  fgb_count_launch(1);
-  CUDA_TRY(cudaGetLastError());
-  return FGB_OK;
 }
 
 //  One CTA sorts one group (<= BK_CAP records of <= BK_SPAN consecutive bins) by the full 128-bit
@@ -684,39 +551,9 @@ kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
       for (int it = 0; it < BK_ITEMS; it++)
         { int idx = base + it*32 + lane;
           bool valid = idx < count;
-          unsigned d = valid ? rec_byte(r[it],byte) : 0;
-          unsigned peers = match_digit(d,valid);
-          int leader = valid ? __ffs(peers)-1 : lane;
-          unsigned b = 0;
-          if (valid && lane == leader)
-            { b = myc[d];
-              myc[d] = b + __popc(peers);
-            }
-          b = __shfl_sync(0xffffffffu,b,leader);
-          rank[it] = b + __popc(peers & lanemask_lt());
-          __syncwarp();
+          rank[it] = warp_rank(myc,valid ? rec_byte(r[it],byte) : 0,valid);
         }
-      __syncthreads();
-      unsigned c = 0, inc = 0;
-      if (tid < 256)
-        { unsigned sum = 0;
-#pragma unroll
-          for (int ww = 0; ww < BK_WARPS; ww++)
-            { unsigned t = wcount[ww*256+tid];
-              wcount[ww*256+tid] = sum;
-              sum += t;
-            }
-          c = sum;
-          inc = warp_incl_scan(c,lane);
-          if (lane == 31) wtot[w] = inc;
-        }
-      __syncthreads();
-      if (tid < 256)
-        { unsigned pre = 0;
-          for (int i = 0; i < w; i++) pre += wtot[i];
-          bexcl[tid] = pre + inc - c;
-        }
-      __syncthreads();
+      digit_offsets(wcount,bexcl,wtot,[](unsigned) {});
 #pragma unroll
       for (int it = 0; it < BK_ITEMS; it++)
         { int idx = base + it*32 + lane;
@@ -904,10 +741,6 @@ extern "C" int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long 
   *result_in_b = 1;
   return FGB_OK;
 }
-
-extern "C" int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, void *d_tmp, long long tmp_bytes,
-                                    int *result_in_b, void *stream)
-{ return fgb_kmer_sort_range_device(d_a,d_b,n,0,1u << 24,d_tmp,tmp_bytes,result_in_b,stream); }
 
 /***********************************************************************************************
  *  Generic exclusive scan of a u32 array (reduce / scan-of-sums / downsweep), used for stream

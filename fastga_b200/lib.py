@@ -626,16 +626,6 @@ def kmers_scan(dgenome, mask, fwd_only, stream=None):
     return ptr.value, n.value
 
 
-def records_group_by_top_byte(src_ptr, n, dst_ptr, stream=None):
-    """groups n records by the first four bases of the k-mer into dst; returns bounds[257]"""
-    L = load_library()
-    bounds = np.zeros(257, dtype=np.int64)
-    L.fgb_records_group_by_top_byte.argtypes = [c_void_p, c_ll, c_void_p, c_void_p, c_void_p]
-    _check(L.fgb_records_group_by_top_byte(c_void_p(src_ptr), n, c_void_p(dst_ptr), _ptr(bounds), stream),
-           "fgb_records_group_by_top_byte")
-    return bounds
-
-
 def records_group_by_owner(src_ptr, n, owner256, world, dst_ptr, stream=None):
     """groups n k-mer records by the rank owning their first four bases (owner256[top byte]) into dst;
     returns bounds[world+1]"""

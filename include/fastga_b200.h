@@ -213,10 +213,8 @@ void fgb_device_free(void *p);
 /* unsorted k-mer records of the contigs with mask[c] != 0; fwd_only drops reverse-strand entries */
 int  fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only,
                     void **d_recs, long long *n, void *stream);
-/* d_out[bounds257[b] .. bounds257[b+1]) = the records whose top k-mer byte is b (d_recs is scratch) */
-int  fgb_records_group_by_top_byte(void *d_recs, long long n, void *d_out, long long *bounds257,
-                                   void *stream);
-/* the same by destination only: owner256[b] = rank owning top byte b; d_out[bounds[w] .. bounds[w+1]) */
+/* k-mer records grouped by destination: owner256[b] = rank owning top k-mer byte b; d_out[bounds[w] .. bounds[w+1])
+   holds the records of rank w */
 int  fgb_records_group_by_owner(const void *d_recs, long long n, const int *owner256, int world,
                                 void *d_out, long long *bounds, void *stream);
 /* sorted + indexed table over records whose 12-base prefix lies in [plo,phi) (one rank's slice) */
