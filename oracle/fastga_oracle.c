@@ -970,9 +970,16 @@ uint8_t *orc_result_traces(orc_result *R) { return R->tpool; }
 /*  SELF mode of align_contigs (FastGA.c:3030, :3247-3262): a contig against itself, forward
     strand, is aligned strictly above or strictly below the main diagonal and not at all across
     it.  In that last branch the reference only clears abpos/aepos, so the tube advances with the
-    bepos of the previous alignment (the orc_path below persists across calls, as Path does).  */
-static int g_self = 0;
+    bepos of the previous alignment (the orc_path below persists across calls, as Path does).
+    orc_set_straddle(1) advances it with 0 instead, as the CUDA path does; 0 (the default) is the
+    reference.  orc_self_counters reads what the last search went through: [0] straddles (calls not
+    made), [1] straddles where the previous bepos was past alow (the two advances differ), [2] calls
+    with lbord >= 0, [3] calls with hbord >= 0.  */
+static int g_self = 0, g_straddle_zero = 0;
+static int64_t g_self_cnt[4];
 void orc_set_self(int on) { g_self = on; }
+void orc_set_straddle(int zero) { g_straddle_zero = zero; }
+void orc_self_counters(int64_t *out) { memcpy(out,g_self_cnt,sizeof(g_self_cnt)); }
 
 /* aseq[c], bseq[c]: contig c (ORIGINAL numbering), one base per byte with a sentinel 4 at [-1]
    and [len]; acseq[c]: reverse complement of A contig c, same framing (Complement_Seq). */
@@ -1176,11 +1183,15 @@ static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh,
           int lbord = -1, hbord = -1, called = 1;
           if (g_self && ctg1 == ctg2 && !comp)
             { if (dgmin > 0)
-                lbord = dgmin-1;
+                { lbord = dgmin-1; g_self_cnt[2] += 1; }
               else if (dgmax < 0)
-                hbord = -(dgmax+1);
+                { hbord = -(dgmax+1); g_self_cnt[3] += 1; }
               else
-                { path->abpos = path->aepos = 0; called = 0; }
+                { path->abpos = path->aepos = 0; called = 0;
+                  g_self_cnt[0] += 1;
+                  if (path->bepos > alow) g_self_cnt[1] += 1;
+                  if (g_straddle_zero) path->bbpos = path->bepos = 0;
+                }
             }
           if (called)
             orc_local_alignment(S->work,S->spec,S->as,alen,S->bs,blen,comp,
@@ -1219,6 +1230,7 @@ static int64_t search(const rec128 *seeds, int64_t n, const orc_layout *L, const
   S.log = log; S.work->log = log;
   S.alnMin = P->align_min - 50;
   S.alnRate = P->align_rate + .05;
+  memset(g_self_cnt,0,sizeof(g_self_cnt));
   chain_scan(seeds,n,L,P->chain_break,P->chain_min,search_triple,search_hit,&S);
   free(path.trace);
   orc_free_work(S.work);

@@ -1,5 +1,6 @@
 """TEST INFRASTRUCTURE: ctypes access to oracle/liboracle.so (the CPU restatement), the unmodified
 reference built into oracle/_ref (binaries + libfastga_ref.so) and the stored results of its runs."""
+import contextlib
 import ctypes as C
 import hashlib
 import json
@@ -548,9 +549,36 @@ def oracle_pipeline(gA, gB, rank=None, **kw):
                 lines=al.canonical_lines(), perm1=pa, perm2=pb)
 
 
-def oracle_pipeline_self(g, **kw):
-    """SELF mode (FastGA A) through the CPU oracle + the product's host filter (groundwork for
-    SURVEY row a-7; no CUDA path uses it yet)."""
+SELF_COUNTERS = ("straddles", "stale_straddles", "lbord_calls", "hbord_calls")
+
+
+@contextlib.contextmanager
+def self_search(straddle_zero=False):
+    """search() / search_calls() in SELF mode while inside: a contig against itself, forward strand, gets
+    the band borders of align_contigs and no call across the main diagonal.  straddle_zero: such a
+    straddle advances the tube with 0, as the CUDA path does, instead of the reference's stale bepos."""
+    o = orc()
+    o.orc_set_self(1)
+    o.orc_set_straddle(int(straddle_zero))
+    try:
+        yield
+    finally:
+        o.orc_set_self(0)
+        o.orc_set_straddle(0)
+
+
+def self_counters():
+    """what the last search went through in SELF mode (SELF_COUNTERS): straddles, straddles where the
+    previous bepos lies past the chain's alow (so the two advances differ), calls with lbord >= 0 and
+    calls with hbord >= 0"""
+    out = np.zeros(4, dtype=np.int64)
+    orc().orc_self_counters(out.ctypes.data_as(C.c_void_p))
+    return dict(zip(SELF_COUNTERS, (int(v) for v in out)))
+
+
+def oracle_pipeline_self(g, straddle_zero=False, **kw):
+    """SELF mode (FastGA A) through the CPU oracle + the product's host filter; "counters" holds
+    self_counters() of the search"""
     from fastga_b200 import lib
     pa, ra = contig_rank(g.clen)
     t, s = gix_build(g, ra)
@@ -558,12 +586,10 @@ def oracle_pipeline_self(g, **kw):
     layout = seed_layout(g, g)
     recs = seed_records(seeds, layout)
     skw = {k: v for k, v in kw.items() if k in ("chain_break", "chain_min", "align_min", "align_rate")}
-    o = orc()
-    o.orc_set_self(1)
-    try:
+    with self_search(straddle_zero):
         ov, tp, nhit = search(recs, layout, g, g, pa, pa, g.freq, **skw)
-    finally:
-        o.orc_set_self(0)
+        cnt = self_counters()
     O = pack_overlaps(ov, tp, ra, ra, layout[2], layout[3])
     al = lib.filter_overlaps(O.h, pa, pa, layout[2], layout[3])
-    return dict(nseeds=len(seeds), sumlen=sumlen, nhit=nhit, nraw=len(ov), alns=al, lines=al.canonical_lines())
+    return dict(nseeds=len(seeds), sumlen=sumlen, nhit=nhit, nraw=len(ov), alns=al, lines=al.canonical_lines(),
+                counters=cnt, seedrecs=recs, layout=layout, perm=pa)

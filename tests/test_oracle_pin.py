@@ -241,8 +241,9 @@ def test_oracle_on_example_regions_vs_live_reference(tmp_path):
 
 def _self_genomes():
     """genomes with internal homology for SELF mode (FastGA A): a diverged duplication inside and
-    across contigs plus an inverted copy, and two tandem-repeat genomes (near-diagonal chains: the
-    'nothing across the main diagonal' branch and the band borders of align_contigs)"""
+    across contigs plus an inverted copy, and two tandem-repeat genomes (near-diagonal chains: the band
+    borders of align_contigs).  None of them reaches the 'nothing across the main diagonal' branch:
+    self_cases.py builds the genomes that do."""
     rng = np.random.default_rng(5)
     a = rng.integers(0, 4, 300_000, dtype=np.uint8)
     dup = synth.diverged_copy(rng, a[50_000:150_000], 0.05, sv_every=40_000)
