@@ -215,25 +215,6 @@ static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-
 //  2^24 prefix index.
 
 #define GIX_FWD_ONLY 0x80000000u     // flag bit carried in `phi` down to syncmer_kernel
-#define GIX_NO_INDEX 0x40000000u     // table only: no prefix index, no LCP bytes (the T1 side of a merge reads neither)
-
-static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi, fgb_gix **out, void *stream);
-
-extern "C" int fgb_gix_build(const fgb_genome *g, fgb_gix **out, void *stream)
-{ return gix_build_range(g,0u,1u << 24,out,stream); }
-
-//  Forward-strand entries only: the table of the genome that supplies the adaptamers.  Reverse
-//  entries of T1 never seed (FastGA.c:921-928), so the fused path does not build, sort or read them.
-extern "C" int fgb_gix_build_forward(const fgb_genome *g, fgb_gix **out, void *stream)
-{ return gix_build_range(g,0u,(1u << 24) | GIX_FWD_ONLY,out,stream); }
-
-//  Only the k-mers whose 12-base prefix lies in [plo,phi): one rank's share of a table that is
-//  built cooperatively (every rank scans the genome, sorts 1/N of the records, the sorted shares
-//  concatenate in rank order -- fastga_b200/shard.py all-gathers them over NCCL).
-extern "C" int fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi, fgb_gix **out, void *stream)
-{ if (plo > phi || phi > (1u << 24)) return FGB_ERR_ARG;
-  return gix_build_range(g,plo,phi,out,stream);
-}
 
 //  The fine prefix bins a table's scan lays its records out by (fgb_kmer_sort_fine_binned_device):
 //  bin f = (prefix24 >> fsh) - (plo >> fsh) holds records [start[f], start[f+1]), f < nf.
@@ -355,10 +336,10 @@ static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo,
   return FGB_OK;
 }
 
-static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags, fgb_gix **out, void *stream)
+//  index = false: the table only, without prefix index and LCP bytes (the T1 side of a merge reads neither)
+static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags, bool index, fgb_gix **out,
+                           void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  const bool index = !(phi_flags & GIX_NO_INDEX);
-  phi_flags &= ~GIX_NO_INDEX;
   const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
   std::unique_ptr<fgb_gix> x(new fgb_gix());
   gix_bytes(g,x.get());
@@ -375,6 +356,21 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
   if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,pfb,st,index))) return rc;
   *out = x.release();
   return FGB_OK;
+}
+
+extern "C" int fgb_gix_build(const fgb_genome *g, fgb_gix **out, void *stream)
+{ return gix_build_range(g,0u,1u << 24,true,out,stream); }
+
+//  Forward-strand entries only: the table of the genome that supplies the adaptamers.  Reverse
+//  entries of T1 never seed (FastGA.c:921-928), so the fused path does not build, sort or read them.
+extern "C" int fgb_gix_build_forward(const fgb_genome *g, fgb_gix **out, void *stream)
+{ return gix_build_range(g,0u,(1u << 24) | GIX_FWD_ONLY,true,out,stream); }
+
+//  Only the k-mers whose 12-base prefix lies in [plo,phi): one prefix range of a table, binned and
+//  sorted relative to plo.
+extern "C" int fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi, fgb_gix **out, void *stream)
+{ if (plo > phi || phi > (1u << 24)) return FGB_ERR_ARG;
+  return gix_build_range(g,plo,phi,true,out,stream);
 }
 
 /***********************************************************************************************
@@ -414,34 +410,6 @@ extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned pl
 }
 
 extern "C" long long fgb_gix_size(const fgb_gix *x) { return x->n; }
-
-//  device-to-device copy of the sorted records into a caller-owned device buffer (n x 16 bytes)
-extern "C" int fgb_gix_copy_table(const fgb_gix *x, void *d_dst, void *stream)
-{ CUDA_TRY(cudaMemcpyAsync(d_dst,x->d_tab,sizeof(rec128)*x->n,cudaMemcpyDeviceToDevice,(cudaStream_t) stream));
-  CUDA_TRY(cudaStreamSynchronize((cudaStream_t) stream));
-  return FGB_OK;
-}
-
-//  A GIX over sorted device-layout records that already sit in device memory (copied).
-extern "C" int fgb_gix_from_device(const void *d_tab, long long n, int post_bytes, int cont_bytes,
-                                   int ncontig, fgb_gix **out, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  if (n >= 0xfffffff0ll) return FGB_ERR_LIMIT;
-  std::unique_ptr<fgb_gix> x(new fgb_gix());
-  x->n = n; x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
-  CUDA_TRY(x->d_tab.alloc(n+1,st));
-  CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
-  CUDA_TRY(x->d_adj.alloc((size_t) x->n + 32,st));
-  CUDA_TRY(cudaMemcpyAsync(x->d_tab,d_tab,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-  int rc;
-  { stage_timer t(&g_timings.index_ms,st);
-    rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
-  }
-  CUDA_TRY(cudaStreamSynchronize(st));
-  if (rc) return rc;
-  *out = x.release();
-  return FGB_OK;
-}
 extern "C" int fgb_gix_post_bytes(const fgb_gix *x) { return x->post_bytes; }
 extern "C" int fgb_gix_cont_bytes(const fgb_gix *x) { return x->cont_bytes; }
 
@@ -735,131 +703,86 @@ struct fgb_run_stats
             us_gix, us_seeds, us_extend, us_filter, nkmers1_fwd,
             slow_cycles, slow_waves, paired_waves, pairings; };
 
-static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
-                             std::unique_ptr<fgb_gix> *own, const float *freqA, int freq, int chain_break,
-                             int chain_min, int align_min, double align_rate, fgb_alns **out,
-                             fgb_run_stats *stats, void *stream);
-
-//  Device-resident genomes in, final alignments out (the timed "step" of bench.py).
-extern "C" int fgb_align_resident(const fgb_genome *A, const fgb_genome *B, const float *freqA,
-                                  int freq, int chain_break, int chain_min, int align_min,
-                                  double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ std::unique_ptr<fgb_gix> x[2];
-  fgb_gix *p = NULL;
+//  The whole path on staged genomes: k-mer tables -> adaptamer merge -> seed sort -> extension -> filter.
+//  self: SELF mode (`FastGA A`, B == A): one both-strand table merged against itself by the self block
+//  rule, and the band borders of align_contigs for a contig against itself.
+static int align_pipeline(const fgb_genome *A, const fgb_genome *B, bool self, const float *freqA, int freq,
+                          int chain_break, int chain_min, int align_min, double align_rate, fgb_alns **out,
+                          fgb_run_stats *stats, cudaStream_t st)
+{ fgb_run_stats s = {};
+  fgb_seeds *ps = NULL; fgb_overlaps *po = NULL;
   int rc;
-  long long t0 = now_us();
-  //  adaptamer side: forward strand only, and only the table (the merge reads the OTHER table's index)
-  if ((rc = gix_build_range(A,0u,(1u << 24) | GIX_FWD_ONLY | GIX_NO_INDEX,&p,stream))) return rc;
-  x[0].reset(p);
-  if ((rc = fgb_gix_build(B,&p,stream))) return rc;
-  x[1].reset(p);
-  long long t1 = now_us();
-  //  the tables are this call's own: they go back to the allocator as soon as the merge has read them
-  //  (two tables + seeds + sort buffer of a multi-Gbp pair do not fit side by side)
-  rc = align_tables_impl(A,B,x[0].get(),x[1].get(),x,freqA,freq,chain_break,chain_min,align_min,align_rate,
-                         out,stats,stream);
-  if (stats) stats->us_gix = t1 - t0;
-  return rc;
-}
-
-//  Merge + seed sort + extension + filter from prebuilt tables (x2 may have been assembled from
-//  shares built on several ranks).
-extern "C" int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1,
-                                const fgb_gix *x2, const float *freqA,
-                                int freq, int chain_break, int chain_min, int align_min,
-                                double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ return align_tables_impl(A,B,x1,x2,NULL,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream); }
-
-//  own: the two table handles when they are this call's to release (right after the merge), else NULL
-static int align_tables_impl(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
-                             std::unique_ptr<fgb_gix> *own, const float *freqA, int freq, int chain_break,
-                             int chain_min, int align_min, double align_rate, fgb_alns **out,
-                             fgb_run_stats *stats, void *stream)
-{ fgb_seeds *ps = NULL; fgb_overlaps *po = NULL;
-  int rc;
-  long long t0 = now_us(), t1 = t0, t2, t3, t4;
-  const long long n1 = x1->n_both, n2 = x2->n;
-  { seed_bits L;
-    dblock<rec128> d_a; long long n = 0, sumlen = 0, n1m = 0;
-    rc = seed_layout_of(x1,x2,A->maxlen,B->maxlen,&L);
-    if (!rc) rc = seeds_merge_impl(x1,x2,A->maxlen,B->maxlen,freq,false,L,d_a,&n,&sumlen,&n1m,(cudaStream_t) stream);
-    if (own) { own[0].reset(); own[1].reset(); }
-    if (!rc) rc = seeds_sort_impl(std::move(d_a),n,L,A->maxlen,B->maxlen,false,sumlen,n1m,&ps,(cudaStream_t) stream);
+  long long t0 = now_us(), t1, t2, t3, t4;
+  { std::unique_ptr<fgb_gix> x1, x2;
+    fgb_gix *p = NULL;
+    //  pair: the adaptamer side forward strand only, and only the table (the merge reads B's index)
+    if ((rc = gix_build_range(A,0u,(1u << 24) | (self ? 0u : GIX_FWD_ONLY),self,&p,st))) return rc;
+    x1.reset(p);
+    if (!self)
+      { if ((rc = gix_build_range(B,0u,1u << 24,true,&p,st))) return rc;
+        x2.reset(p);
+      }
+    const fgb_gix *xb = self ? x1.get() : x2.get();
+    t1 = now_us();
+    s.nkmers1 = x1->n_both; s.nkmers2 = xb->n;
+    seed_bits L;
+    dblock<rec128> d_a; long long n = 0;
+    rc = seed_layout_of(x1.get(),xb,A->maxlen,B->maxlen,&L);
+    if (!rc) rc = seeds_merge_impl(x1.get(),xb,A->maxlen,B->maxlen,freq,self,L,d_a,&n,&s.sumlen,&s.nkmers1_fwd,st);
+    //  the tables go back to the allocator as soon as the merge has read them (two tables + seeds + sort
+    //  buffer of a multi-Gbp pair do not fit side by side)
+    x1.reset(); x2.reset();
+    if (!rc) rc = seeds_sort_impl(std::move(d_a),n,L,A->maxlen,B->maxlen,self,s.sumlen,s.nkmers1_fwd,&ps,st);
   }
   if (rc) return rc;
   std::unique_ptr<fgb_seeds> sd(ps);
-  const long long n1f = sd->n1_merged;
+  s.nseeds = sd->n;
   t2 = now_us();
-  short *tables = (short *) malloc(65536*sizeof(short));
+  std::vector<short> tables(65536);
   int ave = 0;
-  fgb_align_spec(1.-align_rate,freqA,tables,&ave);           // FastGA.c:3760
-  rc = fgb_extend(sd.get(),A,B,chain_break,chain_min,align_min,align_rate,tables,ave,100,&po,stream);
-  free(tables);
+  fgb_align_spec(1.-align_rate,freqA,tables.data(),&ave);           // FastGA.c:3760
+  rc = fgb_extend(sd.get(),A,B,chain_break,chain_min,align_min,align_rate,tables.data(),ave,100,&po,st);
   t3 = now_us();
-  long long nseeds = sd->n, sumlen = sd->sumlen;
-  int jb = sd->jc_bits, ib = sd->ic_bits;
+  const int jb = sd->jc_bits, ib = sd->ic_bits;
   sd.reset();
   if (rc) return rc;
   std::unique_ptr<fgb_overlaps> ov(po);
   rc = fgb_filter(ov.get(),A->perm.data(),B->perm.data(),jb,ib,1,out);
   t4 = now_us();
-  if (stats)
-    { stats->us_gix = t1-t0; stats->us_seeds = t2-t1; stats->us_extend = t3-t2; stats->us_filter = t4-t3; unsigned long long c[16];
-      fgb_overlaps_counters(ov.get(),c);
-      stats->nkmers1 = n1; stats->nkmers2 = n2; stats->nseeds = nseeds; stats->sumlen = sumlen;
-      stats->nkmers1_fwd = n1f;
-      stats->nhits = (long long) c[0]; stats->nla = (long long) c[1]; stats->nwaves = (long long) c[2];
-      stats->ncells = (long long) c[3]; stats->nraw = 0;
-      stats->nseg = (long long) c[5]; stats->nwork = (long long) c[6];
-      stats->warp_cycles = (long long) c[8]; stats->wave_cycles = (long long) c[9];
-      stats->extract_cycles = (long long) c[10];
-      stats->slow_cycles = (long long) ((c[15] >> 40) << 12); stats->slow_waves = (long long) ((c[15] >> 16) & 0xffffff);
-      stats->paired_waves = (long long) c[11]; stats->pairings = (long long) c[12];
-      stats->h2d_bytes = A->h2d_bytes + B->h2d_bytes + 65536*2;
-      stats->d2h_bytes = fgb_overlaps_bytes(ov.get()) + 16 + 8*1024*2 + 64;
-    }
+  unsigned long long c[16];
+  fgb_overlaps_counters(ov.get(),c);
+  s.us_gix = t1-t0; s.us_seeds = t2-t1; s.us_extend = t3-t2; s.us_filter = t4-t3;
+  s.nhits = (long long) c[0]; s.nla = (long long) c[1]; s.nwaves = (long long) c[2]; s.ncells = (long long) c[3];
+  s.nseg = (long long) c[5]; s.nwork = (long long) c[6];
+  s.warp_cycles = (long long) c[8]; s.wave_cycles = (long long) c[9]; s.extract_cycles = (long long) c[10];
+  s.slow_cycles = (long long) ((c[15] >> 40) << 12); s.slow_waves = (long long) ((c[15] >> 16) & 0xffffff);
+  s.paired_waves = (long long) c[11]; s.pairings = (long long) c[12];
+  s.h2d_bytes = A->h2d_bytes + (self ? 0 : B->h2d_bytes) + 65536*2;
+  s.d2h_bytes = fgb_overlaps_bytes(ov.get()) + 16 + 8*1024*(self ? 1 : 2) + 64;    // 8 KB of bucket counts per table
+  if (stats) *stats = s;
   return rc;
 }
 
-//  The reference-facing call: host .bps images + contig tables in, alignments out; every
+//  Device-resident genomes in, final alignments out (the timed "step" of bench.py).
+extern "C" int fgb_align_resident(const fgb_genome *A, const fgb_genome *B, const float *freqA,
+                                  int freq, int chain_break, int chain_min, int align_min,
+                                  double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream)
+{ return align_pipeline(A,B,false,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,
+                        (cudaStream_t) stream);
+}
+
+//  The reference-facing calls: host .bps images + contig tables in, alignments out; every
 //  host<->device copy happens inside.
-//  SELF mode: `FastGA A` (one source).  Same path with T2 = T1, BMXPOS = AMXPOS, the self block rule
-//  in the merge and the band borders of align_contigs for a contig against itself.
 extern "C" int fgb_fastga_self(const unsigned char *bps, long long nb, int nc, const long long *clen,
                                const long long *boff, const float *freq4,
                                int freq, int chain_break, int chain_min, int align_min, double align_rate,
                                fgb_alns **out, fgb_run_stats *stats, void *stream)
-{ fgb_genome *pA = NULL; fgb_gix *px = NULL; fgb_seeds *ps = NULL; fgb_overlaps *po = NULL;
+{ fgb_genome *p = NULL;
   int rc;
-  if ((rc = fgb_genome_create(bps,nb,nc,clen,boff,1,&pA,stream))) return rc;
-  std::unique_ptr<fgb_genome> A(pA);
-  if ((rc = fgb_gix_build(A.get(),&px,stream))) return rc;
-  std::unique_ptr<fgb_gix> x(px);
-  rc = fgb_seeds_find_self(x.get(),A->maxlen,freq,&ps,stream);
-  long long n1 = x->n;
-  x.reset();
-  if (rc) return rc;
-  std::unique_ptr<fgb_seeds> sd(ps);
-  short *tables = (short *) malloc(65536*sizeof(short));
-  int ave = 0;
-  fgb_align_spec(1.-align_rate,freq4,tables,&ave);
-  rc = fgb_extend(sd.get(),A.get(),A.get(),chain_break,chain_min,align_min,align_rate,tables,ave,100,&po,stream);
-  free(tables);
-  long long nseeds = sd->n, sumlen = sd->sumlen;
-  int jb = sd->jc_bits, ib = sd->ic_bits;
-  sd.reset();
-  if (rc) return rc;
-  std::unique_ptr<fgb_overlaps> ov(po);
-  rc = fgb_filter(ov.get(),A->perm.data(),A->perm.data(),jb,ib,1,out);
-  if (stats)
-    { memset(stats,0,sizeof(*stats));
-      unsigned long long c[16];
-      fgb_overlaps_counters(ov.get(),c);
-      stats->nkmers1 = stats->nkmers2 = n1; stats->nseeds = nseeds; stats->sumlen = sumlen;
-      stats->nhits = (long long) c[0]; stats->nla = (long long) c[1]; stats->nwaves = (long long) c[2];
-      stats->ncells = (long long) c[3];
-    }
-  return rc;
+  if ((rc = fgb_genome_create(bps,nb,nc,clen,boff,1,&p,stream))) return rc;
+  std::unique_ptr<fgb_genome> A(p);
+  return align_pipeline(A.get(),A.get(),true,freq4,freq,chain_break,chain_min,align_min,align_rate,out,stats,
+                        (cudaStream_t) stream);
 }
 
 extern "C" int fgb_fastga(const unsigned char *bpsA, long long nbA, int ncA, const long long *clenA,
@@ -874,5 +797,6 @@ extern "C" int fgb_fastga(const unsigned char *bpsA, long long nbA, int ncA, con
   std::unique_ptr<fgb_genome> A(p);
   if ((rc = fgb_genome_create(bpsB,nbB,ncB,clenB,boffB,0,&p,stream))) return rc;
   std::unique_ptr<fgb_genome> B(p);
-  return fgb_align_resident(A.get(),B.get(),freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,stream);
+  return align_pipeline(A.get(),B.get(),false,freqA,freq,chain_break,chain_min,align_min,align_rate,out,stats,
+                        (cudaStream_t) stream);
 }

@@ -131,20 +131,6 @@ class DeviceGix:
         return cls(h)
 
     @classmethod
-    def from_device(cls, dev_ptr, n, post_bytes, cont_bytes, ncontig, stream=None):
-        L = load_library()
-        h = c_void_p()
-        L.fgb_gix_from_device.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, C.POINTER(c_void_p), c_void_p]
-        _check(L.fgb_gix_from_device(c_void_p(dev_ptr), n, post_bytes, cont_bytes, ncontig, C.byref(h), stream),
-               "fgb_gix_from_device")
-        return cls(h)
-
-    def copy_table_to(self, dev_ptr, stream=None):
-        L = load_library()
-        L.fgb_gix_copy_table.argtypes = [c_void_p, c_void_p, c_void_p]
-        _check(L.fgb_gix_copy_table(self.h, c_void_p(dev_ptr), stream), "fgb_gix_copy_table")
-
-    @classmethod
     def upload(cls, tab, post_bytes, cont_bytes, ncontig, stream=None):
         L = load_library()
         h = c_void_p()
@@ -461,72 +447,41 @@ def _alns_out(h):
     return Alignments(fields, toff, pool, nraw)
 
 
+def _whole_path(name, argtypes, args, stream, kw):
+    """calls the whole-path entry point `name` on args + the DEFAULTS-merged parameters -> (Alignments, stats)"""
+    p = dict(DEFAULTS)
+    p.update(kw)
+    L = load_library()
+    h = c_void_p()
+    st = RunStats()
+    fn = getattr(L, name)
+    fn.argtypes = argtypes + [c_int, c_int, c_int, c_int, C.c_double, C.POINTER(c_void_p), C.POINTER(RunStats),
+                              c_void_p]
+    _check(fn(*args, p["freq"], p["chain_break"], p["chain_min"], p["align_min"], float(p["align_rate"]),
+              C.byref(h), C.byref(st), stream), name)
+    return _alns_out(h), st.asdict()
+
+
 def align_resident(dA, dB, freqA, stream=None, **kw):
     """Whole path from device-resident genomes: returns (Alignments, stats dict)"""
-    p = dict(DEFAULTS)
-    p.update(kw)
-    L = load_library()
-    h = c_void_p()
-    st = RunStats()
     f = np.ascontiguousarray(freqA, dtype=np.float32)
-    L.fgb_align_resident.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, C.c_double,
-                                     C.POINTER(c_void_p), C.POINTER(RunStats), c_void_p]
-    _check(L.fgb_align_resident(dA.h, dB.h, _ptr(f), p["freq"], p["chain_break"], p["chain_min"],
-                                p["align_min"], float(p["align_rate"]), C.byref(h), C.byref(st), stream),
-           "fgb_align_resident")
-    return _alns_out(h), st.asdict()
-
-
-def align_tables(dA, dB, xA, xB, freqA, stream=None, **kw):
-    """merge + seed sort + extension + filter from prebuilt tables"""
-    p = dict(DEFAULTS)
-    p.update(kw)
-    L = load_library()
-    h = c_void_p()
-    st = RunStats()
-    f = np.ascontiguousarray(freqA, dtype=np.float32)
-    L.fgb_align_tables.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int,
-                                   C.c_double, C.POINTER(c_void_p), C.POINTER(RunStats), c_void_p]
-    _check(L.fgb_align_tables(dA.h, dB.h, xA.h, xB.h, _ptr(f), p["freq"], p["chain_break"], p["chain_min"],
-                              p["align_min"], float(p["align_rate"]), C.byref(h), C.byref(st), stream),
-           "fgb_align_tables")
-    return _alns_out(h), st.asdict()
+    return _whole_path("fgb_align_resident", [c_void_p, c_void_p, c_void_p], (dA.h, dB.h, _ptr(f)), stream, kw)
 
 
 def fastga_self(g, stream=None, **kw):
     """SELF mode, `FastGA A` with one source (formats.Genome) -> (Alignments, stats)"""
-    p = dict(DEFAULTS)
-    p.update(kw)
-    L = load_library()
-    h = c_void_p()
-    st = RunStats()
     f = np.ascontiguousarray(g.freq, dtype=np.float32)
-    L.fgb_fastga_self.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p,
-                                  c_int, c_int, c_int, c_int, C.c_double,
-                                  C.POINTER(c_void_p), C.POINTER(RunStats), c_void_p]
-    _check(L.fgb_fastga_self(_ptr(g.bps), g.bps.size, g.ncontig, _ptr(g.clen), _ptr(g.boff), _ptr(f),
-                             p["freq"], p["chain_break"], p["chain_min"], p["align_min"], float(p["align_rate"]),
-                             C.byref(h), C.byref(st), stream), "fgb_fastga_self")
-    return _alns_out(h), st.asdict()
+    return _whole_path("fgb_fastga_self", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p],
+                       (_ptr(g.bps), g.bps.size, g.ncontig, _ptr(g.clen), _ptr(g.boff), _ptr(f)), stream, kw)
 
 
 def fastga(gA, gB, stream=None, **kw):
     """The reference-facing call on host buffers (formats.Genome x2) -> (Alignments, stats)"""
-    p = dict(DEFAULTS)
-    p.update(kw)
-    L = load_library()
-    h = c_void_p()
-    st = RunStats()
     f = np.ascontiguousarray(gA.freq, dtype=np.float32)
-    L.fgb_fastga.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p,
-                             c_void_p, c_ll, c_int, c_void_p, c_void_p,
-                             c_int, c_int, c_int, c_int, C.c_double,
-                             C.POINTER(c_void_p), C.POINTER(RunStats), c_void_p]
-    _check(L.fgb_fastga(_ptr(gA.bps), gA.bps.size, gA.ncontig, _ptr(gA.clen), _ptr(gA.boff), _ptr(f),
-                        _ptr(gB.bps), gB.bps.size, gB.ncontig, _ptr(gB.clen), _ptr(gB.boff),
-                        p["freq"], p["chain_break"], p["chain_min"], p["align_min"], float(p["align_rate"]),
-                        C.byref(h), C.byref(st), stream), "fgb_fastga")
-    return _alns_out(h), st.asdict()
+    return _whole_path("fgb_fastga", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_ll, c_int, c_void_p, c_void_p],
+                       (_ptr(gA.bps), gA.bps.size, gA.ncontig, _ptr(gA.clen), _ptr(gA.boff), _ptr(f),
+                        _ptr(gB.bps), gB.bps.size, gB.ncontig, _ptr(gB.clen), _ptr(gB.boff)), stream, kw)
 
 
 def compute_trace_pts(dA, dB, alns, tspace=100, stream=None, with_bad=False):

@@ -38,11 +38,13 @@ typedef struct fgb_overlaps fgb_overlaps;  /* raw local alignments, host residen
 typedef struct fgb_alns     fgb_alns;      /* final alignments in .1aln order, host resident   */
 typedef struct fgb_scripts  fgb_scripts;   /* explicit edit scripts of alignments, host resident */
 
+/* counts and times of one whole-path call; every field means the same in SELF mode, where table 2 is
+ * table 1 and h2d_bytes counts the one genome's image once */
 typedef struct
 { long long nkmers1, nkmers2, nseeds, sumlen, nhits, nla, nwaves, ncells, nraw, h2d_bytes, d2h_bytes,
             nseg, nwork, warp_cycles, wave_cycles, extract_cycles,
             us_gix, us_seeds, us_extend, us_filter,      /* host wall microseconds per phase */
-            nkmers1_fwd,                                 /* forward-strand entries of table 1 (what the merge reads) */
+            nkmers1_fwd,                                 /* entries of table 1 the merge reads (forward strand; SELF: all) */
             slow_cycles, slow_waves,                     /* the extension warp that finished last: its cycles and waves */
             paired_waves, pairings;                      /* waves run by front/back warp pairs, passes handed to a pair */
 } fgb_run_stats;
@@ -82,11 +84,6 @@ int fgb_align_resident(const fgb_genome *A, const fgb_genome *B, const float *fr
                        int freq, int chain_break, int chain_min, int align_min, double align_rate,
                        fgb_alns **out, fgb_run_stats *stats, void *stream);
 
-/* Same from prebuilt tables (x2 possibly assembled from per-rank shares). */
-int fgb_align_tables(const fgb_genome *A, const fgb_genome *B, const fgb_gix *x1, const fgb_gix *x2,
-                     const float *freqA, int freq, int chain_break, int chain_min, int align_min,
-                     double align_rate, fgb_alns **out, fgb_run_stats *stats, void *stream);
-
 /* ---- genome (GDB.h:28-72; Get_Contig / Get_Contig_Piece GDB.c:1739,1841; Complement_Seq) ---- */
 int  fgb_genome_create(const unsigned char *bps, long long bps_bytes, int ncontig,
                        const long long *clen, const long long *boff, int want_revcomp,
@@ -104,12 +101,9 @@ int  fgb_gix_build(const fgb_genome *g, fgb_gix **out, void *stream);
 /* forward-strand entries only: enough for the genome that supplies the adaptamers (its reverse
    entries never seed, FastGA.c:921-928); fgb_seeds_find compacts a both-strand table itself */
 int  fgb_gix_build_forward(const fgb_genome *g, fgb_gix **out, void *stream);
-/* one rank's share (12-base prefix in [plo,phi)) of a cooperatively built table, and the pieces
-   to assemble the shares gathered over NCCL (fastga_b200/shard.py) */
+/* one prefix range of a table: the entries whose 12-base prefix lies in [plo,phi), binned and sorted
+   relative to plo (the tests pin ranged scans and sorts through it) */
 int  fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi, fgb_gix **out, void *stream);
-int  fgb_gix_copy_table(const fgb_gix *x, void *d_dst, void *stream);
-int  fgb_gix_from_device(const void *d_tab, long long n, int post_bytes, int cont_bytes, int ncontig,
-                         fgb_gix **out, void *stream);
 int  fgb_gix_upload(const void *tab, long long n, int post_bytes, int cont_bytes, int ncontig,
                     fgb_gix **out, void *stream);
 /* entries = concatenated .ktab parts, index = the stub's cumulative 2^24 table (libfastk.c:815-840) */

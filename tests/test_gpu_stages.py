@@ -101,8 +101,8 @@ def test_gix_build_with_more_than_65536_bins_is_the_same_table(small_pair, targe
 
 
 def test_gix_shares_of_the_prefix_space_concatenate_to_the_full_table(small_pair):
-    """one rank's share of a cooperatively built table (fgb_gix_build_range) is binned relative to
-    its own prefix range; uneven shares must concatenate to exactly the single-GPU table"""
+    """one prefix range of a table (fgb_gix_build_range) is binned relative to its own range; uneven
+    ranges must concatenate to exactly the whole table"""
     g = small_pair[1]
     dg = lib.DeviceGenome(g)
     full, _, _ = lib.DeviceGix.build(dg).download()
