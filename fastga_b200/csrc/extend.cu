@@ -2308,6 +2308,24 @@ static long long launch_blocks(long long n, int per_block, long long limit, long
   return nb < 1 ? 1 : nb;
 }
 
+//  Sizes of the first step of the retry ladders, or what a test sets to force the ladder's later steps
+//  (read on every call, so a test can set and clear them in one process): FGB_EXTEND_CELLS pebbles and
+//  FGB_EXTEND_STAGE staging bytes per warp, FGB_EXTEND_OUT_SLACK bytes of record buffer beyond what is
+//  known to be needed.  The clamps keep every arena check of the kernels in front of its writes:
+//  - pebbles, 32: each site that drops pebbles (wave(), wave_P) tests avail + 32 > cmax and then writes
+//    at most 32 cells from avail; PebWalk reads only cells[0..idx] of pebbles already written;
+//  - staging, 2: the forward read-out writes pairs downwards from smax & ~1 behind pos < 2, the reverse one
+//    behind 2 > smax and 2*npairs > smax, but folding a pair into the first forward pair writes
+//    fstage[0..1] unchecked (rev_extract), which needs two bytes of the warp's own forward half;
+//  - record slack, 64: emit_record writes only when off + need <= out_cap, so any size is safe; the clamp
+//    keeps the record buffer non-empty.
+static long long ladder_knob(const char *name, long long dflt, long long lo)
+{ const char *s = getenv(name);
+  if (s == NULL) return dflt;
+  const long long v = atoll(s);
+  return v < lo ? lo : v;
+}
+
 //  The per-warp arenas of a launch on nwarps warps: pebbles, trace staging and, for the wide-band
 //  kernels, the wave state in HBM.  alloc() points P at them.
 struct Arenas
@@ -2344,6 +2362,7 @@ struct ExtendOut
 { dblock<unsigned char> buf; u64 cap = 0, used = 0;        // the records, as the device packed them
   std::vector<std::pair<unsigned,int> > rerun;            // (triple, launch number) of every re-run
   unsigned long long hits_done = 0;                       // hits of the hit groups, counted by the host
+  long long launches = 0, regrowths = 0; unsigned reasons = 0;   // fgb_overlaps_retry_info
 };
 
 //  Phase 1: the band segments of the sorted seeds (P.seg_start, P.nseg), the prefilter, and the work
@@ -2491,7 +2510,8 @@ static void first_items(unsigned nwork, ExtendPlan &X)
 //  the items that failed (an arena overflowed: ST_*) and, after the hit-group launch, of every group whose
 //  tube reached the next group's first hit make the next list: each triple whole, hit after hit, on the
 //  wide-band kernel with larger arenas on fewer warps; collect_records drops what they emitted in
-//  earlier launches.  A launch that overflows the record buffer is repeated with a larger one.
+//  earlier launches.  A launch that overflows the record buffer is repeated with a larger one, as the
+//  same step: its records keep the step's launch number and its counts are taken back.
 static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc, ExtendOut &R, cudaStream_t st)
 { if (X.items.empty()) return FGB_OK;
   int dev = 0, nsm = 132;
@@ -2504,8 +2524,9 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
   int bps = 0;
   CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&bps,extend_kernel<EX_W>,EX_WARPS*32,smem));
   if (bps < 1) bps = 1;
-  long long cells_per_warp = 1ll << 17;          // 128 K pebbles = 2 MB per warp
-  int stage_bytes = 1 << 15;
+  long long cells_per_warp = ladder_knob("FGB_EXTEND_CELLS",1ll << 17,32);        // 128 K pebbles = 2 MB per warp
+  int stage_bytes = (int) ladder_knob("FGB_EXTEND_STAGE",1 << 15,2);
+  const long long slack = ladder_knob("FGB_EXTEND_OUT_SLACK",-1,64);            // -1: not set
   long long nblocks = launch_blocks((long long) X.items.size(),EX_NFRONT,(long long) nsm * bps,cells_per_warp);
 
   //  a re-run list holds one item per triple of the list before it, so no list outgrows the first
@@ -2520,16 +2541,20 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
   CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
   P.items = d_items; P.failed = d_failed; P.galast = d_galast;
   P.queue = d_misc + 1; P.nfailed = d_misc + 2; P.out_used = (u64 *) (d_misc + 4); P.need = d_misc + 10;
-  R.cap = (u64) P.nwork * 512 + (64ull << 20);
+  R.cap = slack < 0 ? (u64) P.nwork * 512 + (64ull << 20) : (u64) slack;
   CUDA_TRY(R.buf.alloc(R.cap,st));
+  dblock<u64> d_snap;                            // the counters before a launch: a repeated launch counts nothing
+  CUDA_TRY(d_snap.alloc(16,st));
   u64 used_before = 0;
-  for (int attempt = 0; ; attempt++)
+  int repeats = 0;                               // of this step, for want of record buffer
+  for (int attempt = 0; ; )
     { Arenas ar;
       CUDA_TRY(ar.alloc(P,nblocks * EX_WARPS,cells_per_warp,stage_bytes,attempt > 0,st));
       P.out = R.buf; P.out_cap = R.cap;
       P.nitems = (int) items.size(); P.groups = groups; P.attempt = attempt;
       CUDA_TRY(cudaMemsetAsync(d_misc+1,0,8,st));          // queue, nfailed
       CUDA_TRY(cudaMemsetAsync(d_misc+10,0,4,st));         // reasons of this attempt's failures
+      CUDA_TRY(cudaMemcpyAsync(d_snap,P.counters,16*8,cudaMemcpyDeviceToDevice,st));
       { ev_timer t(1,st);
         if (attempt == 0)
           extend_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P);
@@ -2538,26 +2563,31 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       }
       fgb_count_launch(1);
       CUDA_TRY(cudaGetLastError());
+      R.launches += 1;
       unsigned misc[12];
       CUDA_TRY(cudaMemcpyAsync(misc,d_misc,48,cudaMemcpyDeviceToHost,st));
       if (groups) CUDA_TRY(cudaMemcpyAsync(ga.data(),d_galast,sizeof(long long)*items.size(),cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaStreamSynchronize(st));
       ar.reset();                                          // before the record buffer may grow
+      R.reasons |= misc[10];
       R.used = ((u64) misc[5] << 32) | misc[4];
       if (R.used > R.cap)
-        { //  record buffer too small: grow it (keeping earlier attempts' records) and repeat this attempt
-          if (attempt > 12) return FGB_ERR_OVERFLOW;
+        { //  record buffer too small: grow it (keeping earlier steps' records) and repeat this step as it
+          //  was -- same kernel, arenas and launch number, the counters of before it.  The repeat asks for
+          //  the bytes this launch asked for, so one regrowth is enough; the limit only stops a loop.
+          if (++repeats > 2) return FGB_ERR_OVERFLOW;
+          R.regrowths += 1;
           dblock<unsigned char> d_new;
-          const u64 ncap = R.used * 2 + (64ull << 20);
+          const u64 ncap = slack < 0 ? R.used * 2 + (64ull << 20) : R.used + (u64) slack;
           CUDA_TRY(d_new.alloc(ncap,st));
           if (used_before) CUDA_TRY(cudaMemcpyAsync(d_new,R.buf,used_before,cudaMemcpyDeviceToDevice,st));
           R.buf = std::move(d_new); R.cap = ncap;
           CUDA_TRY(cudaMemcpyAsync(d_misc+4,&used_before,8,cudaMemcpyHostToDevice,st));
+          CUDA_TRY(cudaMemcpyAsync(P.counters,d_snap,16*8,cudaMemcpyDeviceToDevice,st));
           R.used = used_before;
-          for (size_t q = 0; q < R.rerun.size(); q++)        // the repeat runs under the next launch number
-            if (R.rerun[q].second == attempt) R.rerun[q].second = attempt + 1;
           continue;
         }
+      repeats = 0;
       used_before = R.used;
       //  the triples to re-run, by work-list position
       std::vector<unsigned> fw;
@@ -2599,6 +2629,7 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       if (attempt > 0 || (misc[10] & (1u << ST_CELLS))) cells_per_warp *= 8;
       if (attempt > 0 || (misc[10] & (1u << ST_STAGE))) stage_bytes *= 4;
       nblocks = launch_blocks((long long) items.size(),EX_NFRONT,LLONG_MAX,cells_per_warp);
+      attempt += 1;
     }
   return FGB_OK;
 }
@@ -2711,6 +2742,7 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   int rc = (P.nwork > 0) ? extend_launches(P,X,d_misc,R,st) : FGB_OK;
   if (rc == FGB_OK) rc = collect_records(O.get(),R,P.nwork > 0,d_counters,st);
   if (rc) return rc;
+  O->retry[0] = R.launches; O->retry[1] = R.reasons; O->retry[2] = R.regrowths; O->retry[3] = (long long) R.rerun.size();
   *out = O.release();                                        // (the device blocks go back as the call returns)
   return FGB_OK;
 }
@@ -2779,7 +2811,8 @@ extern "C" int fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min
 //  status), status 0 (a call that did not fit the shared-memory wave state or the arenas is re-run on the
 //  wide-band kernel; one that never fits fails the whole call with FGB_ERR_OVERFLOW); toff: n offsets into
 //  `traces` (uint8 pairs, what Compress_TraceTo8 leaves).  traces_cap bytes are available; *traces_used
-//  returns the bytes needed (call again with a larger buffer if it exceeds the capacity).
+//  returns the bytes needed, or more when the records overflowed the record buffer (call again with a
+//  larger buffer if it exceeds the capacity).
 extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, long long n, const int *jobs,
                                     const short *tables, int ave_path, int tspace,
                                     int *paths, long long *toff, unsigned char *traces, long long traces_cap,
@@ -2802,8 +2835,8 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
-  long long cells_per_warp = 1ll << 18;
-  int stage_bytes = 1 << 16;
+  long long cells_per_warp = ladder_knob("FGB_EXTEND_CELLS",1ll << 18,32);
+  int stage_bytes = (int) ladder_knob("FGB_EXTEND_STAGE",1 << 16,2);
   const long long nblocks = launch_blocks(n,EX_WARPS,nsm,cells_per_warp);
   const size_t smem = (size_t) EX_WARPS * STATE_BYTES;
   dblock<short> d_tables; dblock<la_job> d_jobs; dblock<int> d_status; dblock<unsigned> d_misc;
@@ -2811,7 +2844,7 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   Arenas ar;
   std::vector<unsigned char> h;
   std::vector<int> hs(n);
-  u64 out_cap = (u64) n * 256 + (u64) traces_cap + (1ull << 20), out_used = 0;
+  u64 out_cap = (u64) n * 256 + (u64) traces_cap + (u64) ladder_knob("FGB_EXTEND_OUT_SLACK",1ll << 20,64), out_used = 0;
   CUDA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_W>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem));
   CUDA_TRY(d_tables.alloc(65536,st));
   CUDA_TRY(d_jobs.alloc((size_t) n,st));
@@ -2831,7 +2864,9 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (out_used > out_cap) return FGB_ERR_OVERFLOW;
+  //  records that did not fit the record buffer: the bytes they need bound the trace bytes, so a call
+  //  again with that much trace room has a record buffer large enough (paths are not written)
+  if (out_used > out_cap) { *traces_used = (long long) out_used; return FGB_ERR_OVERFLOW; }
   //  calls that did not fit (a band wider than EX_W diagonals, a full arena): again on the wide-band
   //  kernel with the wave state in HBM, growing the arenas each round, as fgb_extend re-runs its triples.
   //  A failed call emitted nothing, so its record comes from the round that completes it.
@@ -2856,7 +2891,7 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaStreamSynchronize(st));
-      if (out_used > out_cap) return FGB_ERR_OVERFLOW;
+      if (out_used > out_cap) { *traces_used = (long long) out_used; return FGB_ERR_OVERFLOW; }
     }
   h.resize((size_t) out_used + 64);
   CUDA_TRY(cudaMemcpyAsync(h.data(),d_out,out_used,cudaMemcpyDeviceToHost,st));
@@ -2882,6 +2917,9 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
 }
 
 extern "C" long long fgb_overlaps_count(const fgb_overlaps *o) { return o->nrec; }
+
+extern "C" void fgb_overlaps_retry_info(const fgb_overlaps *o, long long out[4])
+{ for (int i = 0; i < 4; i++) out[i] = o->retry[i]; }
 
 /***********************************************************************************************
  *  Alignment specification: New_Align_Spec's float/double arithmetic (align.c:222-268) stays

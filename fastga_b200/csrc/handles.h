@@ -46,6 +46,7 @@ struct fgb_overlaps                        // raw local alignments of fgb_extend
   unsigned char *h_buf = nullptr;          // packed records (OUT_HDR + trace padded to 8), malloc'ed
   unsigned long long counters[16] = {0};
   long long nseg = 0, nwork = 0;
+  long long retry[4] = {0};                // fgb_overlaps_retry_info
   fgb_overlaps() = default;
   fgb_overlaps(const fgb_overlaps &) = delete;
   fgb_overlaps &operator=(const fgb_overlaps &) = delete;

@@ -86,6 +86,7 @@ int fgb_align_spec(double ave_corr, const float *freq, short *tables, int *ave_p
 long long fgb_overlaps_bytes(const fgb_overlaps *o);
 const unsigned char *fgb_overlaps_data(const fgb_overlaps *o);
 void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out);
+void fgb_overlaps_retry_info(const fgb_overlaps *o, long long out[4]);
 int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *perm2, int jc_bits, int ic_bits,
                int do_filter, fgb_alns **out);
 

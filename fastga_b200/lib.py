@@ -326,6 +326,15 @@ class DeviceOverlaps:
                 "max_warp_cycles": v[14],
                 "slowest_warp": {"cycles": (v[15] >> 40) << 12, "waves": (v[15] >> 16) & 0xffffff, "la_calls": v[15] & 0xffff}}
 
+    def retry_info(self):
+        """how the extension's launches went: launches run, OR of 1 << ST_* failure reasons (2 band, 4 pebble
+        arena, 8 trace staging, 16 hit-group numbering), record-buffer regrowths, triples re-run"""
+        L = load_library()
+        out = (C.c_longlong * 4)()
+        L.fgb_overlaps_retry_info.argtypes = [c_void_p, c_void_p]
+        L.fgb_overlaps_retry_info(self.h, out)
+        return {"launches": out[0], "reasons": out[1], "regrowths": out[2], "reruns": out[3]}
+
     def records(self):
         """(structured array sorted in reference discovery order, trace byte pool)"""
         L = load_library()

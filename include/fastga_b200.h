@@ -153,6 +153,11 @@ long long fgb_overlaps_bytes(const fgb_overlaps *o);
 long long fgb_overlaps_count(const fgb_overlaps *o);
 const unsigned char *fgb_overlaps_data(const fgb_overlaps *o);
 void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out /* 16 */);
+/* how fgb_extend's launches went: out[0] extension launches run (repeats included), out[1] the OR over
+ * them of 1 << ST_* of the items that failed (2 band too wide, 4 pebble arena full, 8 trace staging
+ * full, 16 a hit group's record numbering ran out), out[2] launches repeated because their records overflowed the record buffer, out[3] triples
+ * re-run (once per re-run step they take part in) */
+void fgb_overlaps_retry_info(const fgb_overlaps *o, long long out[4]);
 void fgb_overlaps_free(fgb_overlaps *o);
 
 /* ---- redundancy filter + final order (FastGA.c:3407-3685, :2818 entwine, :3800 SORT_MAP) ---- */

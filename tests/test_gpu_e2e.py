@@ -46,7 +46,8 @@ def test_scaffolded_15pct_bit_exact_vs_reference():
 
 
 def test_long_alignments_exercise_arena_retry():
-    # no SV breaks: contig-long alignments -> pebble arenas overflow and the retry path runs
+    # no SV breaks: contig-long alignments -> their traces overflow the trace staging (not the pebble arenas)
+    # and their triples are re-run on the wide-band kernel (test_gpu_extend_retry.py checks the regime)
     _vs_reference("long_alignments", 13, 6_000_000, 3, 0.03, 0)
 
 

@@ -66,7 +66,7 @@ def _same_on_side_stream(staged):
 
 
 def test_long_alignments_on_a_side_stream():
-    # contig-long alignments: the arena retry and the wide-band kernel run
+    # contig-long alignments: the trace staging overflows and the re-run on the wide-band kernel runs
     staged = _seeds(*synth.make_pair(13, 6_000_000, 3, 0.03, sv_every=0))
     assert staged[3].n > 0
     recs, _ = _same_on_side_stream(staged)

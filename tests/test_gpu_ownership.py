@@ -174,24 +174,38 @@ def test_seed_sort_refusal_releases_its_blocks():
     assert live() == base
 
 
-def test_local_alignments_overflow_releases_its_blocks():
-    """traces_cap = 0 on calls that produce traces: FGB_ERR_OVERFLOW once the records are back"""
+def test_local_alignments_overflow_releases_its_blocks(monkeypatch):
+    """traces_cap = 0 on calls that produce traces: FGB_ERR_OVERFLOW once the records are back; and
+    FGB_ERR_OVERFLOW from a record buffer too small for the records (FGB_EXTEND_OUT_SLACK), with at
+    least the trace bytes needed"""
     gA, gB, jobs = seam_genomes()
     dA, dB = lib.DeviceGenome(gA, want_revcomp=True), lib.DeviceGenome(gB)
     tables, ave = lib.align_spec(0.7, gA.freq)
-    n = jobs.shape[0]
-    paths = np.zeros((n, 7), dtype=np.int32)
-    toff = np.zeros(n, dtype=np.int64)
-    traces = np.zeros(1, dtype=np.uint8)
-    used = C.c_longlong()
     L = load_library()
     L.fgb_local_alignments.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int,
                                        C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
                                        C.POINTER(C.c_longlong), C.c_void_p]
-    base = live()
-    rc = L.fgb_local_alignments(dA.h, dB.h, n, jobs.ctypes.data, tables.ctypes.data, ave, 100, paths.ctypes.data,
-                                toff.ctypes.data, traces.ctypes.data, 0, C.byref(used), None)
-    assert rc == -4 and used.value > 0
-    assert live() == base
+
+    def call(jobs):
+        n = jobs.shape[0]
+        paths = np.zeros((n, 7), dtype=np.int32)
+        toff = np.zeros(n, dtype=np.int64)
+        traces = np.zeros(1, dtype=np.uint8)
+        used = C.c_longlong()
+        base = live()
+        rc = L.fgb_local_alignments(dA.h, dB.h, n, jobs.ctypes.data, tables.ctypes.data, ave, 100,
+                                    paths.ctypes.data, toff.ctypes.data, traces.ctypes.data, 0, C.byref(used), None)
+        assert live() == base
+        return rc, used.value
+
+    rc, used = call(jobs)
+    assert rc == -4 and used > 0
+    # records of 40 + tlen (padded to 8) bytes over the 256 a job is given, more than 64 in all
+    paths, _, _ = lib.local_alignments(dA, dB, jobs, gA.freq)
+    big = np.ascontiguousarray(jobs[paths[:, 5] >= 300])
+    assert len(big) > 0
+    monkeypatch.setenv("FGB_EXTEND_OUT_SLACK", "64")
+    rc, used = call(big)
+    assert rc == -4 and used >= int(paths[paths[:, 5] >= 300, 5].sum())
     dA.close()
     dB.close()
