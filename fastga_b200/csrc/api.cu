@@ -216,22 +216,30 @@ static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-
 
 #define GIX_FWD_ONLY 0x80000000u     // flag bit carried in `phi` down to syncmer_kernel
 
-//  The fine prefix bins a table's scan lays its records out by (fgb_kmer_sort_fine_binned_device):
-//  bin f = (prefix24 >> fsh) - (plo >> fsh) holds records [start[f], start[f+1]), f < nf.
-struct fine_bins
-{ int fsh = 0;
-  long long nf = 0;
-  std::vector<unsigned> start;
+//  The k-mer partition a table's scan starts (fgb_kmer_sort_digit_device): the partition sorts bits
+//  [fsh, 24) of the 12-base prefix, fsh chosen for an upper bound of n, by a first digit of dbits bits that
+//  the scan's emit pass lays out and 8-bit Onesweep passes above it.  The first digit takes what is left
+//  over by as few passes as leave it at most 9 bits; the scan's count pass gives the histogram of the
+//  first pass's digit in hist.
+struct first_digit
+{ int fsh = 0, dbits = 8;
+  dblock<unsigned long long> hist;
+  first_digit(long long nmax, unsigned plo, unsigned phi)
+    { fsh = fgb_kmer_bin_shift(nmax,plo,phi);
+      int bits = 24 - fsh, passes = (bits - 9 + 7) / 8;
+      if (passes < 1) passes = 1;
+      dbits = bits - 8*passes;
+    }
 };
 
 //  K1/K2: syncmer scan + record build of the contigs selected by `mask` (NULL: all) into a fresh
 //  device buffer of *n unsorted records (room for n+1).  *nrev = reverse entries left out (fwd-only).
-//  fb == NULL: the records are packed tile after tile.  Otherwise the count pass counts them per fine
-//  bin, at the resolution the k-mer sort would pick for an upper bound of n (two records per scanned
-//  position), and the emit pass writes each record straight into its bin; fb gets the bins.
+//  fd == NULL: the records are packed tile after tile.  Otherwise the count pass counts them per tile and
+//  first digit of the k-mer partition, at the resolution the k-mer sort would pick for an upper bound of n
+//  (two records per scanned position), and the emit pass stores them in runs by that digit.
 static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo, unsigned phi_flags,
                     dblock<rec128> &d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
-                    fine_bins *fb, cudaStream_t st)
+                    first_digit **fd_out, cudaStream_t st)
 { int T = fgb_sc_tile();
   std::vector<int> tc, ts;
   long long npos = 0;
@@ -244,32 +252,29 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
   int ntiles = (int) tc.size();
   dblock<int> d_tc, d_ts; dblock<unsigned> d_cnt;
   dblock<u64> d_buck, d_total; dblock<unsigned char> d_tmp;
-  dblock<unsigned> d_fb;                   // fine bins: starts [0,nf), cursors [nf,2nf), check flag [2nf]
-  unsigned bad = 0;
-  long long nf = 0;
-  long long tmpb = fgb_dev_scan_tmp_bytes(ntiles);
+  std::unique_ptr<first_digit> fd;
+  long long ncnt = ntiles;                 // per tile, or per (digit, tile)
   int rc;
   u64 total = 0, rdropped = 0;
-  if (fb)
+  if (fd_out)
     { const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
-      const unsigned bhi = phi > plo ? phi : plo + 1;          // an empty range still gets one (empty) bin
-      fb->fsh = fgb_kmer_bin_shift(2*npos,plo,bhi);
-      fb->nf = nf = (long long) ((((unsigned long long) (bhi - 1)) >> fb->fsh) - ((unsigned long long) plo >> fb->fsh)) + 1;
-      tmpb = fgb_dev_scan_tmp_bytes(nf);
+      fd.reset(new first_digit(2*npos,plo,phi > plo ? phi : plo + 1));    // an empty range still gets one bin
+      CUDA_TRY(fd->hist.alloc(256,st));
+      ncnt = (long long) ntiles << fd->dbits;
     }
+  const long long tmpb = fgb_dev_scan_tmp_bytes(ncnt);
   CUDA_TRY(d_tc.alloc(ntiles+1,st));
   CUDA_TRY(d_ts.alloc(ntiles+1,st));
-  if (fb) CUDA_TRY(d_fb.alloc(2*nf+1,st));
-  else    CUDA_TRY(d_cnt.alloc(ntiles+1,st));
+  CUDA_TRY(d_cnt.alloc(ncnt+1,st));
   CUDA_TRY(d_buck.alloc(1025,st));
   CUDA_TRY(d_total.alloc(1,st));
   CUDA_TRY(d_tmp.alloc(tmpb,st));
   CUDA_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   { stage_timer t(&g_timings.scan_ms,st);
-    if (fb)
-      rc = fgb_syncmer_bin_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_fb,nf,
-                                        fb->fsh,d_total,d_tmp,tmpb,plo,phi_flags,st);
+    if (fd)
+      rc = fgb_syncmer_digit_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_cnt,
+                                          fd->fsh,fd->dbits,fd->hist,d_total,d_tmp,tmpb,plo,phi_flags,st);
     else
       rc = fgb_syncmer_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,
                                     d_buck,d_total,d_tmp,tmpb,plo,phi_flags,st);
@@ -277,51 +282,43 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
     CUDA_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
     if (buck1024) CUDA_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
     CUDA_TRY(cudaMemcpyAsync(&rdropped,d_buck + 1024,8,cudaMemcpyDeviceToHost,st));
-    if (fb)
-      { fb->start.resize((size_t) nf + 1);
-        CUDA_TRY(cudaMemcpyAsync(fb->start.data(),d_fb,sizeof(unsigned)*nf,cudaMemcpyDeviceToHost,st));
-      }
     CUDA_TRY(cudaStreamSynchronize(st));
   }
   if (total >= 0xfffffff0ull) return FGB_ERR_LIMIT;
   dblock<rec128> d_a;
   CUDA_TRY(d_a.alloc(total+1,st));
   { stage_timer t(&g_timings.scan_ms,st);
-    if (fb)
-      { rc = fgb_syncmer_scatter_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_fb,d_fb + nf,nf,
-                                        fb->fsh,(long long) total,d_a,d_fb + 2*nf,plo,phi_flags,st);
-        if (rc) return rc;
-        CUDA_TRY(cudaMemcpyAsync(&bad,d_fb + 2*nf,4,cudaMemcpyDeviceToHost,st));
-      }
+    if (fd)
+      rc = fgb_syncmer_digit_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,fd->fsh,
+                                         fd->dbits,(long long) total,d_a,plo,phi_flags,st);
     else
       rc = fgb_syncmer_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,d_a,plo,phi_flags,st);
   }
   if (rc) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));                   // tc/ts must outlive the copies
-  if (bad) return FGB_ERR_OVERFLOW;                      // a bin came out over- or underfull: d_a is not laid out by bin
-  if (fb) fb->start[nf] = (unsigned) total;
   d_recs = std::move(d_a); *n_out = (long long) total; *nrev = (long long) rdropped;
+  if (fd_out) *fd_out = fd.release();
   return FGB_OK;
 }
 
 //  K3/K4: sorts the records in d_a (consumed: it ends up inside the handle or is released) whose
-//  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.  fb: the fine bins the
+//  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.  fd: the first digit the
 //  scan laid d_a out by; NULL: records in any order (the partition passes lay them out).
-static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const fine_bins *fb,
+static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const first_digit *fd,
                       cudaStream_t st, bool index = true)
 { dblock<rec128> d_b; dblock<unsigned char> d_stmp;
   long long stmpb = fgb_sort128_tmp_bytes(n);
   int rc, inb = 0;
   x->n = n;
   CUDA_TRY(d_b.alloc(n+1,st));
-  if (!fb) CUDA_TRY(d_stmp.alloc(stmpb,st));
+  CUDA_TRY(d_stmp.alloc(stmpb,st));
   if (index)
     { CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
       CUDA_TRY(x->d_adj.alloc((size_t) n + 32,st));
     }
   { stage_timer t(&g_timings.ksort_ms,st);
-    if (fb)
-      rc = fgb_kmer_sort_fine_binned_device(d_a,d_b,n,plo,phi,fb->start.data(),fb->nf,fb->fsh,&inb,st);
+    if (fd)
+      rc = fgb_kmer_sort_digit_device(d_a,d_b,n,plo,phi,fd->fsh,fd->dbits,fd->hist,d_stmp,stmpb,&inb,st);
     else
       rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
   }
@@ -346,14 +343,16 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
   x->ncontig = g->ncontig;
   x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
   dblock<rec128> d_a; long long n = 0, nrev = 0;
-  //  the scan lays the records out by prefix bin; FGB_KSORT_PARTITION=1 packs them by tile and lays them
-  //  out with the Onesweep partition passes instead (both paths can be compared in one process)
+  //  the scan lays the records out by the partition's first digit; FGB_KSORT_PARTITION=1 packs them by tile
+  //  and runs every partition pass with Onesweep instead (both paths can be compared in one process)
   const char *part_env = getenv("FGB_KSORT_PARTITION");
-  fine_bins fb, *pfb = (part_env != NULL && atoi(part_env) != 0) ? NULL : &fb;
-  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,pfb,st);
+  const bool packed = part_env != NULL && atoi(part_env) != 0;
+  first_digit *fdp = NULL;
+  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,packed ? NULL : &fdp,st);
+  std::unique_ptr<first_digit> fd(fdp);
   if (rc) return rc;
   x->n_both = n + nrev;
-  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,pfb,st,index))) return rc;
+  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,fd.get(),st,index))) return rc;
   *out = x.release();
   return FGB_OK;
 }

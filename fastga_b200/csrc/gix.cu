@@ -2,7 +2,7 @@
 // build, prefix index + LCP, and conversion from/to the on-disk .ktab entry format.
 //
 // Replaces (reference file:line):
-//   sample_thread / scan_thread      GIXmake.c:164-328, 406-611    -> syncmer_bin_count/scatter_kernel
+//   sample_thread / scan_thread      GIXmake.c:164-328, 406-611    -> syncmer_digit_count/emit_kernel
 //                                                                     (syncmer_kernel<0/1>: by tile)
 //   setup_thread_plain               GIXmake.c:802-980             -> emit of 128-bit records
 //   msd_sort                         MSDsort.c:404                 -> sort128.cu (10 byte passes)
@@ -177,26 +177,61 @@ static __device__ __forceinline__ unsigned syncmer_mask(u64 E, const unsigned ch
   return sel;
 }
 
-//  EMIT = 0: count pass (sampler histogram; per-tile record counts, or with BINNED per-fine-bin record
-//  counts in bincur).  EMIT = 1: emit pass (records at the tile offsets in tile_count, or with BINNED
-//  scattered into their fine bins through the cursors in bincur).  A fine bin is
-//  (prefix24 >> fsh) - (plo >> fsh).
-template<int EMIT, bool BINNED> static __device__ __forceinline__ void
+//  The record of a sampled position p+i of the staged window (sb = the thread's base offset in it):
+//  forward entry = the 40-mer at j, reverse entry = revcomp of the 40-mer ending at j+12.
+static __device__ __forceinline__ rec128 fwd_rec(const u64 *sw, int s, unsigned cr, int j)
+{ rec128 r;
+  r.hi = rev2(sm_bases64(sw,s));
+  r.lo = (rev2(sm_bases64(sw,s+32)) & 0xffff000000000000ull) | ((u64) cr << 32) | (unsigned) j;
+  return r;
+}
+
+static __device__ __forceinline__ rec128 rev_rec(const u64 *sw, int s, unsigned cr, int j)
+{ u64 e0 = sm_bases64(sw,s-28);                    // bases s..s+31 of the 40-mer, s = j-28
+  u64 e1 = sm_bases64(sw,s+4) & 0xffffull;         // bases s+32..s+39
+  rec128 r;
+  r.hi = ~((e1 << 48) | (e0 >> 16));
+  r.lo = ((~e0 & 0xffffull) << 48) | ((u64) (cr | 0x8000u) << 32) | (unsigned) (j+12);
+  return r;
+}
+
+//  The digit-partitioned scan ranks a tile's records by the first digit of the k-mer partition, bits
+//  [dsh, dsh+dbits) of the 12-base prefix (dbits <= SC_DBITS).  Its emit pass stages them in shared memory
+//  in digit order and stores each digit's run with consecutive lanes.  A tile of up to SC_STAGE records
+//  (a both-strand tile holds about 3.2 K) is staged at once, by all its threads; a more crowded one in
+//  SC_ROUNDS rounds of SC_THREADS/SC_ROUNDS threads (two records per position at most).  SC_STAGE keeps
+//  three CTAs on an SM.
+#define SC_DBITS   9
+#define SC_ROUNDS  4
+#define SC_STAGE   3584
+static_assert(SC_THREADS/SC_ROUNDS*SC_PPT*2 <= SC_STAGE, "a round of a crowded tile must fit the stage");
+#define SC_STAGE_SMEM (SC_STAGE*(sizeof(rec128) + sizeof(unsigned short)))
+
+//  EMIT = 0: count pass (sampler histogram; per-tile record counts, or with DIGIT the [digit][tile] count
+//  matrix dmat and the 256-bin histogram nhist of the 8 prefix bits above the digit).  EMIT = 1: emit pass
+//  (records at the tile offsets in tile_count, or with DIGIT at the bases of the scanned dmat).
+template<int EMIT, bool DIGIT> static __device__ __forceinline__ void
 syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
              const long long *__restrict__ woff, const int *__restrict__ crank,
              const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
              unsigned *__restrict__ tile_count, unsigned long long *__restrict__ buck1024,
              rec128 *__restrict__ out, unsigned plo, unsigned phi_flags,
-             unsigned *__restrict__ bincur, int fsh, unsigned nlim)
+             unsigned *__restrict__ dmat, int dsh, int dbits, unsigned long long *__restrict__ nhist,
+             unsigned nlim)
 { __shared__ u64 sw[SC_WORDS+1];
   __shared__ unsigned char tn[256], tc[256];
   __shared__ unsigned wsum[SC_THREADS/32];
   __shared__ unsigned hist[EMIT == 0 ? 1024 : 1];
+  __shared__ unsigned dcnt[DIGIT ? (1 << SC_DBITS) : 1];
+  __shared__ unsigned dloc[DIGIT && EMIT ? (1 << SC_DBITS) : 1];
+  __shared__ unsigned dbase[DIGIT && EMIT ? (1 << SC_DBITS) : 1];
+  __shared__ unsigned nh[DIGIT && !EMIT ? 256 : 1];
 
   //  bit 31 of phi_flags: forward-strand entries only (the table is only ever the adaptamer side
   //  of a merge, where reverse entries never seed, FastGA.c:921-928)
   const unsigned phi = phi_flags & 0x7fffffffu;
   const bool fwd_only = (phi_flags >> 31) != 0;
+  const unsigned nd = 1u << dbits, dmask = nd - 1;
   int tid = threadIdx.x;
   int c   = tile_contig[blockIdx.x];
   int t0  = tile_start[blockIdx.x];
@@ -208,6 +243,12 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
   tc[tid] = c_TC[tid];
   if (EMIT == 0)
     for (int i = tid; i < 1024; i += SC_THREADS) hist[i] = 0;
+  if (DIGIT)
+    for (int i = tid; i < (1 << SC_DBITS); i += SC_THREADS)
+      { dcnt[i] = 0;
+        if (EMIT) dbase[i] = (unsigned) i < nd ? dmat[(size_t) i*gridDim.x + blockIdx.x] : 0;
+      }
+  if constexpr (DIGIT && !EMIT) nh[tid] = 0;
   for (int i = tid; i < SC_WORDS+1; i += SC_THREADS)
     { long long gw = (t0 >> 5) - 1 + i;
       sw[i] = (gw >= 0 && gw < nw) ? w[gw] : 0ull;
@@ -249,10 +290,22 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
   unsigned rdropped = 0;                       // reverse entries a forward-only table leaves out
   if (fwd_only) { rdropped = __popc(rmask); rmask = 0; }
   unsigned cnt = __popc(fmask) + __popc(rmask);
+  const unsigned cr = (unsigned) crank[c];
+
+  //  this thread's records in order (forward before reverse at each position): f(record)
+  auto each_rec = [&](auto f)
+    { unsigned m = fmask | rmask;
+      while (m)
+        { int i = __ffs(m)-1;
+          m &= m-1;
+          if (fmask >> i & 1) f(fwd_rec(sw,sb+i,cr,p+i));
+          if (rmask >> i & 1) f(rev_rec(sw,sb+i,cr,p+i));
+        }
+    };
 
   int lane = tid & 31, wp = tid >> 5;
   unsigned pre = 0, tot = 0, inc = cnt;
-  if (!BINNED)
+  if (!DIGIT || EMIT)
     {
 #pragma unroll
       for (int o = 1; o < 32; o <<= 1)
@@ -266,43 +319,15 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
           tot += wsum[i];
         }
     }
-  const unsigned cr = (unsigned) crank[c];
-
-  if (BINNED)
-    { //  every record on its own: the k-mers of neighbouring lanes almost never share a fine bin, so
-      //  aggregating a warp's increments (__match_any_sync) merges next to nothing, and a warp-uniform
-      //  loop keeps every lane waiting for the lane with the most records
-      const unsigned fbase = plo >> fsh;
-      unsigned fm = fmask, rm = rmask;
-      while (fm | rm)
-        { rec128 r;
-          r.lo = 0;
-          if (fm)
-            { int i = __ffs(fm)-1;
-              fm &= fm-1;
-              r.hi = rev2(sm_bases64(sw,sb+i));
-              if (EMIT)
-                r.lo = (rev2(sm_bases64(sw,sb+i+32)) & 0xffff000000000000ull) | ((u64) cr << 32) | (unsigned) (p+i);
-            }
-          else
-            { int i = __ffs(rm)-1;
-              rm &= rm-1;
-              u64 e0 = sm_bases64(sw,sb+i-28), e1 = sm_bases64(sw,sb+i+4) & 0xffffull;
-              r.hi = ~((e1 << 48) | (e0 >> 16));
-              r.lo = ((~e0 & 0xffffull) << 48) | ((u64) (cr | 0x8000u) << 32) | (unsigned) (p+i+12);
-            }
-          const unsigned b = (unsigned) (r.hi >> (40 + fsh)) - fbase;
-          if (EMIT == 0)
-            atomicAdd(&bincur[b],1u);                                  // count pass: the bin's count
-          else
-            { const unsigned s = atomicAdd(&bincur[b],1u);             // emit pass: a slot at the bin's cursor
-              if (s < nlim) st_rec(out + s,r);                         // an overrun is caught by kmer_scatter_check_kernel
-            }
-        }
-    }
 
   if (EMIT == 0)
-    { //  10-bit first-5-bases histogram over ALL sampled positions, both strands, as
+    { if (DIGIT)
+        each_rec([&](const rec128 &r)
+          { const unsigned pf = (unsigned) (r.hi >> 40);
+            atomicAdd(&dcnt[(pf >> dsh) & dmask],1u);
+            atomicAdd(&nh[(pf >> (dsh + dbits)) & 0xff],1u);
+          });
+      //  10-bit first-5-bases histogram over ALL sampled positions, both strands, as
       //  sample_thread does (GIXmake.c:318-320); decides the .ktab part split (:669-691).
       unsigned m = sel;
       while (m)
@@ -327,36 +352,72 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
         { rdropped = __reduce_add_sync(0xffffffffu,rdropped);
           if (lane == 0 && rdropped) atomicAdd(&buck1024[1024],(unsigned long long) rdropped);
         }
-      if (!BINNED && tid == 0) tile_count[blockIdx.x] = tot;
+      if (DIGIT)
+        { for (int i = tid; i < nd; i += SC_THREADS) dmat[(size_t) i*gridDim.x + blockIdx.x] = dcnt[i];
+          if (nh[tid]) atomicAdd(&nhist[tid],(unsigned long long) nh[tid]);      // SC_THREADS == 256
+        }
+      else if (tid == 0) tile_count[blockIdx.x] = tot;
       return;
     }
-  if (BINNED) return;
+
+  if (DIGIT)
+    { extern __shared__ __align__(16) unsigned char sc_smem[];
+      rec128 *stage = reinterpret_cast<rec128 *>(sc_smem);                       // [SC_STAGE]
+      unsigned short *rk = reinterpret_cast<unsigned short *>(stage + SC_STAGE);  // rank inside its digit
+      const int nr = tot <= SC_STAGE ? 1 : SC_ROUNDS;                            // rounds of this tile
+      const int RW = SC_THREADS/32/nr;                                           // warps per round
+      for (int rd = 0; rd < nr; rd++)
+        { const bool act = (wp / RW) == rd;
+          unsigned o = pre + inc - cnt;          // this thread's first slot inside its round
+          for (int i = 0; i < rd*RW; i++) o -= wsum[i];
+          const unsigned o0 = o;
+          if (act)
+            each_rec([&](const rec128 &r)
+              { rk[o++] = (unsigned short) atomicAdd(&dcnt[(unsigned) (r.hi >> (40 + dsh)) & dmask],1u); });
+          __syncthreads();
+          //  exclusive scan of the digit counts (two per thread, SC_THREADS*2 >= 2^SC_DBITS)
+          { unsigned v0 = dcnt[2*tid], v1 = dcnt[2*tid+1], s = v0 + v1, x = s;
+#pragma unroll
+            for (int k = 1; k < 32; k <<= 1)
+              { unsigned t = __shfl_up_sync(0xffffffffu,x,k);
+                if (lane >= k) x += t;
+              }
+            if (lane == 31) wsum[wp] = x;
+            __syncthreads();
+            unsigned b = x - s;
+            for (int i = 0; i < wp; i++) b += wsum[i];
+            dloc[2*tid] = b; dloc[2*tid+1] = b + v0;
+          }
+          unsigned rtot = 0;
+          for (int i = 0; i < SC_THREADS/32; i++) rtot += wsum[i];
+          __syncthreads();
+          o = o0;
+          if (act)
+            each_rec([&](const rec128 &r)
+              { const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
+                st_rec(stage + (dloc[d] + rk[o++]),r);
+              });
+          __syncthreads();
+          for (unsigned q = tid; q < rtot; q += SC_THREADS)
+            { rec128 r = ld_rec(stage + q);
+              const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
+              const unsigned s = dbase[d] + (q - dloc[d]);
+              if (s < nlim) st_rec(out + s,r);
+            }
+          __syncthreads();
+          if (rd + 1 < nr)
+            { for (int i = tid; i < nd; i += SC_THREADS) { dbase[i] += dcnt[i]; dcnt[i] = 0; }
+              //  wsum back to the per-warp record counts of the thread prefix
+              unsigned x = inc;
+              if (lane == 31) wsum[wp] = x;
+              __syncthreads();
+            }
+        }
+      return;
+    }
 
   long long o = (long long) tile_count[blockIdx.x] + pre + inc - cnt;
-  unsigned m = fmask | rmask;
-  while (m)
-    { int i = __ffs(m)-1;
-      m &= m-1;
-      int j = p + i;
-      if (fmask >> i & 1)
-        { u64 e0 = sm_bases64(sw,sb+i);
-          u64 e1 = sm_bases64(sw,sb+i+32);
-          rec128 r;
-          r.hi = rev2(e0);
-          r.lo = (rev2(e1) & 0xffff000000000000ull) | ((u64) cr << 32) | (unsigned) j;
-          st_rec(out + o,r);
-          o += 1;
-        }
-      if (rmask >> i & 1)
-        { u64 e0 = sm_bases64(sw,sb+i-28);                    // bases s..s+31, s = j-28
-          u64 e1 = sm_bases64(sw,sb+i+4) & 0xffffull;         // bases s+32..s+39
-          rec128 r;
-          r.hi = ~((e1 << 48) | (e0 >> 16));
-          r.lo = ((~e0 & 0xffffull) << 48) | ((u64) (cr | 0x8000u) << 32) | (unsigned) (j+12);
-          st_rec(out + o,r);
-          o += 1;
-        }
-    }
+  each_rec([&](const rec128 &r) { st_rec(out + o,r); o += 1; });
 }
 
 //  Records packed by tile, for callers that sort them with the partition passes (the sharded path)
@@ -367,34 +428,27 @@ syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
                unsigned *__restrict__ tile_count,       // EMIT=0: out counts; EMIT=1: in offsets
                unsigned long long *__restrict__ buck1024,
                rec128 *__restrict__ out, unsigned plo, unsigned phi_flags)
-{ syncmer_body<EMIT,false>(seq,clen,woff,crank,tile_contig,tile_start,tile_count,buck1024,out,plo,phi_flags,NULL,0,0); }
+{ syncmer_body<EMIT,false>(seq,clen,woff,crank,tile_contig,tile_start,tile_count,buck1024,out,plo,phi_flags,
+                           NULL,0,0,NULL,0); }
 
-//  Records laid out by fine bin: counts per bin, then a scatter through per-bin cursors
+//  Records laid out by the first digit of the k-mer partition: [digit][tile] counts, then the staged emit
 __global__ void __launch_bounds__(SC_THREADS)
-syncmer_bin_count_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
-                         const long long *__restrict__ woff, const int *__restrict__ crank,
-                         const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
-                         unsigned long long *__restrict__ buck1024, unsigned plo, unsigned phi_flags,
-                         unsigned *__restrict__ bin_count, int fsh)
-{ syncmer_body<0,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,buck1024,NULL,plo,phi_flags,bin_count,fsh,0); }
+syncmer_digit_count_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+                           const long long *__restrict__ woff, const int *__restrict__ crank,
+                           const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+                           unsigned long long *__restrict__ buck1024, unsigned plo, unsigned phi_flags,
+                           unsigned *__restrict__ dmat, int dsh, int dbits, unsigned long long *__restrict__ nhist)
+{ syncmer_body<0,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,buck1024,NULL,plo,phi_flags,
+                       dmat,dsh,dbits,nhist,0); }
 
 __global__ void __launch_bounds__(SC_THREADS)
-syncmer_scatter_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
-                       const long long *__restrict__ woff, const int *__restrict__ crank,
-                       const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
-                       rec128 *__restrict__ out, unsigned n, unsigned plo, unsigned phi_flags,
-                       unsigned *__restrict__ bin_cursor, int fsh)
-{ syncmer_body<1,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,NULL,out,plo,phi_flags,bin_cursor,fsh,n); }
-
-//  After the scatter every fine-bin cursor has advanced to the start of the next bin.  Any other value
-//  means the count and emit passes disagreed about which records exist: *bad = 1.
-__global__ void kmer_scatter_check_kernel(const unsigned *__restrict__ cursor, const unsigned *__restrict__ start,
-                                          long long nf, unsigned n, unsigned *__restrict__ bad)
-{ long long f = (long long) blockIdx.x * blockDim.x + threadIdx.x;
-  if (f >= nf) return;
-  unsigned end = (f + 1 < nf) ? start[f+1] : n;
-  if (cursor[f] != end) *bad = 1;
-}
+syncmer_digit_emit_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
+                          const long long *__restrict__ woff, const int *__restrict__ crank,
+                          const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
+                          rec128 *__restrict__ out, unsigned n, unsigned plo, unsigned phi_flags,
+                          unsigned *__restrict__ dbase, int dsh, int dbits)
+{ syncmer_body<1,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,NULL,out,plo,phi_flags,
+                       dbase,dsh,dbits,NULL,n); }
 
 /***********************************************************************************************
  *  Prefix index + LCP over the sorted table (compress_thread, GIXmake.c:1235-1261):
@@ -561,48 +615,49 @@ extern "C" int fgb_syncmer_emit_device(const void *d_seq, const long long *d_cle
   return FGB_OK;
 }
 
-//  Pass 1 of the binned scan: 1024-bin sampler histogram, and the records per fine bin (nf bins of
-//  shift fsh) scanned in place to the bins' first slots; *d_total = number of records.
-extern "C" int fgb_syncmer_bin_count_device(const void *d_seq, const long long *d_clen,
-                                            const long long *d_woff, const int *d_crank,
-                                            const int *d_tile_contig, const int *d_tile_start, int ntiles,
-                                            unsigned long long *d_buck1024, unsigned *d_bin_start, long long nf,
-                                            int fsh, unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                                            unsigned plo, unsigned phi, void *stream)
+//  Pass 1 of the digit-partitioned scan: 1024-bin sampler histogram, the records of each tile per digit
+//  (bits [dsh, dsh+dbits) of the 12-base prefix) in the [digit][tile] matrix d_dmat, scanned in place to
+//  every (digit, tile)'s first slot, and in d_nhist the histogram of the prefix's 8 bits above the digit;
+//  *d_total = number of records.
+extern "C" int fgb_syncmer_digit_count_device(const void *d_seq, const long long *d_clen,
+                                              const long long *d_woff, const int *d_crank,
+                                              const int *d_tile_contig, const int *d_tile_start, int ntiles,
+                                              unsigned long long *d_buck1024, unsigned *d_dmat, int dsh, int dbits,
+                                              unsigned long long *d_nhist, unsigned long long *d_total, void *d_tmp,
+                                              long long tmp_bytes, unsigned plo, unsigned phi, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
+  if (dbits < 1 || dbits > SC_DBITS || dsh < 0 || dsh + dbits + 8 > 32) return FGB_ERR_ARG;
   int rc = init_tables();
   if (rc) return rc;
   CUDA_TRY(cudaMemsetAsync(d_buck1024,0,1025*8,st));
-  CUDA_TRY(cudaMemsetAsync(d_bin_start,0,sizeof(unsigned)*nf,st));
+  CUDA_TRY(cudaMemsetAsync(d_nhist,0,256*8,st));
   if (ntiles > 0)
-    { syncmer_bin_count_kernel<<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
-                                                           d_tile_contig,d_tile_start,d_buck1024,plo,phi,
-                                                           d_bin_start,fsh);
+    { syncmer_digit_count_kernel<<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
+                                                             d_tile_contig,d_tile_start,d_buck1024,plo,phi,
+                                                             d_dmat,dsh,dbits,d_nhist);
       fgb_count_launch(1);
     }
   CUDA_TRY(cudaGetLastError());
-  return fgb_dev_exclusive_scan_u32(d_bin_start,nf,d_total,d_tmp,tmp_bytes,st);
+  return fgb_dev_exclusive_scan_u32(d_dmat,(long long) ntiles << dbits,d_total,d_tmp,tmp_bytes,st);
 }
 
-//  Pass 2: every record straight into its fine bin of d_records (n records), through cursors that start
-//  as a copy of d_bin_start (d_cursor: nf words); then *d_bad = 1 unless every bin came out exactly full.
-extern "C" int fgb_syncmer_scatter_device(const void *d_seq, const long long *d_clen,
-                                          const long long *d_woff, const int *d_crank,
-                                          const int *d_tile_contig, const int *d_tile_start, int ntiles,
-                                          const unsigned *d_bin_start, unsigned *d_cursor, long long nf, int fsh,
-                                          long long n, void *d_records, unsigned *d_bad, unsigned plo,
-                                          unsigned phi, void *stream)
+//  Pass 2: the records of every tile at the (digit, tile) slots of the scanned d_dmat, in runs by digit.
+extern "C" int fgb_syncmer_digit_emit_device(const void *d_seq, const long long *d_clen,
+                                             const long long *d_woff, const int *d_crank,
+                                             const int *d_tile_contig, const int *d_tile_start, int ntiles,
+                                             unsigned *d_dmat, int dsh, int dbits, long long n, void *d_records,
+                                             unsigned plo, unsigned phi, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  CUDA_TRY(cudaMemcpyAsync(d_cursor,d_bin_start,sizeof(unsigned)*nf,cudaMemcpyDeviceToDevice,st));
-  CUDA_TRY(cudaMemsetAsync(d_bad,0,sizeof(unsigned),st));
-  if (ntiles > 0)
-    { syncmer_scatter_kernel<<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
-                                                         d_tile_contig,d_tile_start,(rec128 *) d_records,
-                                                         (unsigned) n,plo,phi,d_cursor,fsh);
-      fgb_count_launch(1);
+  static bool attr_set = false;
+  if (!attr_set)
+    { CUDA_TRY(cudaFuncSetAttribute(syncmer_digit_emit_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                    (int) SC_STAGE_SMEM));
+      attr_set = true;
     }
-  if (nf > 0)
-    { kmer_scatter_check_kernel<<<(unsigned) ((nf + 255) / 256),256,0,st>>>(d_cursor,d_bin_start,nf,(unsigned) n,d_bad);
+  if (ntiles > 0)
+    { syncmer_digit_emit_kernel<<<ntiles,SC_THREADS,SC_STAGE_SMEM,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
+                                                                        d_tile_contig,d_tile_start,(rec128 *) d_records,
+                                                                        (unsigned) n,plo,phi,d_dmat,dsh,dbits);
       fgb_count_launch(1);
     }
   CUDA_TRY(cudaGetLastError());

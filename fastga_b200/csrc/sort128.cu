@@ -19,6 +19,7 @@
 //            16 + 32·passes.
 #include "stages.h"
 #include <stdlib.h>
+#include <utility>
 #include <vector>
 
 #define SORT_THREADS 512
@@ -423,10 +424,10 @@ extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo
  *
  *  Ten full Onesweep passes move 10 x 32 bytes per record through HBM.  Instead:
  *    1. the records are laid out by prefix bin: bin p at [bins[p], bins[p+1]), in any order inside
- *       the bin.  A table built from a genome gets that layout from the scan itself (the count pass
- *       counts per bin, the emit pass scatters into the bins: fgb_kmer_sort_fine_binned_device);
- *       records from elsewhere get it from two Onesweep partition passes on the two MOST
- *       significant key bytes (fgb_kmer_sort_range_device);
+ *       the bin.  Onesweep partition passes on the prefix bits above the bin shift give that
+ *       layout (fgb_kmer_sort_range_device).  A table built from a genome gets the first of them from
+ *       the scan itself: its emit pass stores the records in runs by the lowest digit
+ *       (fgb_kmer_sort_digit_device);
  *    2. consecutive bins are packed into groups of at most BK_CAP records and BK_SPAN bins; one
  *       CTA per group pulls the group into shared memory with one TMA bulk copy, sorts it there
  *       (kmer_bucket_sort_kernel) and writes it back once;
@@ -716,29 +717,50 @@ extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, uns
   return FGB_OK;
 }
 
-//  d_a: n records the syncmer scan scattered by FINE bin, (prefix24 >> fsh) - (plo >> fsh) at
-//  [fstart[f], fstart[f+1]) (fstart on the host, nf+1 entries), with fsh chosen for an upper bound of n.
-//  A bin of the rule for n is a run of whole fine bins, so d_a is already laid out by bin and goes
-//  straight to the bucket sort.  Sorted table lands in d_b (*result_in_b = 1), or stays in d_a when n <= 1.
-extern "C" int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                                                const unsigned *fstart, long long nf, int fsh, int *result_in_b,
-                                                void *stream)
-{ *result_in_b = 0;
+//  d_a: n records the syncmer scan laid out by the first digit of the partition, bits [fsh, fsh+dbits) of
+//  the 12-base prefix; d_nhist: the histogram of the 8 prefix bits above it.  Onesweep passes on the rest
+//  of the prefix above fsh lay the records out by fine bin, (prefix24 >> fsh) - (plo >> fsh), with fsh
+//  chosen for an upper bound of n.  A bin of the rule for n is a run of whole fine bins, so the records then
+//  go straight to the bucket sort.  Sorted table lands in d_a or d_b (*result_in_b).
+extern "C" int fgb_kmer_sort_digit_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
+                                          const u64 *d_nhist, void *d_tmp, long long tmp_bytes, int *result_in_b,
+                                          void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  *result_in_b = 0;
   if (n <= 1) return FGB_OK;
   if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
-  if (phi <= plo || phi > (1u << 24)) return FGB_ERR_ARG;
+  if (phi <= plo || phi > (1u << 24) || tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
   const int sh = fgb_kmer_bin_shift(n,plo,phi);
-  if (sh < fsh || (long long) fstart[nf] != n) return FGB_ERR_ARG;
+  if (sh < fsh) return FGB_ERR_ARG;
+  const sort_tmp T(d_tmp,n);
+  CUDA_TRY(cudaMemcpyAsync(T.hist[0],d_nhist,256*8,cudaMemcpyDeviceToDevice,st));
+  rec128 *src = (rec128 *) d_a, *dst = (rec128 *) d_b;
+  const int b0 = 64 + 40 + fsh + dbits, npass = (128 - b0 + 7) / 8;
+  for (int p = 0; p < npass; p++)
+    { const int b = b0 + 8*p, nd = (p + 1 < npass) ? b + 8 : -1;
+      int rc = onesweep_pass<rec128,16,16>(src,dst,n,b,nd,T,p & 1,st);
+      if (rc) return rc;
+      std::swap(src,dst);
+    }
+
   const unsigned long long base = (unsigned long long) plo >> sh, fbase = (unsigned long long) plo >> fsh;
+  const long long nf = (long long) (((unsigned long long) (phi - 1) >> fsh) - fbase) + 1;
   const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
-  std::vector<unsigned> bins((size_t) nbins + 1);
+  std::vector<unsigned> fstart((size_t) nf + 1), bins((size_t) nbins + 1);
+  { dblock<unsigned> d_fstart;
+    CUDA_TRY(d_fstart.alloc((size_t) (nf+1),st));
+    kmer_bins_kernel<<<(int) ((n + 1 + 255) / 256),256,0,st>>>(src,n,40 + fsh,fbase,d_fstart,nf);
+    fgb_count_launch(1);
+    CUDA_TRY(cudaMemcpyAsync(fstart.data(),d_fstart,sizeof(unsigned)*(size_t) (nf+1),cudaMemcpyDeviceToHost,st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+  }
   for (long long p = 0; p <= nbins; p++)
     { long long f = (long long) ((base + p) << (sh - fsh)) - (long long) fbase;     // first fine bin of bin p
       bins[p] = fstart[f < 0 ? 0 : (f > nf ? nf : f)];
     }
-  int rc = kmer_sort_binned((const rec128 *) d_a,(rec128 *) d_b,bins.data(),nbins,sh,plo,(cudaStream_t) stream);
+  int rc = kmer_sort_binned(src,dst,bins.data(),nbins,sh,plo,st);
   if (rc) return rc;
-  *result_in_b = 1;
+  *result_in_b = (dst == (rec128 *) d_b);
   return FGB_OK;
 }
 

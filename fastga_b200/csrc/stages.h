@@ -28,8 +28,9 @@ int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_
 int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
 int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
                                void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-int fgb_kmer_sort_fine_binned_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                                     const unsigned *fstart, long long nf, int fsh, int *result_in_b, void *stream);
+int fgb_kmer_sort_digit_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
+                               const unsigned long long *d_nhist, void *d_tmp, long long tmp_bytes, int *result_in_b,
+                               void *stream);
 
 // ---- gix.cu: genome staging, syncmer scan, table index and .ktab entries ----
 int fgb_stage_genome_device(const void *d_bps, const long long *d_boff, const long long *d_clen,
@@ -44,16 +45,15 @@ int fgb_syncmer_emit_device(const void *d_seq, const long long *d_clen, const lo
                             const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
                             int ntiles, unsigned *d_tile_offset, void *d_records, unsigned plo,
                             unsigned phi, void *stream);
-int fgb_syncmer_bin_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                                 const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                                 int ntiles, unsigned long long *d_buck1024, unsigned *d_bin_start, long long nf,
-                                 int fsh, unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                                 unsigned plo, unsigned phi, void *stream);
-int fgb_syncmer_scatter_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                               const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                               int ntiles, const unsigned *d_bin_start, unsigned *d_cursor, long long nf, int fsh,
-                               long long n, void *d_records, unsigned *d_bad, unsigned plo, unsigned phi,
-                               void *stream);
+int fgb_syncmer_digit_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
+                                   const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
+                                   int ntiles, unsigned long long *d_buck1024, unsigned *d_dmat, int dsh, int dbits,
+                                   unsigned long long *d_nhist, unsigned long long *d_total, void *d_tmp,
+                                   long long tmp_bytes, unsigned plo, unsigned phi, void *stream);
+int fgb_syncmer_digit_emit_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
+                                  const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
+                                  int ntiles, unsigned *d_dmat, int dsh, int dbits, long long n, void *d_records,
+                                  unsigned plo, unsigned phi, void *stream);
 int fgb_kix_index_device(const void *d_tab, long long n, unsigned *d_pstart, unsigned char *d_adj, void *stream);
 int fgb_ktab_export_device(const void *d_tab, long long n, int pbytes, int cbytes,
                            const long long *d_part_first, int nparts, void *d_out, void *stream);
