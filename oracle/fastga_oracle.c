@@ -931,6 +931,7 @@ typedef struct
 typedef struct
   { int comp, aread, bread;                 /* ORIGINAL contig numbers (Perm applied, :3007-3008) */
     int abpos, bbpos, aepos, bepos, diffs, tlen;
+    int grp;                                /* index of the align_contigs call that found it */
     int64_t toff;                           /* offset of the trace bytes in the trace pool */
   } orc_ovl;
 
@@ -1108,6 +1109,7 @@ typedef struct
     orc_result *R; orc_work *work; orc_path *path; int alnMin; double alnRate;
     orc_calllog *log;                       /* NULL (orc_search), or the call list of orc_search_calls */
     int comp, ctg1, ctg2; int64_t alen, blen, mlen, doffset, aoffset, alast; const char *as, *bs;
+    int ngrp; uint64_t gkey;                /* align_contigs calls so far, (strand, contig pair) of the last */
   } search_ctx;
 
 static void search_triple(void *v, const orc_triple *T)
@@ -1115,6 +1117,8 @@ static void search_triple(void *v, const orc_triple *T)
   const orc_layout *L = S->L;
   int p_jc = 12 + L->anti_bits + L->band_bits, p_ic = p_jc + L->jc_bits, p_cp = p_ic + L->ic_bits;
   const rec128 *r = S->seeds + T->b;
+  if (S->ngrp == 0 || T->key != S->gkey)            /* one align_contigs call per (strand, contig pair) */
+    { S->ngrp += 1; S->gkey = T->key; }
   S->comp = (int) get_bits(r,p_cp,1);
   S->ctg1 = S->perm1[get_bits(r,p_ic,L->ic_bits)];
   S->ctg2 = S->perm2[get_bits(r,p_jc,L->jc_bits)];
@@ -1205,7 +1209,7 @@ static void search_hit(void *v, const orc_triple *T, int64_t alow, int64_t ahgh,
               o.comp = comp; o.aread = ctg1; o.bread = ctg2;
               o.abpos = path->abpos; o.bbpos = path->bbpos;
               o.aepos = path->aepos; o.bepos = path->bepos;
-              o.diffs = path->diffs; o.tlen = path->tlen; o.toff = 0;
+              o.diffs = path->diffs; o.tlen = path->tlen; o.grp = S->ngrp-1; o.toff = 0;
               res_push(S->R,&o,path->trace);
             }
           if (comp) eant = S->mlen - (path->abpos + path->bbpos);
@@ -1293,4 +1297,294 @@ void orc_chains(const rec128 *seeds, int64_t n, const orc_layout *L, int chain_b
   if (trip == NULL || hits == NULL) C.trip = C.hits = NULL;
   chain_scan(seeds,n,L,chain_break,chain_min,chains_triple,chains_hit,&C);
   counts[0] = C.ntrip; counts[1] = C.nhit;
+}
+
+/***********************************************************************************************
+ *  F.  Redundancy filter of align_contigs (FastGA.c:3405-3685) with entwine (:2818-2941), run on
+ *      the records of each align_contigs call, then the SORT_MAP order of la_sort (:3800-3835)
+ *      over every survivor.
+ *
+ *  Restated from the reference's rules, not from fastga_b200/csrc/filter.cu: entwine keeps the
+ *  running separation closest to zero and the last meeting point, the sweeps walk a pointer array
+ *  in libc qsort order, every record carries ELIMINATED / OWNS_TRACE flags, and each fusion cuts
+ *  a fresh trace at the meeting point.  orc_filter_counters reads, per outcome, how often the last
+ *  orc_filter went through each branch (FC_* below).
+ **********************************************************************************************/
+
+#define F_TSPACE      100
+#define F_BOX_FUZZ     10
+#define F_ELIMINATED  0x1
+#define F_OWNS_TRACE  0x2
+
+typedef struct
+  { orc_ovl  o;             /* o.toff unused */
+    uint8_t *trace;         /* (diffs, B-advance) byte pairs */
+    int      flags;
+    int64_t  pos;           /* place in the filter's output stream: the reference's address order */
+  } fl_rec;
+
+enum { FC_S1_BOTH_KEEP_O,   /* sweep 1: same start and end, o kept (o.diffs < w.aepos) */
+       FC_S1_BOTH_DROP_O,   /*          same start and end, o dropped */
+       FC_S1_START_KEEP_O,  /*          same start only, o ends later */
+       FC_S1_START_DROP_O,  /*          same start only, w ends at or after o */
+       FC_S1_END_KEEP_O,    /*          same end only, o starts earlier */
+       FC_S1_END_DROP_O,    /*          same end only, o starts at or after w */
+       FC_S2_B_DISJOINT,    /* sweep 2: B-intervals apart, w skipped */
+       FC_S2_FUSE,          /*          paths meet: o continues as w (every fusion) */
+       FC_S2_FUSE_DEAD_O,   /*          ... into an o that its row has already eliminated */
+       FC_S2_FUSE_W_OWNS,   /*          ... with a w that already owns a fused trace */
+       FC_S2_BOX_DROP_W,    /*          paths apart, w inside o's box */
+       FC_S2_BOX_DROP_O,    /*          paths apart, o inside w's box */
+       FC_S2_APART_KEPT,    /*          paths apart, neither box inside the other */
+       FC_S2_CROSS,         /*          paths touch or cross without a meeting point: no action */
+       FC_S2_ROW_EXTENDED,  /*          a w visited only because a fusion moved o's end */
+       FC_N };
+
+static int64_t g_filter_cnt[FC_N];
+void orc_filter_counters(int64_t *out) { memcpy(out,g_filter_cnt,sizeof(g_filter_cnt)); }
+
+/* min tracks the separation closest to zero; it sticks at 0 once two separations differ in sign
+   or one is 0 (FastGA.c:2876-2887) */
+static int closer(int min, int d)
+{ if (min < 0 && d > min)
+    return (d >= 0 ? 0 : d);
+  if (min > 0 && d < min)
+    return (d <= 0 ? 0 : d);
+  return (min);
+}
+
+/* J starts at or before K on A.  The B-separation K - J at K's start (J interpolated inside its
+   interval), at every trace point both paths pass strictly before the first end, and at that end
+   (the path that does not end there interpolated from the trace point before it).  Returns the
+   separation closest to zero (0: the paths touch or cross); *where is the last of those trace
+   points at separation 0, -1 if there is none (FastGA.c:2818-2941). */
+static int entwine(const orc_ovl *J, const uint8_t *jtr, const orc_ovl *K, const uint8_t *ktr, int *where)
+{ int ac, ae, y2, b2, yp, i, j, k, min;
+
+  *where = -1;
+  y2 = J->bbpos;
+  b2 = K->bbpos;
+  ac = (K->abpos/F_TSPACE)*F_TSPACE;
+  j  = 1 + 2*(K->abpos/F_TSPACE - J->abpos/F_TSPACE);
+  for (i = 1; i < j; i += 2)
+    y2 += jtr[i];
+  if (j == 1)
+    yp = y2 + (jtr[j] * (K->abpos - J->abpos)) / (ac+F_TSPACE - J->abpos);
+  else
+    yp = y2 + (jtr[j] * (K->abpos - ac)) / F_TSPACE;
+  min = b2-yp;
+
+  ae = (J->aepos < K->aepos) ? J->aepos : K->aepos;
+  for (k = 1, ac += F_TSPACE; ac < ae; ac += F_TSPACE, j += 2, k += 2)
+    { y2 += jtr[j];
+      b2 += ktr[k];
+      i = b2-y2;
+      min = closer(min,i);
+      if (i == 0)
+        *where = ac;
+    }
+  ac -= F_TSPACE;
+
+  if (ae == J->aepos)
+    { y2 = J->bepos;
+      if (K->aepos >= ac)
+        b2 += (ktr[k] * (ae-ac)) / F_TSPACE;
+      else
+        b2 += (ktr[k] * (ae-ac)) / (K->aepos-ac);
+    }
+  else
+    { b2 = K->bepos;
+      if (J->aepos >= ac)
+        y2 += (jtr[j] * (ae-ac)) / F_TSPACE;
+      else
+        y2 += (jtr[j] * (ae-ac)) / (J->aepos-ac);
+    }
+  return (closer(min,b2-y2));
+}
+
+static int FL_ASORT(const void *l, const void *r)      /* FastGA.c:2962 */
+{ return ((*(fl_rec **) l)->o.abpos - (*(fl_rec **) r)->o.abpos); }
+
+/* o continues as w from the trace point `where` on: o's intervals up to it, then w's after it */
+static void fuse(fl_rec *o, const fl_rec *w, int where)
+{ orc_ovl *op = &o->o;
+  const orc_ovl *wp = &w->o;
+  int ocut = 2*(((where - op->abpos)-1)/F_TSPACE + 1);
+  int wcut = 2*(((where - wp->abpos)-1)/F_TSPACE + 1);
+  int tlen = ocut + (wp->tlen - wcut), d = 0, g, h = 0;
+  uint8_t *nt = (uint8_t *) malloc(tlen > 0 ? tlen : 1);
+
+  for (g = 0; g < ocut; g += 2, h += 2)
+    { d += (nt[h] = o->trace[g]); nt[h+1] = o->trace[g+1]; }
+  for (g = wcut; g < wp->tlen; g += 2, h += 2)
+    { d += (nt[h] = w->trace[g]); nt[h+1] = w->trace[g+1]; }
+  if (o->flags & F_OWNS_TRACE)
+    free(o->trace);
+  o->trace  = nt;
+  o->flags |= F_OWNS_TRACE;
+  op->tlen  = tlen;
+  op->diffs = d;
+  op->aepos = wp->aepos;
+  op->bepos = wp->bepos;
+}
+
+/* the redundancy filter of one align_contigs call on perm[0..n) */
+static void filter_call(fl_rec **perm, int n)
+{ int j, k, where, dist;
+
+  qsort(perm,n,sizeof(fl_rec *),FL_ASORT);
+
+  //  Sweep 1: equal start points or equal end points
+
+  for (j = n-1; j >= 0; j--)
+    { fl_rec  *o  = perm[j];
+      orc_ovl *op = &o->o;
+      for (k = j+1; k < n; k++)
+        { fl_rec  *w  = perm[k];
+          orc_ovl *wp = &w->o;
+          int      same_start, same_end, drop_o;
+
+          if (op->aepos <= wp->abpos)
+            break;
+          if (w->flags & F_ELIMINATED)
+            continue;
+          same_start = (op->abpos == wp->abpos && op->bbpos == wp->bbpos);
+          same_end   = (op->aepos == wp->aepos && op->bepos == wp->bepos);
+          if (same_start && same_end)
+            { drop_o = !(op->diffs < wp->aepos);          /* diffs against aepos, as FastGA.c:3456 */
+              g_filter_cnt[drop_o ? FC_S1_BOTH_DROP_O : FC_S1_BOTH_KEEP_O] += 1;
+            }
+          else if (same_start)
+            { drop_o = !(op->aepos > wp->aepos);
+              g_filter_cnt[drop_o ? FC_S1_START_DROP_O : FC_S1_START_KEEP_O] += 1;
+            }
+          else if (same_end)
+            { drop_o = !(op->abpos < wp->abpos);
+              g_filter_cnt[drop_o ? FC_S1_END_DROP_O : FC_S1_END_KEEP_O] += 1;
+            }
+          else
+            continue;
+          if (drop_o)
+            { o->flags |= F_ELIMINATED;
+              break;
+            }
+          w->flags |= F_ELIMINATED;
+        }
+    }
+
+  //  Sweep 2: paths that meet are fused, a path apart from and boxed in by another is dropped
+
+  for (j = n-1; j >= 0; j--)
+    { fl_rec  *o  = perm[j];
+      orc_ovl *op = &o->o;
+      int      aend0 = op->aepos;
+
+      if (o->flags & F_ELIMINATED)
+        continue;
+      for (k = j+1; k < n; k++)
+        { fl_rec  *w  = perm[k];
+          orc_ovl *wp = &w->o;
+
+          if (op->aepos <= wp->abpos)                   /* o's end is re-read: a fusion moves it */
+            break;
+          if (w->flags & F_ELIMINATED)
+            continue;
+          if (wp->abpos >= aend0)
+            g_filter_cnt[FC_S2_ROW_EXTENDED] += 1;
+          if (op->bepos <= wp->bbpos || op->bbpos >= wp->bepos)
+            { g_filter_cnt[FC_S2_B_DISJOINT] += 1;
+              continue;
+            }
+
+          dist = entwine(op,o->trace,wp,w->trace,&where);
+          if (where != -1)
+            { g_filter_cnt[FC_S2_FUSE] += 1;
+              if (o->flags & F_ELIMINATED)
+                g_filter_cnt[FC_S2_FUSE_DEAD_O] += 1;
+              if (w->flags & F_OWNS_TRACE)
+                g_filter_cnt[FC_S2_FUSE_W_OWNS] += 1;
+              fuse(o,w,where);
+              w->flags |= F_ELIMINATED;
+              continue;
+            }
+          if (dist == 0)
+            { g_filter_cnt[FC_S2_CROSS] += 1;
+              continue;
+            }
+          if ((op->aepos - op->abpos) + F_BOX_FUZZ >= wp->aepos - wp->abpos)
+            { if (wp->aepos <= op->aepos + F_BOX_FUZZ && wp->bbpos >= op->bbpos - F_BOX_FUZZ &&
+                  wp->bepos <= op->bepos + F_BOX_FUZZ)
+                { g_filter_cnt[FC_S2_BOX_DROP_W] += 1;
+                  w->flags |= F_ELIMINATED;
+                  continue;
+                }
+            }
+          else
+            { if (op->aepos <= wp->aepos + F_BOX_FUZZ && op->bbpos >= wp->bbpos - F_BOX_FUZZ &&
+                  op->bepos <= wp->bepos + F_BOX_FUZZ && op->abpos >= wp->abpos - F_BOX_FUZZ)
+                { g_filter_cnt[FC_S2_BOX_DROP_O] += 1;
+                  o->flags |= F_ELIMINATED;              /* o still finishes its row */
+                  continue;
+                }
+            }
+          g_filter_cnt[FC_S2_APART_KEPT] += 1;
+        }
+    }
+}
+
+static int SORT_MAP(const void *x, const void *y)     /* FastGA.c:3800-3835, position for address */
+{ const fl_rec *l = *(fl_rec **) x;
+  const fl_rec *r = *(fl_rec **) y;
+
+  if (l->o.aread != r->o.aread)
+    return (l->o.aread - r->o.aread);
+  if (l->o.abpos != r->o.abpos)
+    return (l->o.abpos - r->o.abpos);
+  if (l->o.bread != r->o.bread)
+    return (l->o.bread - r->o.bread);
+  if (l->o.comp != r->o.comp)
+    return (l->o.comp - r->o.comp);
+  return ((l->pos > r->pos) - (l->pos < r->pos));
+}
+
+/*  orc_filter: in[0..n) are raw alignments in discovery order (traces at tpool + in[i].toff), and
+    every run of equal in[i].grp is the output of one align_contigs call.  Filters each call
+    (do_filter = 0: keeps every record), writes the survivors of each call in sweep order one call
+    after the other, and returns them in R in SORT_MAP order, ties by that position.  */
+int64_t orc_filter(const orc_ovl *in, int64_t n, const uint8_t *tpool, int do_filter, orc_result *R)
+{ fl_rec  *rec  = (fl_rec *) malloc(sizeof(fl_rec)*(n > 0 ? n : 1));
+  fl_rec **perm = (fl_rec **) malloc(sizeof(fl_rec *)*(n > 0 ? n : 1));
+  fl_rec **live = (fl_rec **) malloc(sizeof(fl_rec *)*(n > 0 ? n : 1));
+  int64_t  i, b, e, nlive = 0;
+
+  memset(g_filter_cnt,0,sizeof(g_filter_cnt));
+  for (i = 0; i < n; i++)
+    { rec[i].o = in[i];
+      rec[i].trace = (uint8_t *) tpool + in[i].toff;
+      rec[i].flags = 0;
+      rec[i].pos = -1;
+    }
+  for (b = 0; b < n; b = e)
+    { for (e = b; e < n && in[e].grp == in[b].grp; e++)
+        perm[e-b] = rec+e;
+      if (do_filter)
+        filter_call(perm,(int) (e-b));
+      for (i = 0; i < e-b; i++)
+        if ((perm[i]->flags & F_ELIMINATED) == 0)
+          { perm[i]->pos = nlive;
+            live[nlive++] = perm[i];
+          }
+    }
+
+  qsort(live,nlive,sizeof(fl_rec *),SORT_MAP);
+  for (i = 0; i < nlive; i++)
+    res_push(R,&live[i]->o,live[i]->trace);
+
+  for (i = 0; i < n; i++)
+    if (rec[i].flags & F_OWNS_TRACE)
+      free(rec[i].trace);
+  free(live);
+  free(perm);
+  free(rec);
+  return (nlive);
 }

@@ -162,10 +162,10 @@ def reference(key, inputs, compute):
 
 def ref_alignments(wd, a, b, threads=8, extra=()):
     """FastGA -v -k -T<n> -1:ref <extra> a [b] in workdir: -v counters + count and md5 of the canonical
-    records"""
+    records (aln_md5), and md5 of the same lines in the file's order (aln_order_md5)"""
     st = parse_fastga_log(ref_fastga(wd, a, b, threads=threads, extra=extra))
-    recs = oneview_records(os.path.join(wd, "ref.1aln"))
-    st.update(records=len(recs), aln_md5=md5_lines(recs))
+    recs = oneview_records(os.path.join(wd, "ref.1aln"), ordered=True)
+    st.update(records=len(recs), aln_md5=md5_lines(sorted(recs)), aln_order_md5=md5_lines(recs))
     return st
 
 
@@ -293,9 +293,9 @@ def parse_fastga_log(log):
     return d
 
 
-def oneview_records(path):
+def oneview_records(path, ordered=False):
     """Canonical form of a .1aln: one text line per alignment ('A ..| R | D ..| T ..| X ..'),
-    sorted (SURVEY 8c)."""
+    sorted (SURVEY 8c); ordered: in the file's order instead."""
     out = subprocess.run([os.path.join(REF_DIR, "ONEview"), path], stdout=subprocess.PIPE, text=True,
                          check=True).stdout
     recs, cur = [], None
@@ -310,7 +310,8 @@ def oneview_records(path):
             cur += " | " + line
     if cur is not None:
         recs.append(cur)
-    recs.sort()
+    if not ordered:
+        recs.sort()
     return recs
 
 
@@ -357,8 +358,8 @@ class OrcParams(C.Structure):
 
 
 OVL_DT = np.dtype([("comp", "i4"), ("aread", "i4"), ("bread", "i4"), ("abpos", "i4"), ("bbpos", "i4"),
-                   ("aepos", "i4"), ("bepos", "i4"), ("diffs", "i4"), ("tlen", "i4"), ("toff", "i8")],
-                  align=True)
+                   ("aepos", "i4"), ("bepos", "i4"), ("diffs", "i4"), ("tlen", "i4"), ("grp", "i4"),
+                   ("toff", "i8")], align=True)
 
 
 def make_spec(freq, ave_corr=0.7, tspace=100):
@@ -517,6 +518,73 @@ def pack_overlaps(ov, tp, rank1, rank2, jb, ib):
     return lib.overlaps_from_buffer(buf)
 
 
+FILTER_COUNTERS = ("s1_same_keep_o", "s1_same_drop_o", "s1_start_keep_o", "s1_start_drop_o", "s1_end_keep_o",
+                   "s1_end_drop_o", "s2_b_disjoint", "s2_fuse", "s2_fuse_dead_o", "s2_fuse_w_owns",
+                   "s2_box_drop_w", "s2_box_drop_o", "s2_apart_kept", "s2_cross", "s2_row_extended")
+
+
+def filter(ov, tp, do_filter=True):
+    """The oracle's redundancy filter and final order (orc_filter) on raw alignments ov (OVL_DT rows in
+    discovery order; each run of equal ov["grp"] is one align_contigs call) with trace pool tp: the
+    survivors in .1aln order, as a lib.Alignments"""
+    from fastga_b200 import lib
+    o = orc()
+    o.orc_new_result.restype = C.c_void_p
+    o.orc_filter.restype = C.c_int64
+    o.orc_filter.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]
+    for f in ("orc_result_ovls", "orc_result_traces"):
+        getattr(o, f).restype = C.c_void_p
+        getattr(o, f).argtypes = [C.c_void_p]
+    o.orc_free_result.argtypes = [C.c_void_p]
+    ov = np.ascontiguousarray(ov, dtype=OVL_DT)
+    tp = np.ascontiguousarray(tp, dtype=np.uint8)
+    if tp.size == 0:
+        tp = np.zeros(1, np.uint8)
+    R = C.c_void_p(o.orc_new_result())
+    n = o.orc_filter(ov.ctypes.data, len(ov), tp.ctypes.data, int(do_filter), R)
+    if n > 0:
+        out = np.ctypeslib.as_array(C.cast(o.orc_result_ovls(R), C.POINTER(C.c_uint8)),
+                                    shape=(n * OVL_DT.itemsize,)).view(OVL_DT).copy()
+        tl = int((out["toff"] + out["tlen"]).max())
+        pool = np.ctypeslib.as_array(C.cast(o.orc_result_traces(R), C.POINTER(C.c_uint8)), shape=(max(tl, 1),)).copy()
+    else:
+        out, pool = np.zeros(0, dtype=OVL_DT), np.zeros(1, dtype=np.uint8)
+    o.orc_free_result(R)
+    fields = np.stack([out[f] for f in lib.ALN_FIELDS], axis=1).astype(np.int32).reshape(-1, 9)
+    return lib.Alignments(fields, out["toff"].astype(np.int64), pool, len(ov))
+
+
+def alignment_differences(got, want):
+    """'' when two lib.Alignments hold the same records field by field and trace byte by trace byte, in
+    the same order; else the first difference"""
+    if len(got) != len(want):
+        return "%d records != %d" % (len(got), len(want))
+    for i in range(len(got)):
+        if not np.array_equal(got.fields[i], want.fields[i]):
+            return "record %d: %s != %s" % (i, got.fields[i].tolist(), want.fields[i].tolist())
+        if not np.array_equal(got.trace(i), want.trace(i)):
+            return "record %d: trace %s != %s" % (i, got.trace(i).tolist(), want.trace(i).tolist())
+    return ""
+
+
+def check_filters_and_order(r, st):
+    """an oracle_pipeline(_self) result r against a ref_alignments run st: the product's filter on the
+    oracle's raw records gave the oracle filter's records in its order, and that order is the
+    reference's .1aln order"""
+    d = alignment_differences(r["alns_product"], r["alns"])
+    assert d == "", "fgb_filter != orc_filter: " + d
+    assert md5_lines(r["order_lines"]) == st["aln_order_md5"]
+
+
+def filter_counters():
+    """per outcome (FILTER_COUNTERS), how often the last filter() went through each branch of the two
+    sweeps; s2_fuse counts every fusion, s2_fuse_dead_o and s2_fuse_w_owns the fusions among them into
+    an o its row had already eliminated and with a w that already owned a fused trace"""
+    out = np.zeros(len(FILTER_COUNTERS), dtype=np.int64)
+    orc().orc_filter_counters(out.ctypes.data_as(C.c_void_p))
+    return dict(zip(FILTER_COUNTERS, (int(v) for v in out)))
+
+
 def seed_layout(gA, gB):
     amx, bmx = int(gA.clen.max()), int(gB.clen.max())
     ab = int(amx + bmx).bit_length()
@@ -525,7 +593,9 @@ def seed_layout(gA, gB):
 
 
 def oracle_pipeline(gA, gB, rank=None, **kw):
-    """The whole path through the CPU oracle + the product's host filter.  Returns a dict.
+    """The whole path through the CPU oracle, its own redundancy filter included.  Returns a dict; "alns"
+    holds the oracle's final records, "alns_product" the product's host filter (fgb_filter) on the same
+    raw records, "raw" the raw records and their trace pool.
     rank: (rank of every A contig, of every B contig) in place of contig_rank's, for genomes whose
     length ties leave the order open."""
     from fastga_b200 import lib
@@ -542,11 +612,14 @@ def oracle_pipeline(gA, gB, rank=None, **kw):
     skw = {k: v for k, v in kw.items() if k in ("chain_break", "chain_min", "align_min", "align_rate")}
     ov, tp, nhit = search(recs, layout, gA, gB, pa, pb, gA.freq, **skw)
     ckw = {k: v for k, v in skw.items() if k in ("chain_break", "chain_min")}
+    al = filter(ov, tp)
+    fc = filter_counters()
     O = pack_overlaps(ov, tp, ra, rb, layout[2], layout[3])
-    al = lib.filter_overlaps(O.h, pa, pb, layout[2], layout[3])
+    pal = lib.filter_overlaps(O.h, pa, pb, layout[2], layout[3])
     return dict(tabA=tA, tabB=tB, pstartA=sA, pstartB=sB, nseeds=len(seeds), sumlen=sumlen, seedrecs=recs,
                 nhit=nhit, nchain=len(chains(recs, layout, **ckw)[1]), nraw=len(ov), alns=al,
-                lines=al.canonical_lines(), perm1=pa, perm2=pb)
+                lines=al.canonical_lines(), order_lines=al.canonical_lines_unsorted(), alns_product=pal,
+                filter_counters=fc, raw=(ov, tp), layout=layout, perm1=pa, perm2=pb, rank1=ra, rank2=rb)
 
 
 SELF_COUNTERS = ("straddles", "stale_straddles", "lbord_calls", "hbord_calls")
@@ -577,8 +650,8 @@ def self_counters():
 
 
 def oracle_pipeline_self(g, straddle_zero=False, **kw):
-    """SELF mode (FastGA A) through the CPU oracle + the product's host filter; "counters" holds
-    self_counters() of the search"""
+    """SELF mode (FastGA A) through the CPU oracle, its own redundancy filter included; "counters" holds
+    self_counters() of the search, the rest as oracle_pipeline"""
     from fastga_b200 import lib
     pa, ra = contig_rank(g.clen)
     t, s = gix_build(g, ra)
@@ -589,7 +662,10 @@ def oracle_pipeline_self(g, straddle_zero=False, **kw):
     with self_search(straddle_zero):
         ov, tp, nhit = search(recs, layout, g, g, pa, pa, g.freq, **skw)
         cnt = self_counters()
+    al = filter(ov, tp)
+    fc = filter_counters()
     O = pack_overlaps(ov, tp, ra, ra, layout[2], layout[3])
-    al = lib.filter_overlaps(O.h, pa, pa, layout[2], layout[3])
+    pal = lib.filter_overlaps(O.h, pa, pa, layout[2], layout[3])
     return dict(nseeds=len(seeds), sumlen=sumlen, nhit=nhit, nraw=len(ov), alns=al, lines=al.canonical_lines(),
-                counters=cnt, seedrecs=recs, layout=layout, perm=pa)
+                order_lines=al.canonical_lines_unsorted(), alns_product=pal, filter_counters=fc, raw=(ov, tp),
+                counters=cnt, seedrecs=recs, layout=layout, perm=pa, rank=ra)

@@ -169,6 +169,7 @@ def test_oracle_vs_live_reference_run(tmp_path):
     r = ol.oracle_pipeline(gA, gB)
     assert (r["nseeds"], r["nhit"], r["nraw"], len(r["lines"])) == (st["seeds"], st["hits"], st["alns"], st["kept"])
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
 
 
 @pytest.mark.skipif(not ol.have_ref(), reason="oracle/_ref not built")
@@ -206,6 +207,7 @@ def test_oracle_edge_cases_vs_live_reference(name):
     assert r["nseeds"] == st.get("seeds", 0)
     assert r["nhit"] == st.get("hits", 0) == r["nchain"] and r["nraw"] == st.get("alns", 0)
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
     check(r["alns"], r["nhit"])
 
 
@@ -223,6 +225,7 @@ def test_max_contigs_records_do_not_depend_on_the_filler_tie_order():
     r = ol.oracle_pipeline(gA, gB, rank=(ra, ol.contig_rank(gB.clen)[1]))
     assert r["nseeds"] == st["seeds"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
 
 
 def test_oracle_on_example_regions_vs_live_reference(tmp_path):
@@ -237,6 +240,7 @@ def test_oracle_on_example_regions_vs_live_reference(tmp_path):
     r = ol.oracle_pipeline(formats.genome_from_arrays(A), formats.genome_from_arrays(B))
     assert r["nseeds"] == st.get("seeds", 0)
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
 
 
 def _self_genomes():
@@ -305,3 +309,4 @@ def test_oracle_self_mode_vs_live_reference(name, tmp_path):
     assert abs(r["nseeds"] // 2 - st["seeds"]) < 4
     assert r["nhit"] == st["hits"] and r["nraw"] == st["alns"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)

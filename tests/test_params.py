@@ -166,6 +166,7 @@ def test_oracle_at_parameters_vs_reference(name):
         (st.get("seeds", 0), st["hits"], st["alns"], st["kept"])
     assert r["nchain"] == r["nhit"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
     assert st["records"] >= 5
 
 
@@ -177,4 +178,5 @@ def test_oracle_self_mode_at_parameters_vs_reference():
     assert abs(r["nseeds"] // 2 - st["seeds"]) < pc.SELF_THREADS
     assert r["nhit"] == st["hits"] and r["nraw"] == st["alns"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
     assert st["records"] > 10

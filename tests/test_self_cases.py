@@ -90,6 +90,7 @@ def test_self_genome_vs_reference_single_thread(name, tmp_path):
     assert r["nseeds"] // 2 == st["seeds"]
     assert r["nhit"] == st["hits"] and r["nraw"] == st["alns"]
     assert len(r["lines"]) == st["records"] and ol.md5_lines(r["lines"]) == st["aln_md5"]
+    ol.check_filters_and_order(r, st)
     z = ol.oracle_pipeline_self(g, straddle_zero=True)
     assert z["nhit"] == r["nhit"]
     extra = sc.DIVERGENT_RECORDS if name == "divergence" else 0
