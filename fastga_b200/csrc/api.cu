@@ -547,9 +547,21 @@ static int seeds_merge_impl(const fgb_gix *x1, const fgb_gix *x2, long long amxp
   return FGB_OK;
 }
 
-//  K6: sorts n seed records in d_a (consumed) into a handle
-static int seeds_sort_impl(dblock<rec128> d_a, long long n, const seed_bits &L, long long amxpos, long long bmxpos,
-                           bool self, long long sumlen, long long n1m, fgb_seeds **out, cudaStream_t st)
+//  First key bit of the seed sort.  The lcp field (bits 0..5) never breaks a tie: two seeds that agree on
+//  strand, contigs, band, anti-diagonal and diagonal remainder are the same pair of positions.  Records
+//  that make_seed built in the same call (the merges of merge.cu) skip bit 6 too: forward seeds have
+//  diag = bmxpos + (i - j) and anti = i + j, complement seeds diag = maxdag - (i + j) and
+//  anti = amxpos - (i - j), so on either strand diag & 1 (bit 6) is anti & 1 (bit 12) XOR a constant of
+//  the strand (the key's top bit).  Both are sorted above bit 6, so [7, key) gives the order of
+//  [6, key) -- one 8-bit pass less on a key of 57 to 64 bits.  Records from a caller
+//  (fgb_seeds_from_records) keep bit 6.
+#define SEED_SORT_LO_ANY    6
+#define SEED_SORT_LO_MERGED 7
+
+//  K6: sorts n seed records in d_a (consumed) into a handle, on key bits [bit_lo, L.key)
+static int seeds_sort_impl(dblock<rec128> d_a, long long n, const seed_bits &L, int bit_lo, long long amxpos,
+                           long long bmxpos, bool self, long long sumlen, long long n1m, fgb_seeds **out,
+                           cudaStream_t st)
 { dblock<rec128> d_b; dblock<unsigned char> d_tmp;
   std::unique_ptr<fgb_seeds> s(new fgb_seeds());
   s->self_mode = self ? 1 : 0;
@@ -566,9 +578,7 @@ static int seeds_sort_impl(dblock<rec128> d_a, long long n, const seed_bits &L, 
   CUDA_TRY(d_b.alloc(n+1,st));
   CUDA_TRY(d_tmp.alloc(tmpb,st));
   { stage_timer t(&g_timings.ssort_ms,st);
-    //  from bit 6: the lcp field (bits 0..5) cannot break a tie -- two seeds that agree on strand,
-    //  contigs, band, anti-diagonal and diagonal remainder are the same pair of positions
-    rc = fgb_radix_sort_device(d_a,d_b,n,6,L.key,narrow,d_tmp,tmpb,&inb,&d_hiflag,st);
+    rc = fgb_radix_sort_device(d_a,d_b,n,bit_lo,L.key,narrow,d_tmp,tmpb,&inb,&d_hiflag,st);
   }
   if (rc) return rc;
   if (d_hiflag) CUDA_TRY(cudaMemcpyAsync(&hiflag,d_hiflag,8,cudaMemcpyDeviceToHost,st));
@@ -587,7 +597,7 @@ static int seeds_find_impl(const fgb_gix *x1, const fgb_gix *x2, long long amxpo
   if (rc) return rc;
   dblock<rec128> d_a; long long n = 0, sumlen = 0, n1m = 0;
   if ((rc = seeds_merge_impl(x1,x2,amxpos,bmxpos,freq,self,L,d_a,&n,&sumlen,&n1m,st))) return rc;
-  return seeds_sort_impl(std::move(d_a),n,L,amxpos,bmxpos,self,sumlen,n1m,out,st);
+  return seeds_sort_impl(std::move(d_a),n,L,SEED_SORT_LO_MERGED,amxpos,bmxpos,self,sumlen,n1m,out,st);
 }
 
 //  ---- sharded path: seeds leave the merge unsorted, travel to their A-contig's owner, are sorted there ----
@@ -658,7 +668,7 @@ extern "C" int fgb_seeds_from_records(const void *d_recs, long long n, const int
   dblock<rec128> d_a;
   CUDA_TRY(d_a.alloc(n+1,st));
   if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-  return seeds_sort_impl(std::move(d_a),n,L,amxpos,bmxpos,false,sumlen,0,out,st);
+  return seeds_sort_impl(std::move(d_a),n,L,SEED_SORT_LO_ANY,amxpos,bmxpos,false,sumlen,0,out,st);
 }
 
 extern "C" long long fgb_seeds_size(const fgb_seeds *s) { return s->n; }
@@ -731,7 +741,8 @@ static int align_pipeline(const fgb_genome *A, const fgb_genome *B, bool self, c
     //  the tables go back to the allocator as soon as the merge has read them (two tables + seeds + sort
     //  buffer of a multi-Gbp pair do not fit side by side)
     x1.reset(); x2.reset();
-    if (!rc) rc = seeds_sort_impl(std::move(d_a),n,L,A->maxlen,B->maxlen,self,s.sumlen,s.nkmers1_fwd,&ps,st);
+    if (!rc) rc = seeds_sort_impl(std::move(d_a),n,L,SEED_SORT_LO_MERGED,A->maxlen,B->maxlen,self,s.sumlen,
+                                  s.nkmers1_fwd,&ps,st);
   }
   if (rc) return rc;
   std::unique_ptr<fgb_seeds> sd(ps);

@@ -1451,7 +1451,9 @@ static __device__ int handle_hit(const ext_params &P, Ctx &c, TripleCtx &T, long
 #define SCAN_SMEM 1536          // per warp: La Ua (32 x i64) Lm Um (32 x int) Ma (64 x i64) Mm (64 x int)
 
 //  Bands of a triple: L = [b,m) (band c), U = [m,e) (band c+1, if present).  False: nothing to scan.
-static __device__ bool triple_setup(const ext_params &P, unsigned j, TripleCtx &T, unsigned &b, unsigned &m, unsigned &e)
+//  nseg: the band segments (P.nseg, or the device count before the host has read it)
+static __device__ bool triple_setup_n(const ext_params &P, unsigned nseg, unsigned j, TripleCtx &T, unsigned &b,
+                                      unsigned &m, unsigned &e)
 { const rec128 *S = P.seeds;
   b = P.seg_start[j]; m = P.seg_start[j+1]; e = m;
   rec128 r0 = S[b];
@@ -1465,7 +1467,7 @@ static __device__ bool triple_setup(const ext_params &P, unsigned j, TripleCtx &
           (long long) get_bits(rp,P.p_band,P.band_bits) == T.cdiag-1)
         T.isnew = false;
     }
-  if (j+1 < (unsigned) P.nseg)
+  if (j+1 < nseg)
     { rec128 rn = S[m];
       if (get_bits(rn,P.p_jc,P.jc_bits + P.ic_bits + 1) == grp &&
           (long long) get_bits(rn,P.p_band,P.band_bits) == T.cdiag+1)
@@ -1477,6 +1479,10 @@ static __device__ bool triple_setup(const ext_params &P, unsigned j, TripleCtx &
   T.pairkey = (unsigned) grp;
   return true;
 }
+
+static __device__ __forceinline__ bool triple_setup(const ext_params &P, unsigned j, TripleCtx &T, unsigned &b,
+                                                    unsigned &m, unsigned &e)
+{ return triple_setup_n(P,(unsigned) P.nseg,j,T,b,m,e); }
 
 static __device__ void triple_contigs(const ext_params &P, Ctx &c, TripleCtx &T)
 { rec128 r0 = P.seeds[P.seg_start[T.j]];
@@ -1678,6 +1684,11 @@ struct ChainHit { long long alow, ahgh; int dgmin, dgmax; };
 
 struct ChunkPlan { unsigned w, j, k, nch, sL, sU; };            // work-list position, triple, chunk number, chunks of the triple, band starts
 
+//  hit slots of nplan chunks and ntrip work triples: a list of every chunk's recorded hits, plus one per
+//  chunk and per triple for the chains that close across the cuts
+static __host__ __device__ __forceinline__ unsigned long long chain_hit_cap(unsigned long long nplan, long long ntrip)
+{ return nplan * (CH_HCAP + 1) + (unsigned long long) ntrip + 16; }
+
 struct ChunkOut
 { int nhit, over, first_break, head_closed, tail_valid, empty;
   int h_cov, h_mix, h_dgmin, h_dgmax;
@@ -1686,10 +1697,20 @@ struct ChunkOut
   ChainHit hits[CH_HCAP];
 };
 
-__global__ void chain_plan_kernel(ext_params P, ChunkPlan *__restrict__ plan, int nplan)
-{ int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nplan) return;
-  ChunkPlan c = plan[i];
+//  plan[i] for i < *nplan: chunk k of the long work triple w, first[w] <= i < first[w+1] (first: the
+//  exclusive scan of the chunks per work triple, nlong long triples first); launched over a bound of
+//  *nplan threads
+__global__ void chain_plan_kernel(ext_params P, const unsigned *__restrict__ first, unsigned nlong,
+                                  const unsigned long long *__restrict__ nplan, ChunkPlan *__restrict__ plan)
+{ const long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long) *nplan) return;
+  unsigned w = 0, wh = nlong - 1;                                   // last w with first[w] <= i
+  while (w < wh)
+    { const unsigned md = (w + wh + 1) >> 1;
+      if (first[md] <= (unsigned) i) w = md; else wh = md - 1;
+    }
+  ChunkPlan c;
+  c.w = w; c.k = (unsigned) i - first[w]; c.nch = first[w+1] - first[w];
   c.j = P.work[c.w];
   TripleCtx T; unsigned b, m, e;
   if (!triple_setup(P,c.j,T,b,m,e)) { c.sL = P.seg_start[c.j+1]; c.sU = c.sL; plan[i] = c; return; }
@@ -1733,11 +1754,12 @@ struct ChunkSink
 };
 
 __global__ void __launch_bounds__(128)
-chain_chunk_kernel(ext_params P, const ChunkPlan *__restrict__ plan, int nplan, ChunkOut *__restrict__ outs)
+chain_chunk_kernel(ext_params P, const ChunkPlan *__restrict__ plan, const unsigned long long *__restrict__ nplan,
+                   ChunkOut *__restrict__ outs)
 { __shared__ __align__(16) unsigned char sm[4*SCAN_SMEM];
   const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
-  const int i = blockIdx.x * 4 + wp;
-  if (i >= nplan) return;
+  const long long i = (long long) blockIdx.x * 4 + wp;
+  if (i >= (long long) *nplan) return;
   const ChunkPlan c = plan[i];
   ChunkOut *out = outs + i;
   TripleCtx T; unsigned b, m, e;
@@ -1798,7 +1820,8 @@ chain_chunk_kernel(ext_params P, const ChunkPlan *__restrict__ plan, int nplan, 
 //  one thread per work triple: its chunks in order -> the ordered hit list of the triple
 __global__ void chain_stitch_kernel(ext_params P, const ChunkPlan *__restrict__ plan, const ChunkOut *__restrict__ outs,
                                     const unsigned *__restrict__ first_chunk, int ntrip, ChainHit *__restrict__ hits,
-                                    unsigned long long *__restrict__ hit_used, unsigned long long hit_cap,
+                                    unsigned long long *__restrict__ hit_used,
+                                    const unsigned long long *__restrict__ nplan,
                                     uint2 *__restrict__ hrange /* start, count | 0x80000000: scan in extend_kernel */,
                                     int2 *__restrict__ tinfo /* (strand, contig pair) key and band of the triple */)
 { int w = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1809,6 +1832,7 @@ __global__ void chain_stitch_kernel(ext_params P, const ChunkPlan *__restrict__ 
   if (c1 == c0) { hrange[w] = make_uint2(0u,0x80000000u); return; }          // not pre-scanned
   if (!triple_setup(P,plan[c0].j,T,b,m,e)) { hrange[w] = make_uint2(0u,0u); return; }
   tinfo[w] = make_int2((int) T.pairkey,(int) T.cdiag);
+  const unsigned long long hit_cap = chain_hit_cap(*nplan,ntrip);
   unsigned long long total = 0; bool over = false;
   for (unsigned k = c0; k < c1; k++) { total += (unsigned long long) outs[k].nhit + 1; over |= (outs[k].over != 0); }
   total += 1;
@@ -1870,33 +1894,91 @@ static __device__ __forceinline__ bool upper_differs(const rec128 &a, const rec1
   return (a.hi >> (pos-64)) != (b.hi >> (pos-64));
 }
 
-//  K7: marks the start of every band segment: seeds i-1 and i differ above the anti field.
+//  K7: the band segments of the sorted seeds in one pass.  Seed i starts a segment when seeds i-1 and i
+//  differ above the anti field; seg_start[r] = i for the r-th start.  A tile stages its records and the
+//  one before it in shared memory, flags the starts, ranks them with a block scan and takes the starts of
+//  the tiles before it from a decoupled look-back (status word = count | flag << 62: 1 = the tile's own
+//  count, 2 = inclusive of every tile before it; tiles are handed out by an atomic ticket, so every
+//  predecessor is running).  The tile holding the last seed writes *nseg_out and seg_start[nseg] = n.
 
-__global__ void seg_flag_kernel(const rec128 *__restrict__ seeds, long long n, int p_band,
-                                unsigned *__restrict__ flag)
-{ long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  unsigned f = 1;
-  if (i > 0)
-    { rec128 a = seeds[i-1], b = seeds[i];
-      f = upper_differs(a,b,p_band);
+#define SEG_THREADS 256
+#define SEG_ITEMS   8                         // consecutive seeds a thread ranks (one flag byte each)
+#define SEG_TILE    (SEG_THREADS*SEG_ITEMS)
+#define SEG_AGG     (1ull << 62)
+#define SEG_INC     (2ull << 62)
+#define SEG_MASK    ((1ull << 62) - 1)
+
+static __device__ __forceinline__ unsigned seg_warp_scan(unsigned v, int lane)
+{
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1)
+    { unsigned t = __shfl_up_sync(FULL,v,o);
+      if (lane >= o) v += t;
     }
-  flag[i] = f;
+  return v;
 }
 
-//  (heads are recomputed from the seeds, so the scan can run in place on the flag array)
-__global__ void seg_fill2_kernel(const rec128 *__restrict__ seeds, long long n, int p_band,
-                                 const unsigned *__restrict__ pos, unsigned *__restrict__ seg_start,
-                                 unsigned nseg)
-{ long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x;
-  if (i > n) return;
-  if (i == n) { seg_start[nseg] = (unsigned) n; return; }
-  bool head = true;
-  if (i > 0)
-    { rec128 a = seeds[i-1], b = seeds[i];
-      head = upper_differs(a,b,p_band);
+__global__ void __launch_bounds__(SEG_THREADS)
+seg_scan_kernel(const rec128 *__restrict__ seeds, long long n, int p_band, unsigned *__restrict__ seg_start,
+                u64 *status /* [ntiles], zeroed */, unsigned *__restrict__ ticket, unsigned *__restrict__ nseg_out)
+{ __shared__ rec128 rs[SEG_TILE + 1];                        // rs[0]: the seed before the tile
+  __shared__ __align__(8) unsigned char head[SEG_TILE];
+  __shared__ unsigned wtot[SEG_THREADS/32];
+  __shared__ unsigned tile_s;
+  __shared__ u64 excl_s;
+  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
+  if (tid == 0) tile_s = atomicAdd(ticket,1u);
+  __syncthreads();
+  const unsigned tile = tile_s;
+  const long long t0 = (long long) tile * SEG_TILE;
+  const int cnt = (int) min((long long) SEG_TILE,n - t0);
+  for (int i = tid; i < cnt; i += SEG_THREADS) rs[i+1] = ld_rec(seeds + t0 + i);
+  if (tid == 0 && t0 > 0) rs[0] = ld_rec(seeds + t0 - 1);
+  __syncthreads();
+  for (int i = tid; i < SEG_TILE; i += SEG_THREADS)
+    head[i] = (i < cnt) && (t0 + i == 0 || upper_differs(rs[i],rs[i+1],p_band));
+  __syncthreads();
+  const u64 fl = *reinterpret_cast<const u64 *>(head + tid*SEG_ITEMS);
+  const unsigned c = (unsigned) __popcll(fl);
+  const unsigned inc = seg_warp_scan(c,lane);
+  if (lane == 31) wtot[w] = inc;
+  __syncthreads();
+  unsigned wpre = 0, agg = 0;
+#pragma unroll
+  for (int k = 0; k < SEG_THREADS/32; k++) { if (k < w) wpre += wtot[k]; agg += wtot[k]; }
+  if (w == 0)
+    { u64 excl = 0;
+      if (lane == 0) atomicExch((unsigned long long *) status + tile,(tile == 0 ? SEG_INC : SEG_AGG) | agg);
+      //  look-back: 32 predecessors a round, up to the nearest one that holds an inclusive count
+      volatile const u64 *stt = status;
+      for (long long t = (long long) tile - 1; t >= 0; )
+        { const long long q = t - lane;
+          const u64 v = (q >= 0) ? stt[q] : SEG_INC;
+          const unsigned incm = __ballot_sync(FULL,(v & SEG_INC) != 0);
+          const int lim = incm ? __ffs(incm) - 1 : 31;
+          const unsigned need = (lim == 31) ? FULL : ((2u << lim) - 1u);
+          if (__ballot_sync(FULL,(v >> 62) == 0) & need) continue;  // a predecessor has published nothing yet
+          u64 sum = (lane <= lim) ? (v & SEG_MASK) : 0;
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(FULL,sum,o);
+          excl += sum;
+          if (incm) break;
+          t -= 32;
+        }
+      if (lane == 0)
+        { if (tile != 0) atomicExch((unsigned long long *) status + tile,SEG_INC | (excl + agg));
+          excl_s = excl;
+          if (t0 + cnt == n)
+            { *nseg_out = (unsigned) (excl + agg);
+              seg_start[excl + agg] = (unsigned) n;
+            }
+        }
     }
-  if (head) seg_start[pos[i]] = (unsigned) i;
+  __syncthreads();
+  u64 r = excl_s + wpre + inc - c;
+#pragma unroll
+  for (int k = 0; k < SEG_ITEMS; k++)
+    if ((fl >> (8*k)) & 1) seg_start[r++] = (unsigned) (t0 + tid*SEG_ITEMS + k);
 }
 
 //  K7 prefilter: one thread per band segment.  A chain needs cov >= chain_min and one seed covers
@@ -1949,19 +2031,66 @@ static __device__ bool serial_has_chain(const ext_params &P, const TripleCtx &T,
   return false;
 }
 
-__global__ void prefilter_kernel(ext_params P, unsigned *__restrict__ work_long, unsigned *__restrict__ work_short,
-                                 unsigned *__restrict__ nwork /* [0] long [1] short */,
-                                 unsigned *__restrict__ long_size)
-{ unsigned j = blockIdx.x * blockDim.x + threadIdx.x;
-  if (j >= (unsigned) P.nseg) return;
-  TripleCtx T; unsigned b, m, e;
-  if (!triple_setup(P,j,T,b,m,e) || e - b < (unsigned) ((P.chain_min + 79) / 80)) return;
-  if (e - b > PREF_LONG)
-    { unsigned o = atomicAdd(nwork,1u);
-      work_long[o] = j; long_size[o] = e - b;
+//  Grid-stride over the *nseg segments the segment pass counted; long_sum adds up the long triples' seeds.
+__global__ void prefilter_kernel(ext_params P, const unsigned *__restrict__ nseg_p, unsigned *__restrict__ work_long,
+                                 unsigned *__restrict__ work_short, unsigned *__restrict__ nwork /* [0] long [1] short */,
+                                 unsigned *__restrict__ long_size, unsigned long long *__restrict__ long_sum)
+{ const unsigned nseg = *nseg_p;
+  for (unsigned j = blockIdx.x * blockDim.x + threadIdx.x; j < nseg; j += gridDim.x * blockDim.x)
+    { TripleCtx T; unsigned b, m, e;
+      if (!triple_setup_n(P,nseg,j,T,b,m,e) || e - b < (unsigned) ((P.chain_min + 79) / 80)) continue;
+      if (e - b > PREF_LONG)
+        { unsigned o = atomicAdd(nwork,1u);
+          work_long[o] = j; long_size[o] = e - b;
+          atomicAdd(long_sum,(unsigned long long) (e - b));
+        }
+      else if (serial_has_chain(P,T,b,m,e))
+        work_short[atomicAdd(nwork+1,1u)] = j;
     }
-  else if (serial_has_chain(P,T,b,m,e))
-    work_short[atomicAdd(nwork+1,1u)] = j;
+}
+
+//  The long triples in launch order: key = (smax - seeds) << jbits | triple, ascending = most seeds first,
+//  then the lower triple; sorted as a 16-byte record with hi = 0
+__global__ void long_key_kernel(const unsigned *__restrict__ lj, const unsigned *__restrict__ ls, unsigned nlong,
+                                int jbits, u64 smax, rec128 *__restrict__ key)
+{ const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nlong) return;
+  rec128 r; r.lo = ((smax - ls[q]) << jbits) | lj[q]; r.hi = 0;
+  key[q] = r;
+}
+
+__global__ void long_unpack_kernel(const rec128 *__restrict__ key, unsigned nlong, int jbits, u64 smax,
+                                   unsigned *__restrict__ work, unsigned *__restrict__ wsize)
+{ const unsigned q = blockIdx.x * blockDim.x + threadIdx.x;
+  if (q >= nlong) return;
+  const u64 v = key[q].lo;
+  work[q] = (unsigned) (v & ((1ull << jbits) - 1));
+  wsize[q] = (unsigned) (smax - (v >> jbits));
+}
+
+//  Chunks of chain detection per work triple (the long ones, [0,nlong), are scanned in chunks of `chunk`
+//  merged seeds; first[nwork] = 0 so the scan leaves the chunk total there)
+__global__ void chain_nch_kernel(const unsigned *__restrict__ wsize, unsigned nlong, unsigned nwork, long long chunk,
+                                 unsigned *__restrict__ first)
+{ const unsigned w = blockIdx.x * blockDim.x + threadIdx.x;
+  if (w > nwork) return;
+  unsigned nch = 0;
+  if (w < nlong)
+    { nch = (unsigned) (((unsigned long long) wsize[w] + chunk - 1) / chunk);
+      if (nch < 1) nch = 1;
+    }
+  first[w] = nch;
+}
+
+//  The hit lists into the mapped pinned staging buffer: the first min(*hit_used, hit cap) slots
+__global__ void hits_to_host_kernel(const ChainHit *__restrict__ hits, const unsigned long long *__restrict__ hit_used,
+                                    const unsigned long long *__restrict__ nplan, int ntrip, ChainHit *dst)
+{ unsigned long long m = *hit_used;
+  const unsigned long long cap = chain_hit_cap(*nplan,ntrip);
+  if (m > cap) m = cap;
+  for (unsigned long long q = (unsigned long long) blockIdx.x * blockDim.x + threadIdx.x; q < m;
+       q += (unsigned long long) gridDim.x * blockDim.x)
+    dst[q] = hits[q];
 }
 
 #define WSTATE_BYTES(W) ((W)*(4*4+8) + 32)
@@ -2367,116 +2496,128 @@ struct ExtendOut
 
 //  Phase 1: the band segments of the sorted seeds (P.seg_start, P.nseg), the prefilter, and the work
 //  triples (P.work, P.nwork): long ones first, largest first (the kernel's makespan is its longest
-//  triple, so it must not start late), then the short ones that hold a chain.  wsize gets the seed
-//  counts of the long triples in work order; it stays empty when there are none, or too many to sort.
+//  triple, so it must not start late), then the short ones that hold a chain.  One wait, for the counts
+//  that size the work list.  L.nlong long triples are sorted (none when there are more than 2^20: they
+//  keep the prefilter's order and are scanned in extend_kernel); L.wsize holds their seed counts in work
+//  order, L.sum the seeds of every long triple.
+static int bitlen_u64(u64 v) { int b = 0; while (v > 0) { b += 1; v >>= 1; } return b; }
+
+struct LongTriples { dblock<unsigned> wsize; unsigned nlong = 0; unsigned long long sum = 0; };
+
 static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, dblock<unsigned> &d_seg,
-                          dblock<unsigned> &d_work, std::vector<unsigned> &wsize, cudaStream_t st)
-{ const long long n = S->n, tmpb = fgb_dev_scan_tmp_bytes(n);
-  dblock<u64> d_total; dblock<unsigned> d_flag; dblock<unsigned char> d_tmp;
-  CUDA_TRY(d_total.alloc(1,st));
-  CUDA_TRY(d_flag.alloc(n+1,st));
-  CUDA_TRY(d_tmp.alloc(tmpb,st));
-  seg_flag_kernel<<<(int) ((n + 255) / 256),256,0,st>>>(S->d_rec,n,P.p_band,d_flag);
-  int rc = fgb_dev_exclusive_scan_u32(d_flag,n,d_total,d_tmp,tmpb,st);
-  if (rc) return rc;
-  u64 tot = 0;
-  CUDA_TRY(cudaMemcpyAsync(&tot,d_total,8,cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  const unsigned nseg = (unsigned) tot;
-  CUDA_TRY(d_seg.alloc(nseg+2,st));
-  CUDA_TRY(d_work.alloc(3ll*nseg+3,st));
-  seg_fill2_kernel<<<(int) ((n + 1 + 255) / 256),256,0,st>>>(S->d_rec,n,P.p_band,d_flag,d_seg,nseg);
-  P.seg_start = d_seg; P.nseg = (int) nseg;
-  prefilter_kernel<<<(nseg + 127)/128,128,0,st>>>(P,d_work,d_work + nseg + 1,d_misc + 6,d_work + 2ll*nseg + 2);
-  fgb_count_launch(3);
+                          dblock<unsigned> &d_work, LongTriples &L, cudaStream_t st)
+{ const long long n = S->n;
+  const long long ntiles = (n + SEG_TILE - 1) / SEG_TILE;
+  //  a long triple holds more than PREF_LONG seeds, and a seed lies in at most two triples (its own band
+  //  segment's and the one below), so there are at most 2n / 65 of them
+  const long long lcap = n / 32 + 2;
+  dblock<u64> d_status; dblock<unsigned> d_cand;
+  CUDA_TRY(d_status.alloc((size_t) ntiles + 1,st));
+  CUDA_TRY(d_seg.alloc((size_t) n + 2,st));
+  CUDA_TRY(d_cand.alloc((size_t) (2*lcap + n + 1),st));           // long triples | their sizes | short ones
+  CUDA_TRY(cudaMemsetAsync(d_status,0,8*((size_t) ntiles + 1),st));
+  unsigned *d_nseg = d_misc + 11;
+  seg_scan_kernel<<<(unsigned) ntiles,SEG_THREADS,0,st>>>(S->d_rec,n,P.p_band,d_seg,d_status,
+                                                          (unsigned *) (d_status + ntiles),d_nseg);
+  int dev = 0, nsm = 132;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
+  const long long pb = (n + 127) / 128 < 16ll*nsm ? (n + 127) / 128 : 16ll*nsm;
+  P.seg_start = d_seg;
+  prefilter_kernel<<<(unsigned) pb,128,0,st>>>(P,d_nseg,d_cand,d_cand + 2*lcap,d_misc + 6,d_cand + lcap,
+                                               (unsigned long long *) (d_misc + 12));
+  fgb_count_launch(2);
   CUDA_TRY(cudaGetLastError());
-  unsigned nw2[2];
-  CUDA_TRY(cudaMemcpyAsync(nw2,d_misc + 6,8,cudaMemcpyDeviceToHost,st));
+  unsigned cnt[8];                                           // words 6-13 of d_misc
+  CUDA_TRY(cudaMemcpyAsync(cnt,d_misc + 6,32,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  if (nw2[0] >= 1 && nw2[0] <= (1u << 20))
-    { std::vector<unsigned> lj(nw2[0]), ls(nw2[0]), ord(nw2[0]);
-      CUDA_TRY(cudaMemcpyAsync(lj.data(),d_work,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
-      CUDA_TRY(cudaMemcpyAsync(ls.data(),d_work + 2ll*nseg + 2,4ull*nw2[0],cudaMemcpyDeviceToHost,st));
-      CUDA_TRY(cudaStreamSynchronize(st));
-      for (unsigned q = 0; q < nw2[0]; q++) ord[q] = q;
-      std::sort(ord.begin(),ord.end(),[&](unsigned a, unsigned b)
-                { return ls[a] != ls[b] ? ls[a] > ls[b] : lj[a] < lj[b]; });
-      std::vector<unsigned> sj(nw2[0]);
-      wsize.resize(nw2[0]);
-      for (unsigned q = 0; q < nw2[0]; q++) { sj[q] = lj[ord[q]]; wsize[q] = ls[ord[q]]; }
-      CUDA_TRY(cudaMemcpyAsync(d_work,sj.data(),4ull*nw2[0],cudaMemcpyHostToDevice,st));
-      CUDA_TRY(cudaStreamSynchronize(st));
+  const unsigned nseg = cnt[5], nlong = cnt[0], nshort = cnt[1];
+  L.sum = (unsigned long long) cnt[6] | ((unsigned long long) cnt[7] << 32);
+  P.nseg = (int) nseg;
+  CUDA_TRY(d_work.alloc((size_t) nlong + nshort + 1,st));
+  if (nlong >= 1 && nlong <= (1u << 20))
+    { const int sbits = bitlen_u64((u64) n), jbits = bitlen_u64((u64) nseg);
+      const u64 smax = (1ull << sbits) - 1;
+      const long long tmpb = fgb_sort128_tmp_bytes(nlong);
+      dblock<rec128> d_ka, d_kb; dblock<unsigned char> d_tmp;
+      CUDA_TRY(d_ka.alloc((size_t) nlong + 1,st));
+      CUDA_TRY(d_kb.alloc((size_t) nlong + 1,st));
+      CUDA_TRY(d_tmp.alloc((size_t) tmpb,st));
+      CUDA_TRY(L.wsize.alloc((size_t) nlong,st));
+      long_key_kernel<<<(nlong + 255)/256,256,0,st>>>(d_cand,d_cand + lcap,nlong,jbits,smax,d_ka);
+      int inb = 0; u64 *d_hf = NULL;
+      int rc = fgb_radix_sort_device(d_ka,d_kb,nlong,0,sbits + jbits,1,d_tmp,tmpb,&inb,&d_hf,st);
+      if (rc) return rc;
+      long_unpack_kernel<<<(nlong + 255)/256,256,0,st>>>(inb ? d_kb : d_ka,nlong,jbits,smax,d_work,L.wsize);
+      fgb_count_launch(2);
+      CUDA_TRY(cudaGetLastError());
+      L.nlong = nlong;
     }
-  CUDA_TRY(cudaMemcpyAsync(d_work + nw2[0],d_work + nseg + 1,sizeof(unsigned)*nw2[1],
-                           cudaMemcpyDeviceToDevice,st));
-  P.work = d_work; P.nwork = (int) (nw2[0] + nw2[1]);
+  else if (nlong > 0)
+    CUDA_TRY(cudaMemcpyAsync(d_work,d_cand,sizeof(unsigned)*nlong,cudaMemcpyDeviceToDevice,st));
+  if (nshort > 0)
+    CUDA_TRY(cudaMemcpyAsync(d_work + nlong,d_cand + 2*lcap,sizeof(unsigned)*nshort,cudaMemcpyDeviceToDevice,st));
+  P.work = d_work; P.nwork = (int) (nlong + nshort);
   return FGB_OK;
 }
 
-//  Phase 2: chain detection of the long work triples, chunk-parallel (chain_plan / chain_chunk /
-//  chain_stitch; the short ones are scanned in extend_kernel), `chunk` merged seeds a chunk.  The hit
-//  lists stay in d_hits for the kernel and come to the host (X.hrange, X.tinfo, X.hh) in one staged
-//  download.
-static int chain_detect(const ext_params &P, const std::vector<unsigned> &wsize, long long chunk, unsigned *d_misc,
+//  Phase 2: chain detection of the sorted long work triples, chunk-parallel (chain_plan / chain_chunk /
+//  chain_stitch; the short ones are scanned in extend_kernel), `chunk` merged seeds a chunk.  The chunk
+//  plan is built on the device from the triples' sizes, every kernel runs over a bound of the chunk count
+//  (sum of ceil(size / chunk) <= L.sum / chunk + L.nlong).  The hit lists stay in d_hits for the kernel and
+//  come to the host (X.hrange, X.tinfo, X.hh) through the pinned staging buffer, with one wait.
+static int chain_detect(const ext_params &P, const LongTriples &L, long long chunk, unsigned *d_misc,
                         dblock<ChainHit> &d_hits, ExtendPlan &X, cudaStream_t st)
-{ const unsigned nwork = (unsigned) P.nwork;
-  std::vector<ChunkPlan> plan;
-  std::vector<unsigned> first(nwork + 1);
-  for (unsigned w = 0; w < nwork; w++)
-    { unsigned nch = 0;
-      if (w < wsize.size())
-        { nch = (unsigned) (((unsigned long long) wsize[w] + chunk - 1) / chunk);
-          if (nch < 1) nch = 1;
-        }
-      first[w] = (unsigned) plan.size();
-      for (unsigned k = 0; k < nch; k++)
-        { ChunkPlan c; c.w = w; c.j = 0; c.k = k; c.nch = nch; c.sL = c.sU = 0; plan.push_back(c); }
-    }
-  first[nwork] = (unsigned) plan.size();
-  const int nplan = (int) plan.size();
-  const unsigned long long hit_cap = (unsigned long long) nplan * (CH_HCAP + 1) + nwork + 16;
+{ const unsigned nwork = (unsigned) P.nwork, nlong = L.nlong;
+  const unsigned long long pmax = L.sum / (unsigned long long) chunk + nlong + 1;
+  const unsigned long long cap_max = chain_hit_cap(pmax,nwork);
+  const long long tmpb = fgb_dev_scan_tmp_bytes((long long) nwork + 1);
   dblock<ChunkPlan> d_plan; dblock<ChunkOut> d_couts; dblock<unsigned> d_first;
-  dblock<uint2> d_hrange; dblock<int2> d_tinfo;
-  CUDA_TRY(d_plan.alloc((size_t) nplan,st));
-  CUDA_TRY(d_couts.alloc((size_t) nplan,st));
-  CUDA_TRY(d_first.alloc((size_t) (nwork + 1),st));
-  CUDA_TRY(d_hits.alloc((size_t) hit_cap,st));
+  dblock<uint2> d_hrange; dblock<int2> d_tinfo; dblock<u64> d_nplan; dblock<unsigned char> d_tmp;
+  CUDA_TRY(d_plan.alloc((size_t) pmax,st));
+  CUDA_TRY(d_couts.alloc((size_t) pmax,st));
+  CUDA_TRY(d_first.alloc((size_t) nwork + 1,st));
+  CUDA_TRY(d_hits.alloc((size_t) cap_max,st));
   CUDA_TRY(d_hrange.alloc((size_t) nwork,st));
   CUDA_TRY(d_tinfo.alloc((size_t) nwork,st));
-  CUDA_TRY(cudaMemcpyAsync(d_plan,plan.data(),sizeof(ChunkPlan)*(size_t) nplan,cudaMemcpyHostToDevice,st));
-  CUDA_TRY(cudaMemcpyAsync(d_first,first.data(),sizeof(unsigned)*(size_t) (nwork + 1),cudaMemcpyHostToDevice,st));
+  CUDA_TRY(d_nplan.alloc(1,st));
+  CUDA_TRY(d_tmp.alloc((size_t) tmpb,st));
   CUDA_TRY(cudaMemsetAsync(d_misc + 8,0,8,st));
-  chain_plan_kernel<<<(nplan + 127)/128,128,0,st>>>(P,d_plan,nplan);
-  chain_chunk_kernel<<<(nplan + 3)/4,128,0,st>>>(P,d_plan,nplan,d_couts);
+  chain_nch_kernel<<<(nwork + 1 + 255)/256,256,0,st>>>(L.wsize,nlong,nwork,chunk,d_first);
+  fgb_count_launch(1);
+  int rc = fgb_dev_exclusive_scan_u32(d_first,(long long) nwork + 1,d_nplan,d_tmp,tmpb,st);
+  if (rc) return rc;
+  chain_plan_kernel<<<(unsigned) ((pmax + 127)/128),128,0,st>>>(P,d_first,nlong,d_nplan,d_plan);
+  chain_chunk_kernel<<<(unsigned) ((pmax + 3)/4),128,0,st>>>(P,d_plan,d_nplan,d_couts);
   chain_stitch_kernel<<<(nwork + 127)/128,128,0,st>>>(P,d_plan,d_couts,d_first,(int) nwork,d_hits,
-                                                     (unsigned long long *) (d_misc + 8),hit_cap,d_hrange,d_tinfo);
+                                                     (unsigned long long *) (d_misc + 8),d_nplan,d_hrange,d_tinfo);
   fgb_count_launch(3);
+  //  staging layout: hits used, chunks | hrange | tinfo | the hit lists
+  const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork;
+  const size_t o4 = (o3 + 15) & ~(size_t) 15;
+  unsigned char *hp, *dp;
+  CUDA_TRY(pinned_staging(o4 + sizeof(ChainHit)*(size_t) cap_max,&hp));
+  CUDA_TRY(cudaHostGetDevicePointer((void **) &dp,hp,0));
+  hits_to_host_kernel<<<2*132,256,0,st>>>(d_hits,(const unsigned long long *) (d_misc + 8),d_nplan,(int) nwork,
+                                          (ChainHit *) (dp + o4));
+  fgb_count_launch(1);
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaStreamSynchronize(st));                 // plan / first are host vectors
-  //  the small result arrays come back through the pinned staging buffer: three copies in flight and
-  //  one synchronisation instead of a staged, synchronous copy each
+  CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(hp + 8,d_nplan,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaStreamSynchronize(st));
+  unsigned long long nplan = 0;
+  memcpy(&X.hused,hp,8);
+  memcpy(&nplan,hp + 8,8);
   X.hrange.resize(nwork); X.tinfo.resize(nwork);
-  { const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork;
-    unsigned char *hp;
-    CUDA_TRY(pinned_staging(o3,&hp));
-    CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    memcpy(&X.hused,hp,8);
-    memcpy(X.hrange.data(),hp + o1,sizeof(uint2)*(size_t) nwork);
-    memcpy(X.tinfo.data(),hp + o2,sizeof(int2)*(size_t) nwork);
-  }
-  X.hasked = X.hused; X.hit_cap = hit_cap; X.nplan = nplan;
-  if (X.hused > hit_cap) X.hused = hit_cap;
+  memcpy(X.hrange.data(),hp + o1,sizeof(uint2)*(size_t) nwork);
+  memcpy(X.tinfo.data(),hp + o2,sizeof(int2)*(size_t) nwork);
+  X.hit_cap = chain_hit_cap(nplan,nwork); X.nplan = (long long) nplan;
+  X.hasked = X.hused;
+  if (X.hused > X.hit_cap) X.hused = X.hit_cap;
   X.hh.resize((size_t) X.hused + 1);
-  if (X.hused > 0)
-    { unsigned char *hp;
-      CUDA_TRY(pinned_staging(sizeof(ChainHit)*(size_t) X.hused,&hp));
-      CUDA_TRY(cudaMemcpyAsync(hp,d_hits,sizeof(ChainHit)*(size_t) X.hused,cudaMemcpyDeviceToHost,st));
-      CUDA_TRY(cudaStreamSynchronize(st));
-      memcpy(X.hh.data(),hp,sizeof(ChainHit)*(size_t) X.hused);
-    }
+  memcpy(X.hh.data(),hp + o4,sizeof(ChainHit)*(size_t) X.hused);
   return FGB_OK;
 }
 
@@ -2719,7 +2860,8 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   CUDA_TRY(d_counters.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_counters,0,16*8,st));
   P.counters = d_counters;
-  //  words 1 queue, 2 failed items, 4-5 record bytes, 6-7 prefilter counts, 8-9 hits listed, 10 failure reasons
+  //  words 1 queue, 2 failed items, 4-5 record bytes, 6-7 prefilter counts, 8-9 hits listed, 10 failure reasons,
+  //  11 band segments, 12-13 seeds of the long triples
   CUDA_TRY(d_misc.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
 
@@ -2727,11 +2869,11 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   ExtendPlan X;
   if (S->n > 0)
     { ev_timer t(0,st);
-      std::vector<unsigned> wsize;
-      int rc = extend_triples(P,S,d_misc,d_seg,d_work,wsize,st);
+      LongTriples L;
+      int rc = extend_triples(P,S,d_misc,d_seg,d_work,L,st);
       if (rc) return rc;
-      if (!wsize.empty() && chunk > 0)
-        { rc = chain_detect(P,wsize,chunk,d_misc,d_hits,X,st);
+      if (L.nlong > 0 && chunk > 0)
+        { rc = chain_detect(P,L,chunk,d_misc,d_hits,X,st);
           if (rc) return rc;
           P.hits = d_hits;
         }
@@ -2762,16 +2904,16 @@ extern "C" int fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min
   dblock<unsigned> d_misc, d_seg, d_work; dblock<ChainHit> d_hits;
   CUDA_TRY(d_misc.alloc(16,st));
   CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
-  std::vector<unsigned> wsize;
-  int rc = extend_triples(P,S,d_misc,d_seg,d_work,wsize,st);
+  LongTriples L;
+  int rc = extend_triples(P,S,d_misc,d_seg,d_work,L,st);
   if (rc) return rc;
   ExtendPlan X;
-  if (!wsize.empty() && chunk_seeds > 0)
-    { rc = chain_detect(P,wsize,chunk_seeds,d_misc,d_hits,X,st);
+  if (L.nlong > 0 && chunk_seeds > 0)
+    { rc = chain_detect(P,L,chunk_seeds,d_misc,d_hits,X,st);
       if (rc) return rc;
     }
   const long long nwork = P.nwork;
-  info[0] = nwork; info[1] = (long long) wsize.size(); info[2] = (long long) X.hused;
+  info[0] = nwork; info[1] = (long long) L.nlong; info[2] = (long long) X.hused;
   info[3] = (long long) X.hasked; info[4] = (long long) X.hit_cap; info[5] = X.nplan;
   if (nwork > trip_cap || (long long) X.hused > hits_cap) return FGB_ERR_OVERFLOW;
   //  the end of a triple: the next band segment too when it is the band above in the same group
@@ -2796,7 +2938,7 @@ extern "C" int fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min
       const uint2 hr = X.hrange.empty() ? make_uint2(0u,0x80000000u) : X.hrange[(size_t) w];
       const int2 ti = X.tinfo.empty() ? make_int2(-1,0) : X.tinfo[(size_t) w];
       long long *t = trip + 7*w;
-      t[0] = seg[j]; t[1] = e; t[2] = (w < (long long) wsize.size()); t[3] = ti.x; t[4] = ti.y; t[5] = hr.x; t[6] = hr.y;
+      t[0] = seg[j]; t[1] = e; t[2] = (w < (long long) L.nlong); t[3] = ti.x; t[4] = ti.y; t[5] = hr.x; t[6] = hr.y;
     }
   for (unsigned long long q = 0; q < X.hused; q++)
     { const ChainHit &h = X.hh[(size_t) q];
