@@ -214,32 +214,24 @@ static void gix_bytes(const fgb_genome *g, fgb_gix *x)        // GIXmake.c:1888-
 //  K1..K4: syncmer scan -> 128-bit records laid out by prefix bin -> bucket sort on the whole record ->
 //  2^24 prefix index.
 
-#define GIX_FWD_ONLY 0x80000000u     // flag bit carried in `phi` down to syncmer_kernel
+#define GIX_FWD_ONLY 0x80000000u     // flag bit carried in `phi` down to the syncmer scan
 
-//  The k-mer partition a table's scan starts (fgb_kmer_sort_digit_device): the partition sorts bits
-//  [fsh, 24) of the 12-base prefix, fsh chosen for an upper bound of n, by a first digit of dbits bits that
-//  the scan's emit pass lays out and 8-bit Onesweep passes above it.  The first digit takes what is left
-//  over by as few passes as leave it at most 9 bits; the scan's count pass gives the histogram of the
-//  first pass's digit in hist.
-struct first_digit
-{ int fsh = 0, dbits = 8;
+//  How the syncmer scan laid its records out for the k-mer sort (fgb_kmer_sort_device): in runs by the first
+//  digit of the k-mer partition, bits [fsh, fsh+dbits) of the 12-base prefix, with the histogram of the 8
+//  prefix bits above it in hist.  dbits = 0: no layout, the records are in any order.
+struct scan_layout
+{ int fsh = 0, dbits = 0;
   dblock<unsigned long long> hist;
-  first_digit(long long nmax, unsigned plo, unsigned phi)
-    { fsh = fgb_kmer_bin_shift(nmax,plo,phi);
-      int bits = 24 - fsh, passes = (bits - 9 + 7) / 8;
-      if (passes < 1) passes = 1;
-      dbits = bits - 8*passes;
-    }
 };
 
-//  K1/K2: syncmer scan + record build of the contigs selected by `mask` (NULL: all) into a fresh
-//  device buffer of *n unsorted records (room for n+1).  *nrev = reverse entries left out (fwd-only).
-//  fd == NULL: the records are packed tile after tile.  Otherwise the count pass counts them per tile and
-//  first digit of the k-mer partition, at the resolution the k-mer sort would pick for an upper bound of n
-//  (two records per scanned position), and the emit pass stores them in runs by that digit.
+//  K1/K2: syncmer scan + record build of the contigs selected by `mask` (NULL: all) into a fresh device buffer
+//  of *n records (room for n+1).  *nrev = reverse entries left out (fwd-only).  The count pass counts the
+//  records per tile and first digit of the k-mer partition, at the resolution the k-mer sort would pick for
+//  an upper bound of n (two records per scanned position), and the emit pass stores them in runs by that
+//  digit; lay describes the result.
 static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo, unsigned phi_flags,
                     dblock<rec128> &d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
-                    first_digit **fd_out, cudaStream_t st)
+                    scan_layout &lay, cudaStream_t st)
 { int T = fgb_sc_tile();
   std::vector<int> tc, ts;
   long long npos = 0;
@@ -252,17 +244,13 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
   int ntiles = (int) tc.size();
   dblock<int> d_tc, d_ts; dblock<unsigned> d_cnt;
   dblock<u64> d_buck, d_total; dblock<unsigned char> d_tmp;
-  std::unique_ptr<first_digit> fd;
-  long long ncnt = ntiles;                 // per tile, or per (digit, tile)
   int rc;
   u64 total = 0, rdropped = 0;
-  if (fd_out)
-    { const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
-      fd.reset(new first_digit(2*npos,plo,phi > plo ? phi : plo + 1));    // an empty range still gets one bin
-      CUDA_TRY(fd->hist.alloc(256,st));
-      ncnt = (long long) ntiles << fd->dbits;
-    }
+  const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
+  fgb_kmer_first_digit(2*npos,plo,phi > plo ? phi : plo + 1,&lay.fsh,&lay.dbits);    // an empty range still gets one bin
+  const long long ncnt = (long long) ntiles << lay.dbits;
   const long long tmpb = fgb_dev_scan_tmp_bytes(ncnt);
+  CUDA_TRY(lay.hist.alloc(256,st));
   CUDA_TRY(d_tc.alloc(ntiles+1,st));
   CUDA_TRY(d_ts.alloc(ntiles+1,st));
   CUDA_TRY(d_cnt.alloc(ncnt+1,st));
@@ -272,12 +260,8 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
   CUDA_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
   { stage_timer t(&g_timings.scan_ms,st);
-    if (fd)
-      rc = fgb_syncmer_digit_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_cnt,
-                                          fd->fsh,fd->dbits,fd->hist,d_total,d_tmp,tmpb,plo,phi_flags,st);
-    else
-      rc = fgb_syncmer_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,
-                                    d_buck,d_total,d_tmp,tmpb,plo,phi_flags,st);
+    rc = fgb_syncmer_digit_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_cnt,
+                                        lay.fsh,lay.dbits,lay.hist,d_total,d_tmp,tmpb,plo,phi_flags,st);
     if (rc) return rc;
     CUDA_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
     if (buck1024) CUDA_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
@@ -288,23 +272,18 @@ static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo
   dblock<rec128> d_a;
   CUDA_TRY(d_a.alloc(total+1,st));
   { stage_timer t(&g_timings.scan_ms,st);
-    if (fd)
-      rc = fgb_syncmer_digit_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,fd->fsh,
-                                         fd->dbits,(long long) total,d_a,plo,phi_flags,st);
-    else
-      rc = fgb_syncmer_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,d_a,plo,phi_flags,st);
+    rc = fgb_syncmer_digit_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,lay.fsh,
+                                       lay.dbits,(long long) total,d_a,plo,phi_flags,st);
   }
   if (rc) return rc;
   CUDA_TRY(cudaStreamSynchronize(st));                   // tc/ts must outlive the copies
   d_recs = std::move(d_a); *n_out = (long long) total; *nrev = (long long) rdropped;
-  if (fd_out) *fd_out = fd.release();
   return FGB_OK;
 }
 
 //  K3/K4: sorts the records in d_a (consumed: it ends up inside the handle or is released) whose
-//  12-base prefixes lie in [plo,phi), builds the prefix index and the LCP bytes.  fd: the first digit the
-//  scan laid d_a out by; NULL: records in any order (the partition passes lay them out).
-static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const first_digit *fd,
+//  12-base prefixes lie in [plo,phi), laid out as lay says, builds the prefix index and the LCP bytes.
+static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const scan_layout &lay,
                       cudaStream_t st, bool index = true)
 { dblock<rec128> d_b; dblock<unsigned char> d_stmp;
   long long stmpb = fgb_sort128_tmp_bytes(n);
@@ -317,10 +296,7 @@ static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo,
       CUDA_TRY(x->d_adj.alloc((size_t) n + 32,st));
     }
   { stage_timer t(&g_timings.ksort_ms,st);
-    if (fd)
-      rc = fgb_kmer_sort_digit_device(d_a,d_b,n,plo,phi,fd->fsh,fd->dbits,fd->hist,d_stmp,stmpb,&inb,st);
-    else
-      rc = fgb_kmer_sort_range_device(d_a,d_b,n,plo,phi,d_stmp,stmpb,&inb,st);
+    rc = fgb_kmer_sort_device(d_a,d_b,n,plo,phi,lay.fsh,lay.dbits,lay.hist,d_stmp,stmpb,&inb,st);
   }
   if (rc) return rc;
   x->d_tab = std::move(inb ? d_b : d_a);                  // the other side goes back as the call returns
@@ -343,16 +319,16 @@ static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags
   x->ncontig = g->ncontig;
   x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
   dblock<rec128> d_a; long long n = 0, nrev = 0;
-  //  the scan lays the records out by the partition's first digit; FGB_KSORT_PARTITION=1 packs them by tile
-  //  and runs every partition pass with Onesweep instead (both paths can be compared in one process)
-  const char *part_env = getenv("FGB_KSORT_PARTITION");
-  const bool packed = part_env != NULL && atoi(part_env) != 0;
-  first_digit *fdp = NULL;
-  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,packed ? NULL : &fdp,st);
-  std::unique_ptr<first_digit> fd(fdp);
+  scan_layout lay;
+  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,lay,st);
   if (rc) return rc;
   x->n_both = n + nrev;
-  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,fd.get(),st,index))) return rc;
+  //  FGB_KSORT_PARTITION=1: the sort ignores the scan's layout and runs every partition pass in Onesweep, a
+  //  second, independent route to the same table (both can be compared in one process)
+  const char *part_env = getenv("FGB_KSORT_PARTITION");
+  const bool ignore_layout = part_env != NULL && atoi(part_env) != 0;
+  const scan_layout none;
+  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,ignore_layout ? none : lay,st,index))) return rc;
   *out = x.release();
   return FGB_OK;
 }
@@ -380,11 +356,13 @@ extern "C" int fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned p
  **********************************************************************************************/
 
 //  unsorted k-mer records of the contigs with mask[c] != 0 (device buffer handed to the caller:
-//  fgb_device_free); fwd_only: forward-strand entries only (the adaptamer side)
+//  fgb_device_free); fwd_only: forward-strand entries only (the adaptamer side).  The scan's layout is
+//  dropped: the caller regroups the records by owner and each owner sorts its share from any order.
 extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only,
                               void **d_recs, long long *n, void *stream)
 { dblock<rec128> d; long long nrev = 0;
-  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),d,n,&nrev,NULL,NULL,(cudaStream_t) stream);
+  scan_layout lay;
+  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),d,n,&nrev,NULL,lay,(cudaStream_t) stream);
   if (rc) return rc;
   *d_recs = d.release();
   return FGB_OK;
@@ -402,7 +380,7 @@ extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned pl
   dblock<rec128> d_a;
   CUDA_TRY(d_a.alloc(n+1,st));
   if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-  int rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,NULL,st);
+  int rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,scan_layout(),st);
   if (rc) return rc;
   *out = x.release();
   return FGB_OK;

@@ -3,7 +3,6 @@
 //
 // Replaces (reference file:line):
 //   sample_thread / scan_thread      GIXmake.c:164-328, 406-611    -> syncmer_digit_count/emit_kernel
-//                                                                     (syncmer_kernel<0/1>: by tile)
 //   setup_thread_plain               GIXmake.c:802-980             -> emit of 128-bit records
 //   msd_sort                         MSDsort.c:404                 -> sort128.cu (10 byte passes)
 //   compress_thread / k_sort writer  GIXmake.c:1211-1278,1300-1596 -> kix_index/ktab_export kernels
@@ -195,7 +194,7 @@ static __device__ __forceinline__ rec128 rev_rec(const u64 *sw, int s, unsigned 
   return r;
 }
 
-//  The digit-partitioned scan ranks a tile's records by the first digit of the k-mer partition, bits
+//  The scan ranks a tile's records by the first digit of the k-mer partition, bits
 //  [dsh, dsh+dbits) of the 12-base prefix (dbits <= SC_DBITS).  Its emit pass stages them in shared memory
 //  in digit order and stores each digit's run with consecutive lanes.  A tile of up to SC_STAGE records
 //  (a both-strand tile holds about 3.2 K) is staged at once, by all its threads; a more crowded one in
@@ -207,14 +206,14 @@ static __device__ __forceinline__ rec128 rev_rec(const u64 *sw, int s, unsigned 
 static_assert(SC_THREADS/SC_ROUNDS*SC_PPT*2 <= SC_STAGE, "a round of a crowded tile must fit the stage");
 #define SC_STAGE_SMEM (SC_STAGE*(sizeof(rec128) + sizeof(unsigned short)))
 
-//  EMIT = 0: count pass (sampler histogram; per-tile record counts, or with DIGIT the [digit][tile] count
-//  matrix dmat and the 256-bin histogram nhist of the 8 prefix bits above the digit).  EMIT = 1: emit pass
-//  (records at the tile offsets in tile_count, or with DIGIT at the bases of the scanned dmat).
-template<int EMIT, bool DIGIT> static __device__ __forceinline__ void
+//  EMIT = 0: count pass (sampler histogram, the [digit][tile] count matrix dmat and the 256-bin histogram
+//  nhist of the 8 prefix bits above the digit).  EMIT = 1: emit pass (records at the bases of the scanned
+//  dmat).
+template<int EMIT> static __device__ __forceinline__ void
 syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
              const long long *__restrict__ woff, const int *__restrict__ crank,
              const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
-             unsigned *__restrict__ tile_count, unsigned long long *__restrict__ buck1024,
+             unsigned long long *__restrict__ buck1024,
              rec128 *__restrict__ out, unsigned plo, unsigned phi_flags,
              unsigned *__restrict__ dmat, int dsh, int dbits, unsigned long long *__restrict__ nhist,
              unsigned nlim)
@@ -222,10 +221,10 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
   __shared__ unsigned char tn[256], tc[256];
   __shared__ unsigned wsum[SC_THREADS/32];
   __shared__ unsigned hist[EMIT == 0 ? 1024 : 1];
-  __shared__ unsigned dcnt[DIGIT ? (1 << SC_DBITS) : 1];
-  __shared__ unsigned dloc[DIGIT && EMIT ? (1 << SC_DBITS) : 1];
-  __shared__ unsigned dbase[DIGIT && EMIT ? (1 << SC_DBITS) : 1];
-  __shared__ unsigned nh[DIGIT && !EMIT ? 256 : 1];
+  __shared__ unsigned dcnt[1 << SC_DBITS];
+  __shared__ unsigned dloc[EMIT ? (1 << SC_DBITS) : 1];
+  __shared__ unsigned dbase[EMIT ? (1 << SC_DBITS) : 1];
+  __shared__ unsigned nh[EMIT ? 1 : 256];
 
   //  bit 31 of phi_flags: forward-strand entries only (the table is only ever the adaptamer side
   //  of a merge, where reverse entries never seed, FastGA.c:921-928)
@@ -243,12 +242,11 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
   tc[tid] = c_TC[tid];
   if (EMIT == 0)
     for (int i = tid; i < 1024; i += SC_THREADS) hist[i] = 0;
-  if (DIGIT)
-    for (int i = tid; i < (1 << SC_DBITS); i += SC_THREADS)
-      { dcnt[i] = 0;
-        if (EMIT) dbase[i] = (unsigned) i < nd ? dmat[(size_t) i*gridDim.x + blockIdx.x] : 0;
-      }
-  if constexpr (DIGIT && !EMIT) nh[tid] = 0;
+  for (int i = tid; i < (1 << SC_DBITS); i += SC_THREADS)
+    { dcnt[i] = 0;
+      if (EMIT) dbase[i] = (unsigned) i < nd ? dmat[(size_t) i*gridDim.x + blockIdx.x] : 0;
+    }
+  if constexpr (!EMIT) nh[tid] = 0;
   for (int i = tid; i < SC_WORDS+1; i += SC_THREADS)
     { long long gw = (t0 >> 5) - 1 + i;
       sw[i] = (gw >= 0 && gw < nw) ? w[gw] : 0ull;
@@ -304,29 +302,12 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
     };
 
   int lane = tid & 31, wp = tid >> 5;
-  unsigned pre = 0, tot = 0, inc = cnt;
-  if (!DIGIT || EMIT)
-    {
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1)
-        { unsigned t = __shfl_up_sync(0xffffffffu,inc,o);
-          if (lane >= o) inc += t;
-        }
-      if (lane == 31) wsum[wp] = inc;
-      __syncthreads();
-      for (int i = 0; i < SC_THREADS/32; i++)
-        { if (i < wp) pre += wsum[i];
-          tot += wsum[i];
-        }
-    }
-
   if (EMIT == 0)
-    { if (DIGIT)
-        each_rec([&](const rec128 &r)
-          { const unsigned pf = (unsigned) (r.hi >> 40);
-            atomicAdd(&dcnt[(pf >> dsh) & dmask],1u);
-            atomicAdd(&nh[(pf >> (dsh + dbits)) & 0xff],1u);
-          });
+    { each_rec([&](const rec128 &r)
+        { const unsigned pf = (unsigned) (r.hi >> 40);
+          atomicAdd(&dcnt[(pf >> dsh) & dmask],1u);
+          atomicAdd(&nh[(pf >> (dsh + dbits)) & 0xff],1u);
+        });
       //  10-bit first-5-bases histogram over ALL sampled positions, both strands, as
       //  sample_thread does (GIXmake.c:318-320); decides the .ktab part split (:669-691).
       unsigned m = sel;
@@ -352,84 +333,78 @@ syncmer_body(const u64 *__restrict__ seq, const long long *__restrict__ clen,
         { rdropped = __reduce_add_sync(0xffffffffu,rdropped);
           if (lane == 0 && rdropped) atomicAdd(&buck1024[1024],(unsigned long long) rdropped);
         }
-      if (DIGIT)
-        { for (int i = tid; i < nd; i += SC_THREADS) dmat[(size_t) i*gridDim.x + blockIdx.x] = dcnt[i];
-          if (nh[tid]) atomicAdd(&nhist[tid],(unsigned long long) nh[tid]);      // SC_THREADS == 256
-        }
-      else if (tid == 0) tile_count[blockIdx.x] = tot;
+      for (int i = tid; i < nd; i += SC_THREADS) dmat[(size_t) i*gridDim.x + blockIdx.x] = dcnt[i];
+      if (nh[tid]) atomicAdd(&nhist[tid],(unsigned long long) nh[tid]);          // SC_THREADS == 256
       return;
     }
 
-  if (DIGIT)
-    { extern __shared__ __align__(16) unsigned char sc_smem[];
-      rec128 *stage = reinterpret_cast<rec128 *>(sc_smem);                       // [SC_STAGE]
-      unsigned short *rk = reinterpret_cast<unsigned short *>(stage + SC_STAGE);  // rank inside its digit
-      const int nr = tot <= SC_STAGE ? 1 : SC_ROUNDS;                            // rounds of this tile
-      const int RW = SC_THREADS/32/nr;                                           // warps per round
-      for (int rd = 0; rd < nr; rd++)
-        { const bool act = (wp / RW) == rd;
-          unsigned o = pre + inc - cnt;          // this thread's first slot inside its round
-          for (int i = 0; i < rd*RW; i++) o -= wsum[i];
-          const unsigned o0 = o;
-          if (act)
-            each_rec([&](const rec128 &r)
-              { rk[o++] = (unsigned short) atomicAdd(&dcnt[(unsigned) (r.hi >> (40 + dsh)) & dmask],1u); });
-          __syncthreads();
-          //  exclusive scan of the digit counts (two per thread, SC_THREADS*2 >= 2^SC_DBITS)
-          { unsigned v0 = dcnt[2*tid], v1 = dcnt[2*tid+1], s = v0 + v1, x = s;
+  //  records of the tile before this thread's (pre + inc - cnt), and in all (tot)
+  unsigned pre = 0, tot = 0, inc = cnt;
 #pragma unroll
-            for (int k = 1; k < 32; k <<= 1)
-              { unsigned t = __shfl_up_sync(0xffffffffu,x,k);
-                if (lane >= k) x += t;
-              }
-            if (lane == 31) wsum[wp] = x;
-            __syncthreads();
-            unsigned b = x - s;
-            for (int i = 0; i < wp; i++) b += wsum[i];
-            dloc[2*tid] = b; dloc[2*tid+1] = b + v0;
-          }
-          unsigned rtot = 0;
-          for (int i = 0; i < SC_THREADS/32; i++) rtot += wsum[i];
-          __syncthreads();
-          o = o0;
-          if (act)
-            each_rec([&](const rec128 &r)
-              { const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
-                st_rec(stage + (dloc[d] + rk[o++]),r);
-              });
-          __syncthreads();
-          for (unsigned q = tid; q < rtot; q += SC_THREADS)
-            { rec128 r = ld_rec(stage + q);
-              const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
-              const unsigned s = dbase[d] + (q - dloc[d]);
-              if (s < nlim) st_rec(out + s,r);
-            }
-          __syncthreads();
-          if (rd + 1 < nr)
-            { for (int i = tid; i < nd; i += SC_THREADS) { dbase[i] += dcnt[i]; dcnt[i] = 0; }
-              //  wsum back to the per-warp record counts of the thread prefix
-              unsigned x = inc;
-              if (lane == 31) wsum[wp] = x;
-              __syncthreads();
-            }
-        }
-      return;
+  for (int o = 1; o < 32; o <<= 1)
+    { unsigned t = __shfl_up_sync(0xffffffffu,inc,o);
+      if (lane >= o) inc += t;
+    }
+  if (lane == 31) wsum[wp] = inc;
+  __syncthreads();
+  for (int i = 0; i < SC_THREADS/32; i++)
+    { if (i < wp) pre += wsum[i];
+      tot += wsum[i];
     }
 
-  long long o = (long long) tile_count[blockIdx.x] + pre + inc - cnt;
-  each_rec([&](const rec128 &r) { st_rec(out + o,r); o += 1; });
+  extern __shared__ __align__(16) unsigned char sc_smem[];
+  rec128 *stage = reinterpret_cast<rec128 *>(sc_smem);                       // [SC_STAGE]
+  unsigned short *rk = reinterpret_cast<unsigned short *>(stage + SC_STAGE);  // rank inside its digit
+  const int nr = tot <= SC_STAGE ? 1 : SC_ROUNDS;                            // rounds of this tile
+  const int RW = SC_THREADS/32/nr;                                           // warps per round
+  for (int rd = 0; rd < nr; rd++)
+    { const bool act = (wp / RW) == rd;
+      unsigned o = pre + inc - cnt;          // this thread's first slot inside its round
+      for (int i = 0; i < rd*RW; i++) o -= wsum[i];
+      const unsigned o0 = o;
+      if (act)
+        each_rec([&](const rec128 &r)
+          { rk[o++] = (unsigned short) atomicAdd(&dcnt[(unsigned) (r.hi >> (40 + dsh)) & dmask],1u); });
+      __syncthreads();
+      //  exclusive scan of the digit counts (two per thread, SC_THREADS*2 >= 2^SC_DBITS)
+      { unsigned v0 = dcnt[2*tid], v1 = dcnt[2*tid+1], s = v0 + v1, x = s;
+#pragma unroll
+        for (int k = 1; k < 32; k <<= 1)
+          { unsigned t = __shfl_up_sync(0xffffffffu,x,k);
+            if (lane >= k) x += t;
+          }
+        if (lane == 31) wsum[wp] = x;
+        __syncthreads();
+        unsigned b = x - s;
+        for (int i = 0; i < wp; i++) b += wsum[i];
+        dloc[2*tid] = b; dloc[2*tid+1] = b + v0;
+      }
+      unsigned rtot = 0;
+      for (int i = 0; i < SC_THREADS/32; i++) rtot += wsum[i];
+      __syncthreads();
+      o = o0;
+      if (act)
+        each_rec([&](const rec128 &r)
+          { const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
+            st_rec(stage + (dloc[d] + rk[o++]),r);
+          });
+      __syncthreads();
+      for (unsigned q = tid; q < rtot; q += SC_THREADS)
+        { rec128 r = ld_rec(stage + q);
+          const unsigned d = (unsigned) (r.hi >> (40 + dsh)) & dmask;
+          const unsigned s = dbase[d] + (q - dloc[d]);
+          if (s < nlim) st_rec(out + s,r);
+        }
+      __syncthreads();
+      if (rd + 1 < nr)
+        { for (int i = tid; i < nd; i += SC_THREADS) { dbase[i] += dcnt[i]; dcnt[i] = 0; }
+          //  wsum back to the per-warp record counts of the thread prefix
+          unsigned x = inc;
+          if (lane == 31) wsum[wp] = x;
+          __syncthreads();
+        }
+    }
 }
-
-//  Records packed by tile, for callers that sort them with the partition passes (the sharded path)
-template<int EMIT> __global__ void __launch_bounds__(SC_THREADS)
-syncmer_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
-               const long long *__restrict__ woff, const int *__restrict__ crank,
-               const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
-               unsigned *__restrict__ tile_count,       // EMIT=0: out counts; EMIT=1: in offsets
-               unsigned long long *__restrict__ buck1024,
-               rec128 *__restrict__ out, unsigned plo, unsigned phi_flags)
-{ syncmer_body<EMIT,false>(seq,clen,woff,crank,tile_contig,tile_start,tile_count,buck1024,out,plo,phi_flags,
-                           NULL,0,0,NULL,0); }
 
 //  Records laid out by the first digit of the k-mer partition: [digit][tile] counts, then the staged emit
 __global__ void __launch_bounds__(SC_THREADS)
@@ -438,8 +413,7 @@ syncmer_digit_count_kernel(const u64 *__restrict__ seq, const long long *__restr
                            const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
                            unsigned long long *__restrict__ buck1024, unsigned plo, unsigned phi_flags,
                            unsigned *__restrict__ dmat, int dsh, int dbits, unsigned long long *__restrict__ nhist)
-{ syncmer_body<0,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,buck1024,NULL,plo,phi_flags,
-                       dmat,dsh,dbits,nhist,0); }
+{ syncmer_body<0>(seq,clen,woff,crank,tile_contig,tile_start,buck1024,NULL,plo,phi_flags,dmat,dsh,dbits,nhist,0); }
 
 __global__ void __launch_bounds__(SC_THREADS)
 syncmer_digit_emit_kernel(const u64 *__restrict__ seq, const long long *__restrict__ clen,
@@ -447,8 +421,7 @@ syncmer_digit_emit_kernel(const u64 *__restrict__ seq, const long long *__restri
                           const int *__restrict__ tile_contig, const int *__restrict__ tile_start,
                           rec128 *__restrict__ out, unsigned n, unsigned plo, unsigned phi_flags,
                           unsigned *__restrict__ dbase, int dsh, int dbits)
-{ syncmer_body<1,true>(seq,clen,woff,crank,tile_contig,tile_start,NULL,NULL,out,plo,phi_flags,
-                       dbase,dsh,dbits,NULL,n); }
+{ syncmer_body<1>(seq,clen,woff,crank,tile_contig,tile_start,NULL,out,plo,phi_flags,dbase,dsh,dbits,NULL,n); }
 
 /***********************************************************************************************
  *  Prefix index + LCP over the sorted table (compress_thread, GIXmake.c:1235-1261):
@@ -578,44 +551,7 @@ extern "C" int fgb_stage_genome_device(const void *d_bps, const long long *d_bof
   return FGB_OK;
 }
 
-//  Pass 1 of the scan: per-tile record counts (then scanned in place to offsets), 1024-bin
-//  sampler histogram, and the total number of records in *h_total.
-
-extern "C" int fgb_syncmer_count_device(const void *d_seq, const long long *d_clen,
-                                        const long long *d_woff, const int *d_crank,
-                                        const int *d_tile_contig, const int *d_tile_start, int ntiles,
-                                        unsigned *d_tile_count, unsigned long long *d_buck1024,
-                                        unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                                        unsigned plo, unsigned phi, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  int rc = init_tables();
-  if (rc) return rc;
-  CUDA_TRY(cudaMemsetAsync(d_buck1024,0,1025*8,st));
-  if (ntiles > 0)
-    syncmer_kernel<0><<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
-                                                   d_tile_contig,d_tile_start,d_tile_count,
-                                                   d_buck1024,NULL,plo,phi);
-  fgb_count_launch(1);
-  CUDA_TRY(cudaGetLastError());
-  return fgb_dev_exclusive_scan_u32(d_tile_count,ntiles,d_total,d_tmp,tmp_bytes,st);
-}
-
-extern "C" int fgb_syncmer_emit_device(const void *d_seq, const long long *d_clen,
-                                       const long long *d_woff, const int *d_crank,
-                                       const int *d_tile_contig, const int *d_tile_start, int ntiles,
-                                       unsigned *d_tile_offset, void *d_records, unsigned plo,
-                                       unsigned phi, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  if (ntiles > 0)
-    syncmer_kernel<1><<<ntiles,SC_THREADS,0,st>>>((const u64 *) d_seq,d_clen,d_woff,d_crank,
-                                                   d_tile_contig,d_tile_start,d_tile_offset,
-                                                   NULL,(rec128 *) d_records,plo,phi);
-  fgb_count_launch(1);
-  CUDA_TRY(cudaGetLastError());
-  return FGB_OK;
-}
-
-//  Pass 1 of the digit-partitioned scan: 1024-bin sampler histogram, the records of each tile per digit
+//  Pass 1 of the syncmer scan: 1024-bin sampler histogram, the records of each tile per digit
 //  (bits [dsh, dsh+dbits) of the 12-base prefix) in the [digit][tile] matrix d_dmat, scanned in place to
 //  every (digit, tile)'s first slot, and in d_nhist the histogram of the prefix's 8 bits above the digit;
 //  *d_total = number of records.

@@ -340,6 +340,15 @@ extern "C" long long fgb_sort128_tmp_bytes(long long n)
   return 256*ntiles*8 + (3*256 + 16)*8;
 }
 
+//  The histogram of the first pass's digit, bits [dsh, dsh+8) of the n records in d_a, into T.hist[0].
+static int first_pass_hist(const void *d_a, long long n, int dsh, const sort_tmp &T, cudaStream_t st)
+{ CUDA_TRY(cudaMemsetAsync(T.hist[0],0,256*8,st));
+  int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE), nb = ntiles < 1184 ? ntiles : 1184;
+  sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>((const rec128 *) d_a,n,dsh,T.hist[0]);
+  fgb_count_launch(1);
+  return FGB_OK;
+}
+
 //  One pass: the bin bases of this pass's histogram (cur), the status words zeroed, the Onesweep kernel.
 template <class Key, int IW, int OW>
 static int onesweep_pass(const void *in, void *out, long long n, int dsh, int next_dsh, const sort_tmp &T, int cur,
@@ -380,12 +389,7 @@ extern "C" int fgb_radix_sort_device(void *d_a, void *d_b, long long n, int bit_
   //  second half starts 16-byte aligned, and both may be read one word past their end
   void *half[2] = { d_b, (unsigned char *) d_b + ((8*n + 15) & ~15ll) };
 
-  CUDA_TRY(cudaMemsetAsync(T.hist[0],0,256*8,st));
-  { int ntiles = (int) ((n + SORT_TILE - 1) / SORT_TILE), nb = ntiles < 1184 ? ntiles : 1184;
-    sort_ghist_kernel<<<nb,SORT_THREADS,0,st>>>((const rec128 *) d_a,n,bit_lo,T.hist[0]);
-    fgb_count_launch(1);
-  }
-  int rc = FGB_OK;
+  int rc = first_pass_hist(d_a,n,bit_lo,T,st);
   for (int p = 0; p < npass && rc == FGB_OK; p++)
     { const int b = bit_lo + 8*p, nd = (p + 1 < npass) ? b + 8 : -1, cur = p & 1;
       if (!words)
@@ -408,10 +412,6 @@ extern "C" int fgb_radix_sort_device(void *d_a, void *d_b, long long n, int bit_
   return FGB_OK;
 }
 
-extern "C" int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                                       void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
-{ return fgb_radix_sort_device(d_a,d_b,n,bit_lo,bit_hi,0,d_tmp,tmp_bytes,result_in_b,NULL,stream); }
-
 extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
                                   void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
 { if (byte_lo < 0 || byte_hi > 16 || byte_lo > byte_hi) return FGB_ERR_ARG;
@@ -425,9 +425,8 @@ extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo
  *  Ten full Onesweep passes move 10 x 32 bytes per record through HBM.  Instead:
  *    1. the records are laid out by prefix bin: bin p at [bins[p], bins[p+1]), in any order inside
  *       the bin.  Onesweep partition passes on the prefix bits above the bin shift give that
- *       layout (fgb_kmer_sort_range_device).  A table built from a genome gets the first of them from
- *       the scan itself: its emit pass stores the records in runs by the lowest digit
- *       (fgb_kmer_sort_digit_device);
+ *       layout (fgb_kmer_sort_device).  A table built from a genome gets its lowest digit from the
+ *       scan itself: the scan's emit pass stores the records in runs by that digit;
  *    2. consecutive bins are packed into groups of at most BK_CAP records and BK_SPAN bins; one
  *       CTA per group pulls the group into shared memory with one TMA bulk copy, sorts it there
  *       (kmer_bucket_sort_kernel) and writes it back once;
@@ -611,6 +610,17 @@ extern "C" int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi)
   return sh;
 }
 
+//  The k-mer partition a table's syncmer scan starts: the partition sorts bits [fsh, 24) of the 12-base
+//  prefix, fsh chosen for an upper bound nmax of n, by a first digit of dbits bits that the scan's emit pass
+//  lays out and 8-bit Onesweep passes above it.  The first digit takes what is left over by as few passes
+//  as leave it at most 9 bits.
+extern "C" void fgb_kmer_first_digit(long long nmax, unsigned plo, unsigned phi, int *fsh, int *dbits)
+{ *fsh = fgb_kmer_bin_shift(nmax,plo,phi);
+  int bits = 24 - *fsh, passes = (bits - 9 + 7) / 8;
+  if (passes < 1) passes = 1;
+  *dbits = bits - 8*passes;
+}
+
 //  Sorts the records of src laid out by bin (bin p at [bins[p], bins[p+1]), any order inside a bin;
 //  bins on the host, nbins+1 entries) into dst.  Synchronises the stream.
 static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins, long long nbins, int sh,
@@ -680,68 +690,42 @@ static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins
   return FGB_OK;
 }
 
-//  d_a: n records in any order; d_b: scratch of the same size.  Sorted table lands in d_a or d_b
-//  (*result_in_b).  d_tmp as for fgb_sort128_device.  Partition passes (8-bit digits over the bins'
-//  bits, the top 24 - sh bits of the k-mer: one more pass when that exceeds two bytes) lay the records
-//  out by bin; synchronises the stream once more than kmer_sort_binned (the bin boundaries come to the
-//  host to pack the groups).
-extern "C" int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                                          void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
-{ cudaStream_t st = (cudaStream_t) stream;
-  *result_in_b = 0;
-  if (n <= 1) return FGB_OK;
-  if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
-  if (phi <= plo || phi > (1u << 24)) return FGB_ERR_ARG;
-  const int sh = fgb_kmer_bin_shift(n,plo,phi);
-  const int binshift = 40 + sh;
-  const unsigned long long base = (unsigned long long) plo >> sh;
-  const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
-  int inb = 0;
-  int rc = fgb_sort128_bits_device(d_a,d_b,n,64 + binshift,128,d_tmp,tmp_bytes,&inb,st);
-  if (rc) return rc;
-  rec128 *src = (rec128 *) (inb ? d_b : d_a), *dst = (rec128 *) (inb ? d_a : d_b);
-
-  dblock<unsigned> d_bins;
-  CUDA_TRY(d_bins.alloc((size_t) (nbins+1),st));
-  { int nb = (int) ((n + 1 + 255) / 256);
-    kmer_bins_kernel<<<nb,256,0,st>>>(src,n,binshift,base,d_bins,nbins);
-    fgb_count_launch(1);
-  }
-  std::vector<unsigned> bins((size_t) nbins + 1);
-  CUDA_TRY(cudaMemcpyAsync(bins.data(),d_bins,sizeof(unsigned)*(size_t) (nbins+1),cudaMemcpyDeviceToHost,st));
-  CUDA_TRY(cudaStreamSynchronize(st));
-  d_bins.reset();                                       // before the bucket sort allocates its own
-  rc = kmer_sort_binned(src,dst,bins.data(),nbins,sh,plo,st);
-  if (rc) return rc;
-  *result_in_b = inb ^ 1;
-  return FGB_OK;
-}
-
-//  d_a: n records the syncmer scan laid out by the first digit of the partition, bits [fsh, fsh+dbits) of
-//  the 12-base prefix; d_nhist: the histogram of the 8 prefix bits above it.  Onesweep passes on the rest
-//  of the prefix above fsh lay the records out by fine bin, (prefix24 >> fsh) - (plo >> fsh), with fsh
-//  chosen for an upper bound of n.  A bin of the rule for n is a run of whole fine bins, so the records then
-//  go straight to the bucket sort.  Sorted table lands in d_a or d_b (*result_in_b).
-extern "C" int fgb_kmer_sort_digit_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
-                                          const u64 *d_nhist, void *d_tmp, long long tmp_bytes, int *result_in_b,
-                                          void *stream)
+//  Sorts the n records in d_a whose 12-base prefixes lie in [plo,phi); d_b: scratch of the same size, d_tmp as
+//  for fgb_sort128_device.  The sorted table lands in d_a or d_b (*result_in_b).  Onesweep passes on the prefix
+//  above bit fsh lay the records out by fine bin, (prefix24 >> fsh) - (plo >> fsh); a bin of the rule for n is
+//  a run of whole fine bins, so the records then go straight to the bucket sort.
+//    dbits > 0: the syncmer scan laid d_a out by the first digit of the partition, bits [fsh, fsh+dbits) of
+//      the prefix (fgb_kmer_first_digit, fsh chosen for an upper bound of n), and d_hist holds the histogram
+//      of the 8 prefix bits above it.
+//    dbits = 0: the records are in any order; fsh is the bin shift for n, and the first pass counts its own
+//      histogram.
+//  Synchronises the stream (the fine-bin bounds come to the host to pack the bucket-sort groups).
+extern "C" int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
+                                    const u64 *d_hist, void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   *result_in_b = 0;
   if (n <= 1) return FGB_OK;
   if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
   if (phi <= plo || phi > (1u << 24) || tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
   const int sh = fgb_kmer_bin_shift(n,plo,phi);
+  if (dbits == 0) fsh = sh;
   if (sh < fsh) return FGB_ERR_ARG;
   const sort_tmp T(d_tmp,n);
-  CUDA_TRY(cudaMemcpyAsync(T.hist[0],d_nhist,256*8,cudaMemcpyDeviceToDevice,st));
-  rec128 *src = (rec128 *) d_a, *dst = (rec128 *) d_b;
   const int b0 = 64 + 40 + fsh + dbits, npass = (128 - b0 + 7) / 8;
+  if (dbits == 0)
+    { int rc = first_pass_hist(d_a,n,b0,T,st);
+      if (rc) return rc;
+    }
+  else
+    CUDA_TRY(cudaMemcpyAsync(T.hist[0],d_hist,256*8,cudaMemcpyDeviceToDevice,st));
+  rec128 *src = (rec128 *) d_a, *dst = (rec128 *) d_b;
   for (int p = 0; p < npass; p++)
     { const int b = b0 + 8*p, nd = (p + 1 < npass) ? b + 8 : -1;
       int rc = onesweep_pass<rec128,16,16>(src,dst,n,b,nd,T,p & 1,st);
       if (rc) return rc;
       std::swap(src,dst);
     }
+  CUDA_TRY(cudaGetLastError());
 
   const unsigned long long base = (unsigned long long) plo >> sh, fbase = (unsigned long long) plo >> fsh;
   const long long nf = (long long) (((unsigned long long) (phi - 1) >> fsh) - fbase) + 1;

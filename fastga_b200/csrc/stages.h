@@ -21,30 +21,18 @@ long long fgb_sort128_tmp_bytes(long long n);
 int fgb_radix_sort_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi, int narrow,
                           void *d_tmp, long long tmp_bytes, int *result_in_b, unsigned long long **d_hiflag,
                           void *stream);
-int fgb_sort128_bits_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi,
-                            void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
 int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
                        void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
 int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
-int fgb_kmer_sort_range_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi,
-                               void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
-int fgb_kmer_sort_digit_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
-                               const unsigned long long *d_nhist, void *d_tmp, long long tmp_bytes, int *result_in_b,
-                               void *stream);
+void fgb_kmer_first_digit(long long nmax, unsigned plo, unsigned phi, int *fsh, int *dbits);
+int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
+                         const unsigned long long *d_hist, void *d_tmp, long long tmp_bytes, int *result_in_b,
+                         void *stream);
 
 // ---- gix.cu: genome staging, syncmer scan, table index and .ktab entries ----
 int fgb_stage_genome_device(const void *d_bps, const long long *d_boff, const long long *d_clen,
                             const long long *d_woff, int ncontig, long long total_words,
                             void *d_seq, void *d_rseq, void *stream);
-int fgb_syncmer_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                             const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                             int ntiles, unsigned *d_tile_count, unsigned long long *d_buck1024,
-                             unsigned long long *d_total, void *d_tmp, long long tmp_bytes,
-                             unsigned plo, unsigned phi, void *stream);
-int fgb_syncmer_emit_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
-                            const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
-                            int ntiles, unsigned *d_tile_offset, void *d_records, unsigned plo,
-                            unsigned phi, void *stream);
 int fgb_syncmer_digit_count_device(const void *d_seq, const long long *d_clen, const long long *d_woff,
                                    const int *d_crank, const int *d_tile_contig, const int *d_tile_start,
                                    int ntiles, unsigned long long *d_buck1024, unsigned *d_dmat, int dsh, int dbits,

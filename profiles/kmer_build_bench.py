@@ -1,14 +1,15 @@
 #!/usr/bin/env python
-"""kmer_build_bench.py -- the bench pair's two k-mer tables built by the default path ("scatter": the scan
-stores its records in runs by the first digit of the k-mer partition) against the Onesweep partition
-passes alone (FGB_KSORT_PARTITION=1), alternating the two paths.
+"""kmer_build_bench.py -- the bench pair's two k-mer tables built from one syncmer scan along the two routes
+into the k-mer sort, alternating them: "scatter", the default, where the sort starts from the scan's
+layout (the records in runs by the first digit of the k-mer partition), against "partition"
+(FGB_KSORT_PARTITION=1), where the sort ignores that layout and runs every partition pass in Onesweep.
 
 The tables are the ones the fused path builds: genome A forward-only, genome B both strands.  Times are
 the library's CUDA-event times (stage_ms.scan_ms + stage_ms.ksort_ms of bench.py), summed over the two
 tables.  A separate profiled build of each path splits the time by kernel (torch.profiler, CUDA activity).
 HBM bytes per record, counting 32-byte sectors (reading the staged genome is < 1 byte per record):
   scatter:    16 (emit in runs) + 32 (one partition pass) + 16 (bin bounds) + 32 (bucket sort) = 96
-  partition:  16 (emit) + 16 (histogram) + 2 x 32 (partition passes) + 16 (bin bounds) + 32 = 144
+  partition:  16 (emit in runs) + 16 (histogram) + 2 x 32 (partition passes) + 16 (bin bounds) + 32 = 144
 Prints one JSON line.
 """
 import argparse
