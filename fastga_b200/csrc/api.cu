@@ -26,6 +26,45 @@ struct stage_timer
     }
 };
 
+//  A stage timer that does not wait: its events are read at the next host wait (fgb_stream_wait), or when the
+//  timings are fetched.
+struct lazy_event { cudaEvent_t a, b; float *dst; };
+static std::vector<lazy_event> g_lazy;
+static long long g_waits;
+
+struct lazy_timer
+{ lazy_event e; cudaStream_t st;
+  lazy_timer(float *d, cudaStream_t s) : st(s)
+    { e.dst = d; cudaEventCreate(&e.a); cudaEventCreate(&e.b); cudaEventRecord(e.a,st); }
+  ~lazy_timer() { cudaEventRecord(e.b,st); g_lazy.push_back(e); }
+};
+
+//  adds the elapsed time of every timer whose end has been reached (wait = true: of every timer)
+static void lazy_flush(bool wait)
+{ size_t k = 0;
+  for (const lazy_event &e : g_lazy)
+    { if (wait) cudaEventSynchronize(e.b);
+      else if (cudaEventQuery(e.b) != cudaSuccess) { g_lazy[k++] = e; continue; }
+      float ms = 0;
+      cudaEventElapsedTime(&ms,e.a,e.b);
+      *e.dst += ms;
+      cudaEventDestroy(e.a); cudaEventDestroy(e.b);
+    }
+  cudaGetLastError();
+  g_lazy.resize(k);
+}
+
+//  The host waits of the k-mer table builds: each one counted (fgb_host_waits; the fused path reports the waits of
+//  its table builds as fgb_run_stats.gix_waits).
+cudaError_t fgb_stream_wait(cudaStream_t st)
+{ g_waits += 1;
+  cudaError_t e = cudaStreamSynchronize(st);
+  lazy_flush(false);
+  return e;
+}
+
+extern "C" long long fgb_host_waits() { return g_waits; }
+
 void fgb_timing_add(int which, float ms)
 { if (which == 0) g_timings.triples_ms += ms;
   else if (which == 1) { g_timings.extend_ms += ms; g_timings.extend_launches += 1; }
@@ -110,8 +149,8 @@ extern "C" long long fgb_device_live_bytes()
   return s;
 }
 
-extern "C" void fgb_timings_reset() { memset(&g_timings,0,sizeof(g_timings)); }
-extern "C" void fgb_timings_get(fgb_timings *out) { *out = g_timings; }
+extern "C" void fgb_timings_reset() { lazy_flush(true); memset(&g_timings,0,sizeof(g_timings)); }
+extern "C" void fgb_timings_get(fgb_timings *out) { lazy_flush(true); *out = g_timings; }
 
 /***********************************************************************************************
  *  Genome: the GDB as the path sees it (GDB.h:28-34 GDB_CONTIG {clen, boff} + the .bps image)
@@ -224,112 +263,181 @@ struct scan_layout
   dblock<unsigned long long> hist;
 };
 
-//  K1/K2: syncmer scan + record build of the contigs selected by `mask` (NULL: all) into a fresh device buffer
-//  of *n records (room for n+1).  *nrev = reverse entries left out (fwd-only).  The count pass counts the
-//  records per tile and first digit of the k-mer partition, at the resolution the k-mer sort would pick for
-//  an upper bound of n (two records per scanned position), and the emit pass stores them in runs by that
-//  digit; lay describes the result.
-static int gix_scan(const fgb_genome *g, const unsigned char *mask, unsigned plo, unsigned phi_flags,
-                    dblock<rec128> &d_recs, long long *n_out, long long *nrev, unsigned long long *buck1024,
-                    scan_layout &lay, cudaStream_t st)
-{ int T = fgb_sc_tile();
+//  Words a table build reads back from the device, in pinned memory so that their copies do not wait: the count
+//  pass's record total, the reverse entries it left out, the sampler histogram and the k-mer sort plan's counters.
+struct gix_words
+{ u64 total, buck[1024], rdropped;                    // buck and rdropped: the count pass's 1025 words
+  unsigned plan[4];
+};
+
+//  One table build.  The host waits only where it needs a count from the device: once after the count pass (the
+//  record total sizes the record block and the sort) and once at the end (the plan's count of bins too large for
+//  the bucket sort; there are none in the normal case).  Every block the queued work reads, on the host or the
+//  device, lives here until the wait after it.  The builds of a pair run each step on both tables before the
+//  wait, so a pair waits twice.
+struct gix_job
+{ const fgb_genome *g = nullptr;
+  unsigned plo = 0, phi = 0, flags = 0;
+  bool index = true;
+  std::unique_ptr<fgb_gix> x;
+  scan_layout lay;
   std::vector<int> tc, ts;
+  int ntiles = 0;
+  dblock<int> d_tc, d_ts; dblock<unsigned> d_cnt;
+  dblock<u64> d_buck, d_total; dblock<unsigned char> d_tmp;
+  dblock<rec128> d_a, d_b; dblock<unsigned char> d_stmp, d_plan;
+  long long n = 0;
+  int inb = 0;
+  gix_words *hw = nullptr;
+};
+
+//  pinned words for the (at most two) builds a thread has in flight, allocated once
+static int pinned_words(gix_job &J, int k)
+{ static thread_local gix_words *w = nullptr;
+  if (w == nullptr) CUDA_TRY(cudaHostAlloc((void **) &w,2*sizeof(gix_words),cudaHostAllocDefault));
+  J.hw = w + k;
+  return FGB_OK;
+}
+
+static int gix_job_init(gix_job &J, const fgb_genome *g, unsigned plo, unsigned phi_flags, bool index, int k)
+{ J.g = g; J.plo = plo; J.phi = phi_flags & ~GIX_FWD_ONLY; J.flags = phi_flags; J.index = index;
+  J.x.reset(new fgb_gix());
+  gix_bytes(g,J.x.get());
+  J.x->ncontig = g->ncontig;
+  J.x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
+  return pinned_words(J,k);
+}
+
+//  K1, count pass: syncmer records of the contigs selected by `mask` (NULL: all) counted per tile and first digit
+//  of the k-mer partition, at the resolution the k-mer sort would pick for an upper bound of n (two records per
+//  scanned position); the total, the reverse entries left out (fwd-only) and the sampler histogram go to J.hw.
+static int gix_count(gix_job &J, const unsigned char *mask, cudaStream_t st)
+{ const fgb_genome *g = J.g;
+  int T = fgb_sc_tile();
   long long npos = 0;
   for (int c = 0; c < g->ncontig; c++)
     if (g->clen[c] >= 12 && g->boff[c] >= 0 && (mask == NULL || mask[c]))
       { npos += g->clen[c] - 11;
         for (long long t0 = 0; t0 + 12 <= g->clen[c]; t0 += T)
-          { tc.push_back(c); ts.push_back((int) t0); }
+          { J.tc.push_back(c); J.ts.push_back((int) t0); }
       }
-  int ntiles = (int) tc.size();
-  dblock<int> d_tc, d_ts; dblock<unsigned> d_cnt;
-  dblock<u64> d_buck, d_total; dblock<unsigned char> d_tmp;
-  int rc;
-  u64 total = 0, rdropped = 0;
-  const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
-  fgb_kmer_first_digit(2*npos,plo,phi > plo ? phi : plo + 1,&lay.fsh,&lay.dbits);    // an empty range still gets one bin
-  const long long ncnt = (long long) ntiles << lay.dbits;
+  J.ntiles = (int) J.tc.size();
+  scan_layout &lay = J.lay;
+  fgb_kmer_first_digit(2*npos,J.plo,J.phi > J.plo ? J.phi : J.plo + 1,&lay.fsh,&lay.dbits);    // an empty range still gets one bin
+  const long long ncnt = (long long) J.ntiles << lay.dbits;
   const long long tmpb = fgb_dev_scan_tmp_bytes(ncnt);
   CUDA_TRY(lay.hist.alloc(256,st));
-  CUDA_TRY(d_tc.alloc(ntiles+1,st));
-  CUDA_TRY(d_ts.alloc(ntiles+1,st));
-  CUDA_TRY(d_cnt.alloc(ncnt+1,st));
-  CUDA_TRY(d_buck.alloc(1025,st));
-  CUDA_TRY(d_total.alloc(1,st));
-  CUDA_TRY(d_tmp.alloc(tmpb,st));
-  CUDA_TRY(cudaMemcpyAsync(d_tc,tc.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
-  CUDA_TRY(cudaMemcpyAsync(d_ts,ts.data(),sizeof(int)*ntiles,cudaMemcpyHostToDevice,st));
-  { stage_timer t(&g_timings.scan_ms,st);
-    rc = fgb_syncmer_digit_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_buck,d_cnt,
-                                        lay.fsh,lay.dbits,lay.hist,d_total,d_tmp,tmpb,plo,phi_flags,st);
-    if (rc) return rc;
-    CUDA_TRY(cudaMemcpyAsync(&total,d_total,8,cudaMemcpyDeviceToHost,st));
-    if (buck1024) CUDA_TRY(cudaMemcpyAsync(buck1024,d_buck,8*1024,cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaMemcpyAsync(&rdropped,d_buck + 1024,8,cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-  }
-  if (total >= 0xfffffff0ull) return FGB_ERR_LIMIT;
-  dblock<rec128> d_a;
-  CUDA_TRY(d_a.alloc(total+1,st));
-  { stage_timer t(&g_timings.scan_ms,st);
-    rc = fgb_syncmer_digit_emit_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,d_tc,d_ts,ntiles,d_cnt,lay.fsh,
-                                       lay.dbits,(long long) total,d_a,plo,phi_flags,st);
-  }
+  CUDA_TRY(J.d_tc.alloc(J.ntiles+1,st));
+  CUDA_TRY(J.d_ts.alloc(J.ntiles+1,st));
+  CUDA_TRY(J.d_cnt.alloc(ncnt+1,st));
+  CUDA_TRY(J.d_buck.alloc(1025,st));
+  CUDA_TRY(J.d_total.alloc(1,st));
+  CUDA_TRY(J.d_tmp.alloc(tmpb,st));
+  CUDA_TRY(cudaMemcpyAsync(J.d_tc,J.tc.data(),sizeof(int)*J.ntiles,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(J.d_ts,J.ts.data(),sizeof(int)*J.ntiles,cudaMemcpyHostToDevice,st));
+  lazy_timer t(&g_timings.scan_ms,st);
+  int rc = fgb_syncmer_digit_count_device(g->d_seq,g->d_clen,g->d_woff,g->d_crank,J.d_tc,J.d_ts,J.ntiles,J.d_buck,
+                                          J.d_cnt,lay.fsh,lay.dbits,lay.hist,J.d_total,J.d_tmp,tmpb,J.plo,J.flags,st);
   if (rc) return rc;
-  CUDA_TRY(cudaStreamSynchronize(st));                   // tc/ts must outlive the copies
-  d_recs = std::move(d_a); *n_out = (long long) total; *nrev = (long long) rdropped;
+  CUDA_TRY(cudaMemcpyAsync(&J.hw->total,J.d_total,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(J.hw->buck,J.d_buck,8*1025,cudaMemcpyDeviceToHost,st));
   return FGB_OK;
 }
 
-//  K3/K4: sorts the records in d_a (consumed: it ends up inside the handle or is released) whose
-//  12-base prefixes lie in [plo,phi), laid out as lay says, builds the prefix index and the LCP bytes.
-static int gix_finish(fgb_gix *x, dblock<rec128> d_a, long long n, unsigned plo, unsigned phi, const scan_layout &lay,
-                      cudaStream_t st, bool index = true)
-{ dblock<rec128> d_b; dblock<unsigned char> d_stmp;
-  long long stmpb = fgb_sort128_tmp_bytes(n);
-  int rc, inb = 0;
+//  K2, emit pass (after the wait for the total): the J.n records into J.d_a (room for n+1), in runs by the first
+//  digit of the partition.
+static int gix_emit(gix_job &J, cudaStream_t st)
+{ if (J.hw->total >= 0xfffffff0ull) return FGB_ERR_LIMIT;
+  J.n = (long long) J.hw->total;
+  CUDA_TRY(J.d_a.alloc(J.n+1,st));
+  lazy_timer t(&g_timings.scan_ms,st);
+  return fgb_syncmer_digit_emit_device(J.g->d_seq,J.g->d_clen,J.g->d_woff,J.g->d_crank,J.d_tc,J.d_ts,J.ntiles,
+                                       J.d_cnt,J.lay.fsh,J.lay.dbits,J.n,J.d_a,J.plo,J.flags,st);
+}
+
+//  K3/K4: sorts the J.n records in J.d_a whose 12-base prefixes lie in [plo,phi), laid out as lay says, and builds
+//  the prefix index and the LCP bytes; the plan's counters go to J.hw.
+static int gix_sort(gix_job &J, const scan_layout &lay, cudaStream_t st)
+{ fgb_gix *x = J.x.get();
+  const long long n = J.n, stmpb = fgb_sort128_tmp_bytes(n), planb = fgb_kmer_plan_bytes(n,J.plo,J.phi,lay.fsh,lay.dbits);
+  int rc;
   x->n = n;
-  CUDA_TRY(d_b.alloc(n+1,st));
-  CUDA_TRY(d_stmp.alloc(stmpb,st));
-  if (index)
+  CUDA_TRY(J.d_b.alloc(n+1,st));
+  CUDA_TRY(J.d_stmp.alloc(stmpb,st));
+  CUDA_TRY(J.d_plan.alloc(planb,st));
+  if (J.index)
     { CUDA_TRY(x->d_pstart.alloc((1<<24)+1+8,st));
       CUDA_TRY(x->d_adj.alloc((size_t) n + 32,st));
     }
-  { stage_timer t(&g_timings.ksort_ms,st);
-    rc = fgb_kmer_sort_device(d_a,d_b,n,plo,phi,lay.fsh,lay.dbits,lay.hist,d_stmp,stmpb,&inb,st);
+  { lazy_timer t(&g_timings.ksort_ms,st);
+    rc = fgb_kmer_sort_device(J.d_a,J.d_b,n,J.plo,J.phi,lay.fsh,lay.dbits,lay.hist,J.d_stmp,stmpb,J.d_plan,&J.inb,st);
   }
   if (rc) return rc;
-  x->d_tab = std::move(inb ? d_b : d_a);                  // the other side goes back as the call returns
-  if (index)
-    { stage_timer t(&g_timings.index_ms,st);
-      rc = fgb_kix_index_device(x->d_tab,n,x->d_pstart,x->d_adj,st);
+  CUDA_TRY(cudaMemcpyAsync(J.hw->plan,J.d_plan,16,cudaMemcpyDeviceToHost,st));
+  if (J.index)
+    { lazy_timer t(&g_timings.index_ms,st);
+      rc = fgb_kix_index_device(J.inb ? J.d_b : J.d_a,n,x->d_pstart,x->d_adj,st);
     }
-  if (rc) return rc;
-  CUDA_TRY(cudaStreamSynchronize(st));
+  return rc;
+}
+
+//  After the last wait: the bins too large for the bucket sort, if the plan found any (then the index is built
+//  again over the finished table), and the handle.
+static int gix_done(gix_job &J, cudaStream_t st, fgb_gix **out)
+{ fgb_gix *x = J.x.get();
+  dblock<rec128> &tab = J.inb ? J.d_b : J.d_a;
+  int rc;
+  if (J.hw->plan[1] > 0)
+    { { lazy_timer t(&g_timings.ksort_ms,st);
+        rc = fgb_kmer_sort_oversized(J.inb ? J.d_a : J.d_b,tab,J.n,J.d_plan,J.hw->plan[1],J.hw->plan[2],st);
+      }
+      if (rc) return rc;
+      if (J.index)
+        { lazy_timer t(&g_timings.index_ms,st);
+          if ((rc = fgb_kix_index_device(tab,J.n,x->d_pstart,x->d_adj,st))) return rc;
+        }
+    }
+  x->d_tab = std::move(tab);
+  memcpy(x->buck1024,J.hw->buck,8*1024);
+  x->n_both = J.n + (long long) J.hw->rdropped;
+  *out = J.x.release();
   return FGB_OK;
 }
 
-//  index = false: the table only, without prefix index and LCP bytes (the T1 side of a merge reads neither)
+//  FGB_KSORT_PARTITION=1: the sort ignores the scan's layout and runs every partition pass in Onesweep, a
+//  second, independent route to the same table (both can be compared in one process)
+static const scan_layout &sort_layout(const gix_job &J)
+{ static const scan_layout none;
+  const char *part_env = getenv("FGB_KSORT_PARTITION");
+  return (part_env != NULL && atoi(part_env) != 0) ? none : J.lay;
+}
+
+//  The tables of njob genomes, each step queued for all of them before the wait that follows it: two host waits
+//  for the lot.  Only a table with bins too large for the bucket sort waits more, and then its index is queued
+//  again after the last wait.
+static int gix_build_jobs(gix_job *J, int njob, fgb_gix **out, cudaStream_t st)
+{ int rc;
+  for (int k = 0; k < njob; k++)
+    if ((rc = gix_count(J[k],NULL,st))) return rc;
+  CUDA_TRY(fgb_stream_wait(st));
+  for (int k = 0; k < njob; k++)
+    if ((rc = gix_emit(J[k],st)) || (rc = gix_sort(J[k],sort_layout(J[k]),st))) return rc;
+  CUDA_TRY(fgb_stream_wait(st));
+  for (int k = 0; k < njob; k++)
+    if ((rc = gix_done(J[k],st,out + k))) return rc;
+  return FGB_OK;
+}
+
+//  index = false: the table only, without prefix index and LCP bytes (the T1 side of a merge reads neither).
+//  Returns when the table is complete.
 static int gix_build_range(const fgb_genome *g, unsigned plo, unsigned phi_flags, bool index, fgb_gix **out,
                            void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
-  const unsigned phi = phi_flags & ~GIX_FWD_ONLY;
-  std::unique_ptr<fgb_gix> x(new fgb_gix());
-  gix_bytes(g,x.get());
-  x->ncontig = g->ncontig;
-  x->fwd_only = (phi_flags & GIX_FWD_ONLY) ? 1 : 0;
-  dblock<rec128> d_a; long long n = 0, nrev = 0;
-  scan_layout lay;
-  int rc = gix_scan(g,NULL,plo,phi_flags,d_a,&n,&nrev,x->buck1024,lay,st);
+  gix_job J;
+  int rc = gix_job_init(J,g,plo,phi_flags,index,0);
+  if (!rc) rc = gix_build_jobs(&J,1,out,st);
   if (rc) return rc;
-  x->n_both = n + nrev;
-  //  FGB_KSORT_PARTITION=1: the sort ignores the scan's layout and runs every partition pass in Onesweep, a
-  //  second, independent route to the same table (both can be compared in one process)
-  const char *part_env = getenv("FGB_KSORT_PARTITION");
-  const bool ignore_layout = part_env != NULL && atoi(part_env) != 0;
-  const scan_layout none;
-  if ((rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,ignore_layout ? none : lay,st,index))) return rc;
-  *out = x.release();
+  if (J.hw->plan[1] != 0) CUDA_TRY(fgb_stream_wait(st));        // the index built again after the oversized bins
   return FGB_OK;
 }
 
@@ -360,11 +468,16 @@ extern "C" int fgb_gix_build_range(const fgb_genome *g, unsigned plo, unsigned p
 //  dropped: the caller regroups the records by owner and each owner sorts its share from any order.
 extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only,
                               void **d_recs, long long *n, void *stream)
-{ dblock<rec128> d; long long nrev = 0;
-  scan_layout lay;
-  int rc = gix_scan(g,mask,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),d,n,&nrev,NULL,lay,(cudaStream_t) stream);
+{ cudaStream_t st = (cudaStream_t) stream;
+  gix_job J;
+  int rc = gix_job_init(J,g,0u,(1u << 24) | (fwd_only ? GIX_FWD_ONLY : 0u),false,0);
+  if (!rc) rc = gix_count(J,mask,st);
   if (rc) return rc;
-  *d_recs = d.release();
+  CUDA_TRY(fgb_stream_wait(st));
+  if ((rc = gix_emit(J,st))) return rc;
+  CUDA_TRY(fgb_stream_wait(st));                        // the records are the caller's from here on
+  *n = J.n;
+  *d_recs = J.d_a.release();
   return FGB_OK;
 }
 
@@ -374,15 +487,22 @@ extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned pl
                                     int post_bytes, int cont_bytes, int ncontig, fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   if (n < 0 || n >= 0xfffffff0ll || plo >= phi || phi > (1u << 24)) return FGB_ERR_ARG;
-  std::unique_ptr<fgb_gix> x(new fgb_gix());
-  x->n_both = n; x->post_bytes = post_bytes; x->cont_bytes = cont_bytes; x->ncontig = ncontig;
-  x->fwd_only = fwd_only ? 1 : 0;
-  dblock<rec128> d_a;
-  CUDA_TRY(d_a.alloc(n+1,st));
-  if (n > 0) CUDA_TRY(cudaMemcpyAsync(d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
-  int rc = gix_finish(x.get(),std::move(d_a),n,plo,phi,scan_layout(),st);
+  gix_job J;
+  J.plo = plo; J.phi = phi;
+  J.x.reset(new fgb_gix());
+  J.x->post_bytes = post_bytes; J.x->cont_bytes = cont_bytes; J.x->ncontig = ncontig;
+  J.x->fwd_only = fwd_only ? 1 : 0;
+  int rc = pinned_words(J,0);
   if (rc) return rc;
-  *out = x.release();
+  J.hw->rdropped = 0;
+  memset(J.hw->buck,0,8*1024);
+  J.n = n;
+  CUDA_TRY(J.d_a.alloc(n+1,st));
+  if (n > 0) CUDA_TRY(cudaMemcpyAsync(J.d_a,d_recs,sizeof(rec128)*n,cudaMemcpyDeviceToDevice,st));
+  if ((rc = gix_sort(J,scan_layout(),st))) return rc;
+  CUDA_TRY(fgb_stream_wait(st));
+  if ((rc = gix_done(J,st,out))) return rc;
+  if (J.hw->plan[1] != 0) CUDA_TRY(fgb_stream_wait(st));        // the index built again after the oversized bins
   return FGB_OK;
 }
 
@@ -688,7 +808,7 @@ struct fgb_run_stats
 { long long nkmers1, nkmers2, nseeds, sumlen, nhits, nla, nwaves, ncells, nraw, h2d_bytes, d2h_bytes,
             nseg, nwork, warp_cycles, wave_cycles, extract_cycles,
             us_gix, us_seeds, us_extend, us_filter, nkmers1_fwd,
-            slow_cycles, slow_waves, paired_waves, pairings; };
+            slow_cycles, slow_waves, paired_waves, pairings, gix_waits; };
 
 //  The whole path on staged genomes: k-mer tables -> adaptamer merge -> seed sort -> extension -> filter.
 //  self: SELF mode (`FastGA A`, B == A): one both-strand table merged against itself by the self block
@@ -701,14 +821,17 @@ static int align_pipeline(const fgb_genome *A, const fgb_genome *B, bool self, c
   int rc;
   long long t0 = now_us(), t1, t2, t3, t4;
   { std::unique_ptr<fgb_gix> x1, x2;
-    fgb_gix *p = NULL;
-    //  pair: the adaptamer side forward strand only, and only the table (the merge reads B's index)
-    if ((rc = gix_build_range(A,0u,(1u << 24) | (self ? 0u : GIX_FWD_ONLY),self,&p,st))) return rc;
-    x1.reset(p);
-    if (!self)
-      { if ((rc = gix_build_range(B,0u,1u << 24,true,&p,st))) return rc;
-        x2.reset(p);
-      }
+    fgb_gix *p[2] = { NULL, NULL };
+    const long long w0 = g_waits;
+    { gix_job J[2];
+      //  pair: the adaptamer side forward strand only, and only the table (the merge reads B's index)
+      rc = gix_job_init(J[0],A,0u,(1u << 24) | (self ? 0u : GIX_FWD_ONLY),self,0);
+      if (!rc && !self) rc = gix_job_init(J[1],B,0u,1u << 24,true,1);
+      if (!rc) rc = gix_build_jobs(J,self ? 1 : 2,p,st);
+      x1.reset(p[0]); x2.reset(p[1]);
+      if (rc) return rc;
+    }
+    s.gix_waits = g_waits - w0;
     const fgb_gix *xb = self ? x1.get() : x2.get();
     t1 = now_us();
     s.nkmers1 = x1->n_both; s.nkmers2 = xb->n;

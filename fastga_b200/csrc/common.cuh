@@ -63,6 +63,7 @@ long long fgb_dev_scan_tmp_bytes(long long n);
 
 void fgb_timing_add(int which, float ms);     // 0 triples 1 extend 2 d2h 3 merge kernel
 void fgb_count_launch(int n);                 // kernels launched (bench.py gpu_launches)
+cudaError_t fgb_stream_wait(cudaStream_t st); // cudaStreamSynchronize, counted (fgb_host_waits)
 
 //  stream-ordered device allocation from a retained pool (no cudaMalloc/cudaFree stalls per step)
 cudaError_t fgb_dmalloc(void **p, size_t bytes, cudaStream_t st);

@@ -21,6 +21,8 @@
 #include <stdlib.h>
 #include <utility>
 #include <vector>
+#include <algorithm>
+#include <stdint.h>
 
 #define SORT_THREADS 512
 #ifndef SORT_ITEMS
@@ -427,11 +429,12 @@ extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo
  *       the bin.  Onesweep partition passes on the prefix bits above the bin shift give that
  *       layout (fgb_kmer_sort_device).  A table built from a genome gets its lowest digit from the
  *       scan itself: the scan's emit pass stores the records in runs by that digit;
- *    2. consecutive bins are packed into groups of at most BK_CAP records and BK_SPAN bins; one
- *       CTA per group pulls the group into shared memory with one TMA bulk copy, sorts it there
- *       (kmer_bucket_sort_kernel) and writes it back once;
+ *    2. the bins' starts are found on the device and consecutive bins packed there into groups of at
+ *       most BK_CAP records and BK_SPAN bins (kmer_fine_bounds_kernel, kmer_plan_kernel); a CTA pulls a
+ *       group into shared memory with one TMA bulk copy, sorts it there (kmer_bucket_sort_kernel) and
+ *       writes it back once;
  *    3. bins larger than BK_CAP (repeats) are compacted, sorted with the generic Onesweep sort and
- *       copied back.
+ *       copied back (fgb_kmer_sort_oversized, once the host has read the plan's count of them).
  *  Every record is unique (contig, strand and post differ) and steps 2 and 3 order a bin by the whole
  *  128-bit value, so the order records arrive in inside a bin does not change the table.
  *  HBM traffic per record after the layout: 32 bytes (10 x 32 for a full LSD sort).
@@ -446,26 +449,86 @@ extern "C" int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo
 #define BK_NSUB    (BK_SPAN << BK_SUBBITS)
 #define BK_MAXSUB  32                    // a sub-bin longer than this sends the group down the LSD path
 
-//  bin_start[p] = first record whose bin ((hi >> binshift) - base) is >= p, p in [0,nbins]
-__global__ void kmer_bins_kernel(const rec128 *__restrict__ tab, long long n, int binshift, unsigned long long base,
-                                 unsigned *__restrict__ bin_start, long long nbins)
-{ long long i = (long long) blockIdx.x * blockDim.x + threadIdx.x;
-  if (i > n) return;
-  long long lo = (i == 0) ? -1 : (long long) ((tab[i-1].hi >> binshift) - base);
-  long long hi = (i == n) ? nbins : (long long) ((tab[i].hi >> binshift) - base);
-  if (hi > nbins) hi = nbins;
-  for (long long p = lo+1; p <= hi; p++) bin_start[p] = (unsigned) i;
+//  fstart[p] = first record whose fine bin ((hi >> binshift) - base) is >= p, p in [0,nf]: a lower-bound search
+//  over the partitioned records, whose fine bins never decrease.  About log2(n) 8-byte probes per fine bin, most of
+//  them shared with the neighbouring threads' searches, instead of a pass over all 16 n bytes.
+__global__ void kmer_fine_bounds_kernel(const rec128 *__restrict__ tab, long long n, int binshift, unsigned long long base,
+                                        unsigned *__restrict__ fstart, long long nf)
+{ long long p = (long long) blockIdx.x * blockDim.x + threadIdx.x;
+  if (p > nf) return;
+  long long lo = 0, hi = n;
+  while (lo < hi)
+    { long long md = (lo + hi) >> 1;
+      if ((tab[md].hi >> binshift) - base < (unsigned long long) p) lo = md + 1; else hi = md;
+    }
+  fstart[p] = (unsigned) lo;
 }
 
-//  One CTA sorts one group (<= BK_CAP records of <= BK_SPAN consecutive bins) by the full 128-bit
-//  value.  Fast path: a counting split on the next 10 key bits (shared-memory atomics) leaves
-//  sub-bins of one or two records, and every record finds its place by comparing itself with its
-//  sub-bin.  A group with a crowded sub-bin (repeats) runs sixteen LSD byte passes instead.
+//  The plan of a k-mer sort (fgb_kmer_plan_bytes): counters, the oversized bins, the fine-bin starts and the groups.
+#define KP_NGROUPS 0                      // counter words: groups, oversized bins, records in oversized bins
+#define KP_NOVER   1
+#define KP_OTOTAL  2
+struct kmer_plan
+{ unsigned *ctr, *fstart;
+  uint2 *over;                            // oversized bins: start, length (in no particular order)
+  uint4 *groups;                          // start, count, hi >> binshift of the first bin (in no particular order)
+  kmer_plan(void *d, long long n, long long nf)
+    { long long ocap = n / BK_CAP + 1;
+      ctr = (unsigned *) d;
+      over = (uint2 *) (ctr + 4);
+      fstart = (unsigned *) (over + ocap);
+      groups = (uint4 *) (((uintptr_t) (fstart + nf + 1) + 15) & ~(uintptr_t) 15);
+    }
+};
+
+//  One thread per window of BK_SPAN consecutive bins packs the window's bins greedily into groups: whole bins, at
+//  most BK_CAP records (a window never exceeds BK_SPAN bins).  Bins larger than BK_CAP go to the oversized list.
+//  Bin p starts at the first of its fine bins, fstart[((base + p) << dsh) - fbase].
+__global__ void kmer_plan_kernel(long long nf, long long nbins, int dsh, unsigned long long base,
+                                 unsigned long long fbase, kmer_plan P)
+{ long long p0 = ((long long) blockIdx.x * blockDim.x + threadIdx.x) * BK_SPAN;
+  if (p0 >= nbins) return;
+  const int nb = nbins - p0 < BK_SPAN ? (int) (nbins - p0) : BK_SPAN;
+  unsigned b[BK_SPAN+1];
+#pragma unroll
+  for (int k = 0; k <= BK_SPAN; k++)
+    if (k <= nb)
+      { long long f = (long long) ((base + p0 + k) << dsh) - (long long) fbase;
+        b[k] = P.fstart[f < 0 ? 0 : (f > nf ? nf : f)];
+      }
+  uint4 g[BK_SPAN];
+  int ng = 0;
+  unsigned gs = 0, gc = 0, gp = 0;
+#pragma unroll
+  for (int k = 0; k < BK_SPAN; k++)
+    { if (k >= nb) break;
+      unsigned len = b[k+1] - b[k];
+      if (len == 0) continue;
+      if (len > BK_CAP)
+        { if (gc) { g[ng++] = make_uint4(gs,gc,(unsigned) (base + p0) + gp,0); gc = 0; }
+          P.over[atomicAdd(&P.ctr[KP_NOVER],1u)] = make_uint2(b[k],len);
+          atomicAdd(&P.ctr[KP_OTOTAL],len);
+          continue;
+        }
+      if (gc + len > BK_CAP) { g[ng++] = make_uint4(gs,gc,(unsigned) (base + p0) + gp,0); gc = 0; }
+      if (gc == 0) { gs = b[k]; gp = k; }
+      gc += len;
+    }
+  if (gc) g[ng++] = make_uint4(gs,gc,(unsigned) (base + p0) + gp,0);
+  if (ng == 0) return;
+  unsigned o = atomicAdd(&P.ctr[KP_NGROUPS],(unsigned) ng);
+  for (int k = 0; k < ng; k++) P.groups[o+k] = g[k];
+}
+
+//  Each CTA sorts groups blockIdx.x, blockIdx.x + gridDim.x, ... of the *ngroups groups (<= BK_CAP records of <=
+//  BK_SPAN consecutive bins each) by the full 128-bit value.  Fast path: a counting split on the next 10 key bits
+//  (shared-memory atomics) leaves sub-bins of one or two records, and every record finds its place by comparing
+//  itself with its sub-bin.  A group with a crowded sub-bin (repeats) runs sixteen LSD byte passes instead.
 
 __global__ void __launch_bounds__(BK_THREADS,2)
 kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
                         const uint4 *__restrict__ groups /* start, count, hi >> binshift of its first bin */,
-                        int binshift)
+                        const unsigned *__restrict__ ngroups, int binshift)
 { extern __shared__ __align__(16) unsigned char smem_raw[];
   rec128   *tile   = reinterpret_cast<rec128 *>(smem_raw);
   unsigned *cnt    = reinterpret_cast<unsigned *>(tile + BK_CAP);        // [BK_NSUB+1]; LSD path: wcount[BK_WARPS][256]
@@ -474,109 +537,118 @@ kmer_bucket_sort_kernel(const rec128 *__restrict__ in, rec128 *__restrict__ out,
   __shared__ __align__(8) unsigned long long tbar;
 
   const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const uint4 g = groups[blockIdx.x];
-  const int count = (int) g.y;
-  if (tid == 0)
-    { mbar_init(&tbar,1);
-      tma_load_1d(tile,in + g.x,(unsigned) count * 16u,&tbar);
-    }
-  for (int i = tid; i <= BK_NSUB; i += BK_THREADS) cnt[i] = 0;
-  __syncthreads();
-  mbar_wait(&tbar,0);
-
-  rec128   r[BK_ITEMS];
-  unsigned sub[BK_ITEMS], off[BK_ITEMS];
-  const int base = w*(32*BK_ITEMS);
-  const unsigned b0 = g.z;                     // not tile[0]'s bin: a bin's records come in any order
-  const int subshift = binshift - BK_SUBBITS;
-#pragma unroll
-  for (int it = 0; it < BK_ITEMS; it++)
-    { int idx = base + it*32 + lane;
-      if (idx < count)
-        { r[it] = ld_rec(tile + idx);
-          sub[it] = ((((unsigned) (r[it].hi >> binshift)) - b0) << BK_SUBBITS) | ((unsigned) (r[it].hi >> subshift) & ((1u << BK_SUBBITS)-1));
-          off[it] = atomicAdd(&cnt[sub[it]],1u);
-        }
-    }
-  __syncthreads();
-  //  exclusive scan of the sub-bin counts (8 per thread), crowded sub-bin detection
-  bool big = false;
-  { unsigned v[8], sum = 0;
-#pragma unroll
-    for (int i = 0; i < 8; i++) { v[i] = cnt[8*tid+i]; big |= (v[i] > BK_MAXSUB); sum += v[i]; }
-    unsigned inc = warp_incl_scan(sum,lane);
-    if (lane == 31) wtot[w] = inc;
+  const unsigned ng = *ngroups;
+  if (blockIdx.x >= ng) return;
+  if (tid == 0) mbar_init(&tbar,1);
+  unsigned phase = 0;
+  for (unsigned gi = blockIdx.x; gi < ng; gi += gridDim.x, phase ^= 1)
+    {
+    const uint4 g = groups[gi];
+    const int count = (int) g.y;
+    if (tid == 0)
+      { asm volatile("fence.proxy.async.shared::cta;" ::: "memory");     // the last group's stores before the copy
+        tma_load_1d(tile,in + g.x,(unsigned) count * 16u,&tbar);
+      }
+    for (int i = tid; i <= BK_NSUB; i += BK_THREADS) cnt[i] = 0;
     __syncthreads();
-    unsigned pre = inc - sum;
-    for (int i = 0; i < w; i++) pre += wtot[i];
-#pragma unroll
-    for (int i = 0; i < 8; i++) { cnt[8*tid+i] = pre; pre += v[i]; }
-    if (tid == BK_THREADS-1) cnt[BK_NSUB] = pre;
-  }
-  big = __syncthreads_or(big);
+    mbar_wait(&tbar,phase);
 
-  if (!big)
-    {
+    rec128   r[BK_ITEMS];
+    unsigned sub[BK_ITEMS], off[BK_ITEMS];
+    const int base = w*(32*BK_ITEMS);
+    const unsigned b0 = g.z;                     // not tile[0]'s bin: a bin's records come in any order
+    const int subshift = binshift - BK_SUBBITS;
 #pragma unroll
-      for (int it = 0; it < BK_ITEMS; it++)
-        { int idx = base + it*32 + lane;
-          if (idx < count) st_rec(tile + (cnt[sub[it]] + off[it]),r[it]);
-        }
+    for (int it = 0; it < BK_ITEMS; it++)
+      { int idx = base + it*32 + lane;
+        if (idx < count)
+          { r[it] = ld_rec(tile + idx);
+            sub[it] = ((((unsigned) (r[it].hi >> binshift)) - b0) << BK_SUBBITS) | ((unsigned) (r[it].hi >> subshift) & ((1u << BK_SUBBITS)-1));
+            off[it] = atomicAdd(&cnt[sub[it]],1u);
+          }
+      }
+    __syncthreads();
+    //  exclusive scan of the sub-bin counts (8 per thread), crowded sub-bin detection
+    bool big = false;
+    { unsigned v[8], sum = 0;
+#pragma unroll
+      for (int i = 0; i < 8; i++) { v[i] = cnt[8*tid+i]; big |= (v[i] > BK_MAXSUB); sum += v[i]; }
+      unsigned inc = warp_incl_scan(sum,lane);
+      if (lane == 31) wtot[w] = inc;
       __syncthreads();
-      for (int p = tid; p < count; p += BK_THREADS)
-        { rec128 R = ld_rec(tile + p);
-          unsigned sb = ((((unsigned) (R.hi >> binshift)) - b0) << BK_SUBBITS) | ((unsigned) (R.hi >> subshift) & ((1u << BK_SUBBITS)-1));
-          int s = (int) cnt[sb], e = (int) cnt[sb+1], rank = 0;
-          for (int q = s; q < e; q++)
-            { rec128 Q = ld_rec(tile + q);
-              bool less = (Q.hi < R.hi) || (Q.hi == R.hi && (Q.lo < R.lo || (Q.lo == R.lo && q < p)));
-              rank += less;
-            }
-          st_rec(out + (g.x + s + rank),R);
-        }
-      return;
+      unsigned pre = inc - sum;
+      for (int i = 0; i < w; i++) pre += wtot[i];
+#pragma unroll
+      for (int i = 0; i < 8; i++) { cnt[8*tid+i] = pre; pre += v[i]; }
+      if (tid == BK_THREADS-1) cnt[BK_NSUB] = pre;
     }
+    big = __syncthreads_or(big);
 
-  //  LSD path: all sixteen bytes, records still in registers in load order
-  unsigned *wcount = cnt;
-  unsigned *myc = wcount + w*256;
-  unsigned rank[BK_ITEMS];
-  __syncthreads();
+    if (!big)
+      {
 #pragma unroll
-  for (int i = 0; i < 8; i++) myc[i*32 + lane] = 0;
-  __syncwarp();
-  for (int byte = 0; byte < 16; byte++)
-    {
+        for (int it = 0; it < BK_ITEMS; it++)
+          { int idx = base + it*32 + lane;
+            if (idx < count) st_rec(tile + (cnt[sub[it]] + off[it]),r[it]);
+          }
+        __syncthreads();
+        for (int p = tid; p < count; p += BK_THREADS)
+          { rec128 R = ld_rec(tile + p);
+            unsigned sb = ((((unsigned) (R.hi >> binshift)) - b0) << BK_SUBBITS) | ((unsigned) (R.hi >> subshift) & ((1u << BK_SUBBITS)-1));
+            int s = (int) cnt[sb], e = (int) cnt[sb+1], rank = 0;
+            for (int q = s; q < e; q++)
+              { rec128 Q = ld_rec(tile + q);
+                bool less = (Q.hi < R.hi) || (Q.hi == R.hi && (Q.lo < R.lo || (Q.lo == R.lo && q < p)));
+                rank += less;
+              }
+            st_rec(out + (g.x + s + rank),R);
+          }
+        __syncthreads();
+        continue;
+      }
+
+    //  LSD path: all sixteen bytes, records still in registers in load order
+    unsigned *wcount = cnt;
+    unsigned *myc = wcount + w*256;
+    unsigned rank[BK_ITEMS];
+    __syncthreads();
 #pragma unroll
-      for (int it = 0; it < BK_ITEMS; it++)
-        { int idx = base + it*32 + lane;
-          bool valid = idx < count;
-          rank[it] = warp_rank(myc,valid ? rec_byte(r[it],byte) : 0,valid);
-        }
-      digit_offsets(wcount,bexcl,wtot,[](unsigned) {});
+    for (int i = 0; i < 8; i++) myc[i*32 + lane] = 0;
+    __syncwarp();
+    for (int byte = 0; byte < 16; byte++)
+      {
 #pragma unroll
-      for (int it = 0; it < BK_ITEMS; it++)
-        { int idx = base + it*32 + lane;
-          if (idx < count)
-            { unsigned d = rec_byte(r[it],byte);
-              st_rec(tile + (bexcl[d] + myc[d] + rank[it]),r[it]);
-            }
-        }
-      __syncthreads();
-      if (byte + 1 < 16)
-        {
+        for (int it = 0; it < BK_ITEMS; it++)
+          { int idx = base + it*32 + lane;
+            bool valid = idx < count;
+            rank[it] = warp_rank(myc,valid ? rec_byte(r[it],byte) : 0,valid);
+          }
+        digit_offsets(wcount,bexcl,wtot,[](unsigned) {});
 #pragma unroll
-          for (int it = 0; it < BK_ITEMS; it++)
-            { int idx = base + it*32 + lane;
-              if (idx < count) r[it] = ld_rec(tile + idx);
-            }
+        for (int it = 0; it < BK_ITEMS; it++)
+          { int idx = base + it*32 + lane;
+            if (idx < count)
+              { unsigned d = rec_byte(r[it],byte);
+                st_rec(tile + (bexcl[d] + myc[d] + rank[it]),r[it]);
+              }
+          }
+        __syncthreads();
+        if (byte + 1 < 16)
+          {
 #pragma unroll
-          for (int i = 0; i < 8; i++) myc[i*32 + lane] = 0;
-          __syncwarp();
-        }
+            for (int it = 0; it < BK_ITEMS; it++)
+              { int idx = base + it*32 + lane;
+                if (idx < count) r[it] = ld_rec(tile + idx);
+              }
+#pragma unroll
+            for (int i = 0; i < 8; i++) myc[i*32 + lane] = 0;
+            __syncwarp();
+          }
+      }
+    for (int p = tid; p < count; p += BK_THREADS)
+      st_rec(out + (g.x + p),ld_rec(tile + p));
+    __syncthreads();
     }
-  for (int p = tid; p < count; p += BK_THREADS)
-    st_rec(out + (g.x + p),ld_rec(tile + p));
 }
 
 //  copies record segments: src[sfrom[k] .. +len[k]) -> dst[dfrom[k] ..); pre[] = prefix sums of len
@@ -621,94 +693,48 @@ extern "C" void fgb_kmer_first_digit(long long nmax, unsigned plo, unsigned phi,
   *dbits = bits - 8*passes;
 }
 
-//  Sorts the records of src laid out by bin (bin p at [bins[p], bins[p+1]), any order inside a bin;
-//  bins on the host, nbins+1 entries) into dst.  Synchronises the stream.
-static int kmer_sort_binned(const rec128 *src, rec128 *dst, const unsigned *bins, long long nbins, int sh,
-                            unsigned plo, cudaStream_t st)
-{ const int binshift = 40 + sh;                          // prefix24 = hi >> 40
-  const unsigned base = plo >> sh;
-  int rc = FGB_OK;
-  static bool attr_set = false;
-  if (!attr_set)
-    { CUDA_TRY(cudaFuncSetAttribute(kmer_bucket_sort_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                    (int) BUCKET_SMEM));
-      attr_set = true;
-    }
+//  The bins of the rule for n (fgb_kmer_bin_shift) and the fine bins the partition passes lay out
+static void kmer_bins_of(long long n, unsigned plo, unsigned phi, int *fsh, int dbits, int *sh, long long *nf,
+                         long long *nbins)
+{ *sh = fgb_kmer_bin_shift(n,plo,phi);
+  if (dbits == 0) *fsh = *sh;
+  *nf = (long long) (((unsigned long long) (phi - 1) >> *fsh) - ((unsigned long long) plo >> *fsh)) + 1;
+  *nbins = (long long) (((unsigned long long) (phi - 1) >> *sh) - ((unsigned long long) plo >> *sh)) + 1;
+}
 
-  std::vector<uint4> groups;
-  std::vector<unsigned> ofrom, opre;                    // oversized bins: start, prefix of lengths
-  unsigned ototal = 0;
-  { unsigned gs = bins[0], gc = 0; long long gp = 0;           // group start record, size, first bin
-    for (long long p = 0; p < nbins; p++)
-      { unsigned len = bins[p+1] - bins[p];
-        if (len == 0) continue;
-        if (len > BK_CAP)
-          { if (gc) { groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0)); gc = 0; }
-            ofrom.push_back(bins[p]); opre.push_back(ototal); ototal += len;
-            continue;
-          }
-        if (gc != 0 && (gc + len > BK_CAP || p - gp >= BK_SPAN))
-          { groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0)); gc = 0; }
-        if (gc == 0) { gs = bins[p]; gp = p; }
-        gc += len;
-      }
-    if (gc) groups.push_back(make_uint4(gs,gc,base + (unsigned) gp,0));
-  }
-
-  dblock<uint4> d_groups;
-  if (!groups.empty())
-    { CUDA_TRY(d_groups.alloc(groups.size(),st));
-      CUDA_TRY(cudaMemcpyAsync(d_groups,groups.data(),sizeof(uint4)*groups.size(),cudaMemcpyHostToDevice,st));
-      kmer_bucket_sort_kernel<<<(unsigned) groups.size(),BK_THREADS,BUCKET_SMEM,st>>>(src,dst,d_groups,binshift);
-      fgb_count_launch(1);
-      CUDA_TRY(cudaGetLastError());
-    }
-  if (ototal > 0)
-    { int nseg = (int) ofrom.size();
-      opre.push_back(ototal);
-      std::vector<unsigned> cfrom(opre.begin(),opre.end()-1);            // position in the compact array
-      dblock<rec128> d_c1, d_c2; dblock<unsigned char> d_ctmp; dblock<unsigned> d_seg;
-      long long ctb = fgb_sort128_tmp_bytes(ototal);
-      CUDA_TRY(d_c1.alloc((size_t) ototal+1,st));
-      CUDA_TRY(d_c2.alloc((size_t) ototal+1,st));
-      CUDA_TRY(d_ctmp.alloc(ctb,st));
-      CUDA_TRY(d_seg.alloc(3*(size_t) nseg+1,st));
-      CUDA_TRY(cudaMemcpyAsync(d_seg,ofrom.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
-      CUDA_TRY(cudaMemcpyAsync(d_seg+nseg,cfrom.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
-      CUDA_TRY(cudaMemcpyAsync(d_seg+2*nseg,opre.data(),sizeof(unsigned)*(nseg+1),cudaMemcpyHostToDevice,st));
-      int nb = (int) ((ototal + 255) / 256); if (nb > 4736) nb = 4736;
-      kmer_copy_segments_kernel<<<nb,256,0,st>>>(src,d_c1,d_seg,d_seg+nseg,d_seg+2*nseg,nseg,ototal);
-      int cinb = 0;
-      rc = fgb_sort128_device(d_c1,d_c2,ototal,0,16,d_ctmp,ctb,&cinb,st);
-      if (rc) return rc;
-      kmer_copy_segments_kernel<<<nb,256,0,st>>>(cinb ? d_c2 : d_c1,dst,d_seg+nseg,d_seg,d_seg+2*nseg,nseg,ototal);
-      fgb_count_launch(2);
-      CUDA_TRY(cudaGetLastError());
-      CUDA_TRY(cudaStreamSynchronize(st));                // the staging vectors above must outlive the copies
-    }
-  CUDA_TRY(cudaStreamSynchronize(st));
-  return FGB_OK;
+//  Bytes of the plan block of fgb_kmer_sort_device
+extern "C" long long fgb_kmer_plan_bytes(long long n, unsigned plo, unsigned phi, int fsh, int dbits)
+{ int sh;
+  long long nf = 1, nbins = 1;
+  if (phi > plo) kmer_bins_of(n,plo,phi,&fsh,dbits,&sh,&nf,&nbins);
+  return 16 + 8*(n / BK_CAP + 1) + 4*(nf + 1) + 16 + 16*nbins;
 }
 
 //  Sorts the n records in d_a whose 12-base prefixes lie in [plo,phi); d_b: scratch of the same size, d_tmp as
-//  for fgb_sort128_device.  The sorted table lands in d_a or d_b (*result_in_b).  Onesweep passes on the prefix
-//  above bit fsh lay the records out by fine bin, (prefix24 >> fsh) - (plo >> fsh); a bin of the rule for n is
-//  a run of whole fine bins, so the records then go straight to the bucket sort.
+//  for fgb_sort128_device, d_plan a block of fgb_kmer_plan_bytes.  The sorted table lands in d_a or d_b
+//  (*result_in_b).  Onesweep passes on the prefix above bit fsh lay the records out by fine bin,
+//  (prefix24 >> fsh) - (plo >> fsh); a bin of the rule for n is a run of whole fine bins, so the records then go
+//  straight to the bucket sort.
 //    dbits > 0: the syncmer scan laid d_a out by the first digit of the partition, bits [fsh, fsh+dbits) of
 //      the prefix (fgb_kmer_first_digit, fsh chosen for an upper bound of n), and d_hist holds the histogram
 //      of the 8 prefix bits above it.
 //    dbits = 0: the records are in any order; fsh is the bin shift for n, and the first pass counts its own
 //      histogram.
-//  Synchronises the stream (the fine-bin bounds come to the host to pack the bucket-sort groups).
+//  Does not synchronise: the fine-bin starts and the bucket-sort groups are planned on the device.  The bins
+//  larger than BK_CAP are left out of the result: the plan's first four words (KP_*) count them, and when
+//  there are any, fgb_kmer_sort_oversized puts them in place.
 extern "C" int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
-                                    const u64 *d_hist, void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream)
+                                    const u64 *d_hist, void *d_tmp, long long tmp_bytes, void *d_plan,
+                                    int *result_in_b, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;
   *result_in_b = 0;
+  CUDA_TRY(cudaMemsetAsync(d_plan,0,16,st));
   if (n <= 1) return FGB_OK;
   if (n >= 0xffffffffll) return FGB_ERR_LIMIT;
   if (phi <= plo || phi > (1u << 24) || tmp_bytes < fgb_sort128_tmp_bytes(n)) return FGB_ERR_ARG;
-  const int sh = fgb_kmer_bin_shift(n,plo,phi);
-  if (dbits == 0) fsh = sh;
+  int sh;
+  long long nf, nbins;
+  kmer_bins_of(n,plo,phi,&fsh,dbits,&sh,&nf,&nbins);
   if (sh < fsh) return FGB_ERR_ARG;
   const sort_tmp T(d_tmp,n);
   const int b0 = 64 + 40 + fsh + dbits, npass = (128 - b0 + 7) / 8;
@@ -725,26 +751,66 @@ extern "C" int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, unsigned 
       if (rc) return rc;
       std::swap(src,dst);
     }
-  CUDA_TRY(cudaGetLastError());
 
-  const unsigned long long base = (unsigned long long) plo >> sh, fbase = (unsigned long long) plo >> fsh;
-  const long long nf = (long long) (((unsigned long long) (phi - 1) >> fsh) - fbase) + 1;
-  const long long nbins = (long long) (((unsigned long long) (phi - 1) >> sh) - base) + 1;
-  std::vector<unsigned> fstart((size_t) nf + 1), bins((size_t) nbins + 1);
-  { dblock<unsigned> d_fstart;
-    CUDA_TRY(d_fstart.alloc((size_t) (nf+1),st));
-    kmer_bins_kernel<<<(int) ((n + 1 + 255) / 256),256,0,st>>>(src,n,40 + fsh,fbase,d_fstart,nf);
-    fgb_count_launch(1);
-    CUDA_TRY(cudaMemcpyAsync(fstart.data(),d_fstart,sizeof(unsigned)*(size_t) (nf+1),cudaMemcpyDeviceToHost,st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-  }
-  for (long long p = 0; p <= nbins; p++)
-    { long long f = (long long) ((base + p) << (sh - fsh)) - (long long) fbase;     // first fine bin of bin p
-      bins[p] = fstart[f < 0 ? 0 : (f > nf ? nf : f)];
+  static int grid = 0;
+  if (grid == 0)
+    { int dev, nsm, per;
+      CUDA_TRY(cudaFuncSetAttribute(kmer_bucket_sort_kernel,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) BUCKET_SMEM));
+      CUDA_TRY(cudaGetDevice(&dev));
+      CUDA_TRY(cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev));
+      CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per,kmer_bucket_sort_kernel,BK_THREADS,BUCKET_SMEM));
+      grid = nsm * (per > 0 ? per : 1);
     }
-  int rc = kmer_sort_binned(src,dst,bins.data(),nbins,sh,plo,st);
-  if (rc) return rc;
+  const kmer_plan P(d_plan,n,nf);
+  const unsigned long long base = (unsigned long long) plo >> sh, fbase = (unsigned long long) plo >> fsh;
+  const long long nwin = (nbins + BK_SPAN - 1) / BK_SPAN;
+  kmer_fine_bounds_kernel<<<(int) ((nf + 1 + 255) / 256),256,0,st>>>(src,n,40 + fsh,fbase,P.fstart,nf);
+  kmer_plan_kernel<<<(int) ((nwin + 255) / 256),256,0,st>>>(nf,nbins,sh - fsh,base,fbase,P);
+  kmer_bucket_sort_kernel<<<(unsigned) (nbins < grid ? nbins : grid),BK_THREADS,BUCKET_SMEM,st>>>(src,dst,P.groups,
+                                                                                                  P.ctr + KP_NGROUPS,
+                                                                                                  40 + sh);
+  fgb_count_launch(3);
+  CUDA_TRY(cudaGetLastError());
   *result_in_b = (dst == (rec128 *) d_b);
+  return FGB_OK;
+}
+
+//  The bins the plan of fgb_kmer_sort_device found larger than BK_CAP (nover bins, ototal records: the plan's
+//  KP_NOVER and KP_OTOTAL words): compacted, sorted with the Onesweep sort and copied from the partitioned
+//  records (src, the side the result did not land in) into place in the table (dst).  Synchronises the stream.
+extern "C" int fgb_kmer_sort_oversized(const void *src, void *dst, long long n, const void *d_plan, unsigned nover,
+                                       unsigned ototal, void *stream)
+{ cudaStream_t st = (cudaStream_t) stream;
+  if (nover == 0) return FGB_OK;
+  const kmer_plan P(const_cast<void *>(d_plan),n,0);
+  std::vector<uint2> over(nover);
+  CUDA_TRY(cudaMemcpyAsync(over.data(),P.over,sizeof(uint2)*nover,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(fgb_stream_wait(st));
+  std::sort(over.begin(),over.end(),[](const uint2 &x, const uint2 &y) { return x.x < y.x; });
+  //  in bin order, the sorted compact array holds bin k's records at opre[k]
+  const int nseg = (int) nover;
+  std::vector<unsigned> ofrom(nseg), opre(nseg + 1);
+  opre[0] = 0;
+  for (int k = 0; k < nseg; k++) { ofrom[k] = over[k].x; opre[k+1] = opre[k] + over[k].y; }
+  if (opre[nseg] != ototal) return FGB_ERR_ARG;
+  dblock<rec128> d_c1, d_c2; dblock<unsigned char> d_ctmp; dblock<unsigned> d_seg;
+  long long ctb = fgb_sort128_tmp_bytes(ototal);
+  CUDA_TRY(d_c1.alloc((size_t) ototal+1,st));
+  CUDA_TRY(d_c2.alloc((size_t) ototal+1,st));
+  CUDA_TRY(d_ctmp.alloc(ctb,st));
+  CUDA_TRY(d_seg.alloc(3*(size_t) nseg+1,st));
+  CUDA_TRY(cudaMemcpyAsync(d_seg,ofrom.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(d_seg+nseg,opre.data(),sizeof(unsigned)*nseg,cudaMemcpyHostToDevice,st));
+  CUDA_TRY(cudaMemcpyAsync(d_seg+2*nseg,opre.data(),sizeof(unsigned)*(nseg+1),cudaMemcpyHostToDevice,st));
+  int nb = (int) ((ototal + 255) / 256); if (nb > 4736) nb = 4736;
+  kmer_copy_segments_kernel<<<nb,256,0,st>>>((const rec128 *) src,d_c1,d_seg,d_seg+nseg,d_seg+2*nseg,nseg,ototal);
+  int cinb = 0;
+  int rc = fgb_sort128_device(d_c1,d_c2,ototal,0,16,d_ctmp,ctb,&cinb,st);
+  if (rc) return rc;
+  kmer_copy_segments_kernel<<<nb,256,0,st>>>(cinb ? d_c2 : d_c1,(rec128 *) dst,d_seg+nseg,d_seg,d_seg+2*nseg,nseg,ototal);
+  fgb_count_launch(2);
+  CUDA_TRY(cudaGetLastError());
+  CUDA_TRY(fgb_stream_wait(st));                      // the staging vectors above must outlive the copies
   return FGB_OK;
 }
 

@@ -25,9 +25,12 @@ int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_
                        void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
 int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
 void fgb_kmer_first_digit(long long nmax, unsigned plo, unsigned phi, int *fsh, int *dbits);
+long long fgb_kmer_plan_bytes(long long n, unsigned plo, unsigned phi, int fsh, int dbits);
 int fgb_kmer_sort_device(void *d_a, void *d_b, long long n, unsigned plo, unsigned phi, int fsh, int dbits,
-                         const unsigned long long *d_hist, void *d_tmp, long long tmp_bytes, int *result_in_b,
-                         void *stream);
+                         const unsigned long long *d_hist, void *d_tmp, long long tmp_bytes, void *d_plan,
+                         int *result_in_b, void *stream);
+int fgb_kmer_sort_oversized(const void *src, void *dst, long long n, const void *d_plan, unsigned nover,
+                            unsigned ototal, void *stream);
 
 // ---- gix.cu: genome staging, syncmer scan, table index and .ktab entries ----
 int fgb_stage_genome_device(const void *d_bps, const long long *d_boff, const long long *d_clen,

@@ -38,6 +38,13 @@ def timings_reset():
     load_library().fgb_timings_reset()
 
 
+def host_waits():
+    """host waits of the k-mer table builds so far (a counter)"""
+    L = load_library()
+    L.fgb_host_waits.restype = c_ll
+    return L.fgb_host_waits()
+
+
 def timings_get():
     t = Timings()
     load_library().fgb_timings_get(C.byref(t))
@@ -431,7 +438,8 @@ class RunStats(C.Structure):
     _fields_ = [(n, c_ll) for n in ("nkmers1", "nkmers2", "nseeds", "sumlen", "nhits", "nla", "nwaves",
                                     "ncells", "nraw", "h2d_bytes", "d2h_bytes", "nseg", "nwork", "warp_cycles",
                                     "wave_cycles", "extract_cycles", "us_gix", "us_seeds", "us_extend", "us_filter",
-                                    "nkmers1_fwd", "slow_cycles", "slow_waves", "paired_waves", "pairings")]
+                                    "nkmers1_fwd", "slow_cycles", "slow_waves", "paired_waves", "pairings",
+                                    "gix_waits")]
 
     def asdict(self):
         return {n: getattr(self, n) for n, _ in self._fields_}

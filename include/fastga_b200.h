@@ -46,7 +46,8 @@ typedef struct
             us_gix, us_seeds, us_extend, us_filter,      /* host wall microseconds per phase */
             nkmers1_fwd,                                 /* entries of table 1 the merge reads (forward strand; SELF: all) */
             slow_cycles, slow_waves,                     /* the extension warp that finished last: its cycles and waves */
-            paired_waves, pairings;                      /* waves run by front/back warp pairs, passes handed to a pair */
+            paired_waves, pairings,                      /* waves run by front/back warp pairs, passes handed to a pair */
+            gix_waits;                                   /* host waits of the two table builds, scan to merge launch */
 } fgb_run_stats;
 
 typedef struct
@@ -261,6 +262,7 @@ void fgb_release_cache(void);      /* return cached device blocks to the driver 
 long long fgb_device_live_bytes(void);   /* bytes of device blocks handed out and not yet released */
 void fgb_timings_reset(void);
 void fgb_timings_get(fgb_timings *out);
+long long fgb_host_waits(void);          /* host waits of the k-mer table builds so far (a counter) */
 
 #ifdef __cplusplus
 }
