@@ -178,7 +178,17 @@ typedef struct { uint8_t plen; uint8_t comp; uint16_t icont, jcont; uint32_t ipo
 
 /* Walks T1 and the per-panel slice of T2 with the reference's (plen, vlcp[], rend, eorun) state
    machine.  Emits (plen, T1 entry, T2 entry) for forward T1 entries whose block is < freq.
-   out may be NULL (count only).  Returns the number of seeds; *sumlen gets the sum of plen. */
+   out may be NULL (count only).  Returns the number of seeds; *sumlen gets the sum of plen.
+   orc_merge_counters() reports how often the last call took each branch of the walk (MB_*). */
+
+enum { MB_PANEL, MB_NLCP_GT, MB_NLCP_EQ_EORUN, MB_NLCP_EQ, MB_NLCP_LT, MB_REND_SKIP, MB_NLCP_LT_EORUN,
+       MB_EXT_LB, MB_EXT_GT, MB_EXT_FULL, MB_NCOUNT };
+static int64_t merge_branch[MB_NCOUNT];
+
+void orc_merge_counters(int64_t *out)
+{ int k;
+  for (k = 0; k < MB_NCOUNT; k++) out[k] = merge_branch[k];
+}
 
 int64_t orc_merge(const rec128 *T1, int64_t n1, const rec128 *T2, int64_t n2,
                   const uint32_t *pstart2, int freq, orc_seed *out, int64_t *sumlen)
@@ -188,6 +198,7 @@ int64_t orc_merge(const rec128 *T1, int64_t n1, const rec128 *T2, int64_t n2,
   int     plen = 12, eorun = 0;
   int64_t vlcp[KMER+1], rend = 0, low = 0, hgh = 0, top = 0;
   (void) n2;
+  memset(merge_branch,0,sizeof(merge_branch));
 
 #define LB(x) ((x) >= cend ? 11 : klcp(T2+(x)-1,T2+(x)))      /* ctop[LBYTE] = 11 sentinel (:719) */
 
@@ -202,6 +213,7 @@ int64_t orc_merge(const rec128 *T1, int64_t n1, const rec128 *T2, int64_t n2,
               cpre = -1;
               continue;
             }
+          merge_branch[MB_PANEL] += 1;
           plen = 12;
           vlcp[plen] = rend = cbeg;
           eorun = 0;
@@ -209,15 +221,25 @@ int64_t orc_merge(const rec128 *T1, int64_t n1, const rec128 *T2, int64_t n2,
       else
         { int nlcp = klcp(T1+i-1,e1);                   /* suf1[LBYTE] (:752) */
           if (nlcp > plen)
-            goto pairs;
+            { merge_branch[MB_NLCP_GT] += 1;
+              goto pairs;
+            }
           else if (nlcp == plen)
-            { if (eorun) goto pairs; }
+            { merge_branch[eorun ? MB_NLCP_EQ_EORUN : MB_NLCP_EQ] += 1;
+              if (eorun) goto pairs;
+            }
           else
-            { if (!eorun) rend += 1;
+            { int64_t r0;
+              merge_branch[MB_NLCP_LT] += 1;
+              if (!eorun) rend += 1;
+              r0 = rend;
               while (LB(rend) > nlcp) rend += 1;
+              if (rend > r0) merge_branch[MB_REND_SKIP] += 1;
               plen = LB(rend);
               if (plen < nlcp)
-                { eorun = 1; plen = nlcp; goto range; }
+                { merge_branch[MB_NLCP_LT_EORUN] += 1;
+                  eorun = 1; plen = nlcp; goto range;
+                }
               eorun = 0;
             }
         }
@@ -227,12 +249,18 @@ int64_t orc_merge(const rec128 *T1, int64_t n1, const rec128 *T2, int64_t n2,
           for (d = kbase(T2+rend,plen); d < c; d = kbase(T2+rend,plen))
             { rend += 1;
               if (LB(rend) < plen)
-                { eorun = 1; goto range; }
+                { merge_branch[MB_EXT_LB] += 1;
+                  eorun = 1; goto range;
+                }
             }
-          if (d > c) goto range;
+          if (d > c)
+            { merge_branch[MB_EXT_GT] += 1;
+              goto range;
+            }
           plen += 1;
           vlcp[plen] = rend;
         }
+      merge_branch[MB_EXT_FULL] += 1;
       do rend += 1; while (LB(rend) >= KMER);
       eorun = 1;
 

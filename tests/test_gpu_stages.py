@@ -137,7 +137,8 @@ def test_merge_and_seed_sort_match_oracle(small_pair):
 @pytest.mark.parametrize("copies", [2, 5])
 def test_merge_against_a_denser_second_table(copies):
     """a shard of genome 1 against all of genome 2 (multi-GPU): T2 is several times denser than T1,
-    the merge switches to 32- / 16-entry tiles so that the block's T2 slice still fits its staging"""
+    the merge switches from 512- to 256-, 128- or 64-entry tiles so that the block's T2 slice still fits
+    its staging"""
     rng = np.random.default_rng(90 + copies)
     a = rng.integers(0, 4, 400_000, dtype=np.uint8)
     B = [synth.diverged_copy(rng, a, 0.03 + 0.01 * k, sv_every=60_000) for k in range(copies)]
