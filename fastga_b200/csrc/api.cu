@@ -717,9 +717,12 @@ extern "C" int fgb_seeds_merge(const fgb_gix *x1, const fgb_gix *x2, long long a
 
 //  Count + scatter of n 16-byte records by owner[field], field = the nbits bits at bit pos of the record
 //  (nowner entries): d_out[bounds[w] .. bounds[w+1]) are the records of owner w, order inside a group free.
+//  Every owner entry must name a rank of the world: the kernel indexes its per-rank counters with it.
 static int group_by_owner(const void *d_src, long long n, int pos, int nbits, const int *owner, int nowner,
                           int world, void *d_out, long long *bounds, cudaStream_t st)
 { if (world < 1 || world > 64) return FGB_ERR_ARG;
+  for (int i = 0; i < nowner; i++)
+    if (owner[i] < 0 || owner[i] >= world) return FGB_ERR_ARG;
   for (int w = 0; w <= world; w++) bounds[w] = 0;
   if (n <= 0) return FGB_OK;
   dblock<int> d_owner; dblock<u64> d_cnt;

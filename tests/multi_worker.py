@@ -2,7 +2,10 @@
 every rank scans its contigs, k-mer records and seeds are exchanged with all-to-alls, every rank
 extends the seeds of its A-contigs); rank 0 gathers the record streams and checks the union against
 a single-GPU run of the whole pair.  FGB_MULTI_BACKEND: nccl (default; one GPU per rank) or gloo
-(ranks may share a GPU).  FGB_MULTI_PAIR: a case of tests/edge_cases.py in place of the default pair.
+(ranks may share a GPU).  FGB_MULTI_PAIR: "few_contigs" (three contigs per genome, fewer than the
+ranks of a world of 8, and a B contig with two exact copies of one A segment) or a case of
+tests/edge_cases.py in place of the default pair.  Rank 0 also checks the gathered records in their
+gathered order against the single-GPU run's .1aln order.
 
 Every rank holds both genomes, so a seed routed to the wrong rank would still be extended correctly
 and the union of the records would not show it: every rank also decodes the icont field of each seed
@@ -41,7 +44,16 @@ def main():
     else:
         dist.init_process_group(backend)
     case = os.environ.get("FGB_MULTI_PAIR")
-    if case:
+    if case == "few_contigs":
+        A, B = synth.make_pair(78, 3_000_000, 3, 0.05, sv_every=80_000)
+        # two exact copies of one A segment in a B contig, each between 100 bases that differ from A's
+        # flanks at every position: two alignments with the same A interval, tied on (aread, abpos, bread,
+        # comp), whose order only the discovery order sets
+        import edge_cases
+        seg = np.concatenate([3 - A[0][99_900:100_000], A[0][100_000:130_000], 3 - A[0][130_000:130_100]])
+        B[1] = np.concatenate([B[1][:50_000], seg, B[1][50_000:60_000], seg, B[1][60_000:]])
+        B = edge_cases._distinct(B)
+    elif case:
         import edge_cases
         A, B, _, _ = edge_cases.CASES[case]()
     else:
@@ -58,6 +70,9 @@ def main():
         print("OWNER_MISMATCH rank=%d icont=%s" % (rank, np.unique(ic[own_by_rank[ic] != rank])[:10].tolist()),
               flush=True)
         raise AssertionError("rank %d received seeds of A-contig ranks it does not own" % rank)
+    print("RANK_OK rank=%d contigs=%d seeds=%d records=%d" % (rank, int((shard.owner_of_contigs(gA.clen, world)
+                                                                        == rank).sum()), len(recs), len(alns)),
+          flush=True)
     tot = torch.tensor([st["nkmers1_fwd"], st["nkmers2"], st["nseeds_merged"], st["nseeds"], st["nhits"]],
                        dtype=torch.int64, device=dev)
     dist.all_reduce(tot)
@@ -72,8 +87,16 @@ def main():
         assert t[4] == ws["nhits"], (t, ws["nhits"])
         a, b = merged.canonical_lines(), whole.canonical_lines()
         assert len(a) == len(b) and a == b, (len(a), len(b))
+        a, b = merged.canonical_lines_unsorted(), whole.canonical_lines_unsorted()
+        if a != b:
+            i = next(i for i, (x, y) in enumerate(zip(a, b)) if x != y)
+            print("ORDER_MISMATCH first=%d\n  gathered %s\n  single   %s" % (i, a[i], b[i]), flush=True)
+            raise AssertionError("gathered records are not in the single-GPU .1aln order")
         assert merged.nraw == whole.nraw
-        print("MULTI_OK world=%d records=%d backend=%s maxicont=%d" % (world, len(a), backend, int(maxic.item())))
+        key = merged.fields[:, [1, 3, 2, 0]]
+        ties = int((key[1:] == key[:-1]).all(axis=1).sum())      # records whose order only the gather's tie rule sets
+        print("MULTI_OK world=%d records=%d backend=%s maxicont=%d ties=%d" % (world, len(a), backend,
+                                                                             int(maxic.item()), ties))
     dist.destroy_process_group()
 
 

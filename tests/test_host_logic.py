@@ -1,14 +1,13 @@
-"""CPU tests of the host side: formats, C-ABI surface, sharding + gather (gloo, world_size 2)."""
+"""CPU tests of the host side: formats, C-ABI surface, sharding + gather (gloo, 2 to 4 ranks)."""
 import ctypes
 import os
 import re
-import subprocess
-import sys
 
 import numpy as np
 import pytest
 
 import oracle_lib as ol
+import torchrun_ranks
 from fastga_b200 import formats, shard, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -100,6 +99,9 @@ rank, world = dist.get_rank(), dist.get_world_size()
 rng = np.random.default_rng(7)                       # same stream on every rank: everybody knows every block
 send = rng.integers(0, 50, (world, world))           # send[src][dst] rows
 send[0, 1] = 0                                       # an empty block
+if world > 2:                                        # rank 1 sends nothing, the last rank receives nothing
+    send[1, :] = 0
+    send[:, world - 1] = 0
 blocks = [[rng.integers(-2**62, 2**62, (int(send[s, d]), 2)) for d in range(world)] for s in range(world)]
 mine = np.concatenate(blocks[rank]) if send[rank].sum() else np.zeros((0, 2), np.int64)
 got = shard.exchange_rows(dist, torch.from_numpy(mine.astype(np.int64)), [int(v) for v in send[rank]])
@@ -120,10 +122,18 @@ def test_record_exchange_gloo_world2(tmp_path):
     """the all-to-all of 16-byte records that moves k-mer records and seeds between ranks (N > 1 path)"""
     script = tmp_path / "xworker.py"
     script.write_text(_XWORKER % {"root": ROOT})
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29583", str(script)],
-                       stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-    assert r.returncode == 0 and r.stdout.count("XCHG_OK") == 2, r.stdout[-3000:]
+    rc, out = torchrun_ranks.run(script, 2, 29583, timeout=600)
+    assert rc == 0 and out.count("XCHG_OK") == 2, out[-3000:]
+
+
+@pytest.mark.parametrize("world,port", [(3, 29584), (4, 29585)])
+def test_record_exchange_gloo_zero_length_splits(tmp_path, world, port):
+    """at 3 and 4 ranks, with zero-row splits on both sides: a rank that sends nothing at all, a rank that
+    receives nothing, and an empty block between two others"""
+    script = tmp_path / "xworker.py"
+    script.write_text(_XWORKER % {"root": ROOT})
+    rc, out = torchrun_ranks.run(script, world, port, timeout=600)
+    assert rc == 0 and out.count("XCHG_OK") == world, out[-3000:]
 
 
 _WORKER = r'''
@@ -159,14 +169,61 @@ def test_gather_alignments_gloo_world2(tmp_path):
     script = tmp_path / "worker.py"
     script.write_text(_WORKER % {"root": ROOT, "out": str(tmp_path)})
     env = dict(os.environ, MASTER_ADDR="127.0.0.1", MASTER_PORT="29581")
-    r = subprocess.run([sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2",
-                        "--master-addr", "127.0.0.1", "--master-port", "29581", str(script)],
-                       env=env, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-3000:]
+    rc, out = torchrun_ranks.run(script, 2, 29581, env=env, timeout=600)
+    assert rc == 0, out[-3000:]
     merged = list(np.load(tmp_path / "merged.npy", allow_pickle=True))
     want = sorted(list(np.load(tmp_path / "lines_0.npy", allow_pickle=True)) +
                   list(np.load(tmp_path / "lines_1.npy", allow_pickle=True)))
     assert merged == want
+
+
+_GWORKER = r'''
+import os, sys
+sys.path.insert(0, %(root)r)
+import numpy as np, torch, torch.distributed as dist
+from fastga_b200 import lib, shard
+dist.init_process_group("gloo")
+rank, world = dist.get_rank(), dist.get_world_size()
+rng = np.random.default_rng(300 + rank)
+n = 0 if rank == 1 else 60 + 7 * rank                 # rank 1 has no alignments
+fields = rng.integers(0, 1000, (n, 9)).astype(np.int32)
+fields[:, 0] = rng.integers(0, 2, n)                  # comp
+fields[:, 1] = rng.integers(0, 3, n)                  # local contig numbers
+fields[:, 2] = rng.integers(0, 2, n)                  # bread
+fields[:, 3] = rng.integers(0, 3, n)                  # abpos: few values, so that many records tie on the key
+fields[:, 8] = 2 * rng.integers(1, 6, n)              # tlen
+toff = np.concatenate([[0], np.cumsum(fields[:-1, 8])]).astype(np.int64) if n else np.zeros(0, np.int64)
+pool = rng.integers(0, 256, max(int(fields[:, 8].sum()), 1), dtype=np.uint8)
+cmap = np.array([rank, 10 + rank, 20], dtype=np.int32)   # global contig 20 has records of every rank
+merged = shard.gather_alignments(lib.Alignments(fields, toff, pool, n + 5), cmap, dist, torch.device("cpu"))
+gfields = fields.copy()
+gfields[:, 1] = cmap[fields[:, 1]]
+np.save(os.path.join(%(out)r, "fields_%%d.npy" %% rank), gfields)
+np.save(os.path.join(%(out)r, "lines_%%d.npy" %% rank), np.array(
+    lib.Alignments(gfields, toff, pool, n).canonical_lines_unsorted(), dtype=object), allow_pickle=True)
+if rank == 0:
+    assert merged.nraw == sum((0 if r == 1 else 60 + 7 * r) + 5 for r in range(world)), merged.nraw
+    np.save(os.path.join(%(out)r, "merged.npy"), np.array(merged.canonical_lines_unsorted(), dtype=object),
+            allow_pickle=True)
+dist.destroy_process_group()
+'''
+
+
+def test_gather_alignments_gloo_world3_keeps_each_ranks_order_on_ties(tmp_path):
+    """the gathered records are every rank's records concatenated in rank order and ordered by (aread,
+    abpos, bread, comp) with ties kept in that order (the .1aln order the single-GPU run writes, where
+    records of one A-contig come in discovery order); rank 1 contributes nothing"""
+    script = tmp_path / "gworker.py"
+    script.write_text(_GWORKER % {"root": ROOT, "out": str(tmp_path)})
+    rc, out = torchrun_ranks.run(script, 3, 29586, timeout=600)
+    assert rc == 0, out[-3000:]
+    fields = np.concatenate([np.load(tmp_path / ("fields_%d.npy" % k)) for k in range(3)])
+    lines = sum((list(np.load(tmp_path / ("lines_%d.npy" % k), allow_pickle=True)) for k in range(3)), [])
+    assert len(np.load(tmp_path / "fields_1.npy")) == 0 and len(lines) == len(fields)
+    order = sorted(range(len(fields)), key=lambda i: tuple(fields[i, [1, 3, 2, 0]]))
+    keys = [tuple(fields[i, [1, 3, 2, 0]]) for i in order]
+    assert len(set(keys)) < len(keys) // 2                 # many ties, within a rank and across ranks
+    assert list(np.load(tmp_path / "merged.npy", allow_pickle=True)) == [lines[i] for i in order]
 
 
 # ---- the hit-group rule of fgb_extend (host code of the library, no device) ----
