@@ -2497,10 +2497,17 @@ struct ExtendOut
 //  Phase 1: the band segments of the sorted seeds (P.seg_start, P.nseg), the prefilter, and the work
 //  triples (P.work, P.nwork): long ones first, largest first (the kernel's makespan is its longest
 //  triple, so it must not start late), then the short ones that hold a chain.  One wait, for the counts
-//  that size the work list.  L.nlong long triples are sorted (none when there are more than 2^20: they
-//  keep the prefilter's order and are scanned in extend_kernel); L.wsize holds their seed counts in work
+//  that size the work list.  L.nlong long triples are sorted (none when there are more than 2^20, or than
+//  long_sort_cap(): they keep the prefilter's order and are scanned in extend_kernel); L.wsize holds their seed counts in work
 //  order, L.sum the seeds of every long triple.
 static int bitlen_u64(u64 v) { int b = 0; while (v > 0) { b += 1; v >>= 1; } return b; }
+
+//  The most long triples that are sorted into launch order and go through chain detection: 2^20, or
+//  FGB_LONG_SORT_CAP (0: never; read on every call, so a test can reach the unsorted order on small inputs)
+static long long long_sort_cap()
+{ const char *s = getenv("FGB_LONG_SORT_CAP");
+  return s == NULL ? (1ll << 20) : atoll(s);
+}
 
 struct LongTriples { dblock<unsigned> wsize; unsigned nlong = 0; unsigned long long sum = 0; };
 
@@ -2535,7 +2542,7 @@ static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, d
   L.sum = (unsigned long long) cnt[6] | ((unsigned long long) cnt[7] << 32);
   P.nseg = (int) nseg;
   CUDA_TRY(d_work.alloc((size_t) nlong + nshort + 1,st));
-  if (nlong >= 1 && nlong <= (1u << 20))
+  if (nlong >= 1 && (long long) nlong <= long_sort_cap())
     { const int sbits = bitlen_u64((u64) n), jbits = bitlen_u64((u64) nseg);
       const u64 smax = (1ull << sbits) - 1;
       const long long tmpb = fgb_sort128_tmp_bytes(nlong);
