@@ -482,7 +482,10 @@ extern "C" int fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, in
 }
 
 //  a table over n unsorted device records (copied) whose 12-base prefixes lie in [plo,phi): one
-//  rank's slice of a k-mer-space sharded table
+//  rank's slice of a k-mer-space sharded table.  The range is a precondition this call does not check: a
+//  record outside it wraps the fine-bin and sub-bin arithmetic of fgb_kmer_sort_device, so it is dropped
+//  silently or sends kmer_bucket_sort_kernel's cnt[] index out of bounds.  Refusing such records would need a
+//  device check before the bucket sort, and another host wait on the sharded path.
 extern "C" int fgb_gix_from_records(const void *d_recs, long long n, unsigned plo, unsigned phi, int fwd_only,
                                     int post_bytes, int cont_bytes, int ncontig, fgb_gix **out, void *stream)
 { cudaStream_t st = (cudaStream_t) stream;

@@ -217,7 +217,9 @@ int  fgb_kmers_scan(const fgb_genome *g, const unsigned char *mask, int fwd_only
    holds the records of rank w */
 int  fgb_records_group_by_owner(const void *d_recs, long long n, const int *owner256, int world,
                                 void *d_out, long long *bounds, void *stream);
-/* sorted + indexed table over records whose 12-base prefix lies in [plo,phi) (one rank's slice) */
+/* sorted + indexed table over records whose 12-base prefix lies in [plo,phi) (one rank's slice).  Precondition,
+   not checked: every record's prefix lies in [plo,phi) and the records are unique.  A record outside the range
+   wraps the sort's bin arithmetic: it is dropped silently or corrupts the sort. */
 int  fgb_gix_from_records(const void *d_recs, long long n, unsigned plo, unsigned phi, int fwd_only,
                           int post_bytes, int cont_bytes, int ncontig, fgb_gix **out, void *stream);
 /* adaptamer merge without the seed sort: unsorted seed records, bits[4] = anti/band/jcont/icont

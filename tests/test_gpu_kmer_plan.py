@@ -2,43 +2,15 @@
 records and the bucket-sort groups from a planning kernel, so a table build waits on the host only for the
 count pass's total and, at its end, for the plan's count of bins too large for a CTA.  The tables are pinned to
 the oracle and to FGB_KSORT_PARTITION=1 by test_gpu_kmer_build; this file counts the waits, covers the routes
-that file does not (an empty range, the sharded table from records), and restates the packing rule."""
+that file does not (an empty range, the sharded table from records), and checks the restated packing rule
+(kmer_sort_cases.plan_groups) on random bin sizes."""
 import numpy as np
 import pytest
 
 from fastga_b200 import formats, lib
 
+from kmer_sort_cases import BK_SPAN, plan_groups
 from test_gpu_kmer_build import BK_CAP, _DeviceRecords, assert_matches_oracle, assert_paths_agree, scanned_records
-
-BK_SPAN = 4         # bins a group of the bucket sort may cover
-
-
-def plan_groups(bins):
-    """the planning kernel's rule on bin starts bins[0..nbins]: windows of BK_SPAN bins, each packed greedily into
-    groups (start, count, first bin); bins above BK_CAP records are listed apart as (start, count)"""
-    groups, over = [], []
-    for w0 in range(0, len(bins) - 1, BK_SPAN):
-        gs = gc = gp = 0
-        for p in range(w0, min(w0 + BK_SPAN, len(bins) - 1)):
-            ln = int(bins[p + 1] - bins[p])
-            if ln == 0:
-                continue
-            if ln > BK_CAP:
-                if gc:
-                    groups.append((gs, gc, gp))
-                    gc = 0
-                over.append((int(bins[p]), ln))
-                continue
-            if gc + ln > BK_CAP:
-                groups.append((gs, gc, gp))
-                gc = 0
-            if gc == 0:
-                gs, gp = int(bins[p]), p
-            gc += ln
-        if gc:
-            groups.append((gs, gc, gp))
-    return groups, over
-
 
 @pytest.mark.parametrize("seed", range(6))
 def test_packing_keeps_bins_whole(seed):
