@@ -26,5 +26,8 @@ def load_library():
             raise LibraryMissing(
                 "fastga_b200: %s not found -- run `python __graft_entry__.py` (build()) first; "
                 "there is no CPU fallback" % LIB_PATH)
-        _lib = ctypes.CDLL(LIB_PATH)
+        from .lib import bind
+        L = ctypes.CDLL(LIB_PATH)
+        bind(L)
+        _lib = L
     return _lib

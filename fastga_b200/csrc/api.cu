@@ -810,12 +810,6 @@ extern "C" int fgb_device_ready()
  *  Read_GDB and la_merge (FastGA.c:4927-5205), GIX construction included.
  **********************************************************************************************/
 
-struct fgb_run_stats
-{ long long nkmers1, nkmers2, nseeds, sumlen, nhits, nla, nwaves, ncells, nraw, h2d_bytes, d2h_bytes,
-            nseg, nwork, warp_cycles, wave_cycles, extract_cycles,
-            us_gix, us_seeds, us_extend, us_filter, nkmers1_fwd,
-            slow_cycles, slow_waves, paired_waves, pairings, gix_waits; };
-
 //  The whole path on staged genomes: k-mer tables -> adaptamer merge -> seed sort -> extension -> filter.
 //  self: SELF mode (`FastGA A`, B == A): one both-strand table merged against itself by the self block
 //  rule, and the band borders of align_contigs for a contig against itself.
@@ -866,14 +860,14 @@ static int align_pipeline(const fgb_genome *A, const fgb_genome *B, bool self, c
   std::unique_ptr<fgb_overlaps> ov(po);
   rc = fgb_filter(ov.get(),A->perm.data(),B->perm.data(),jb,ib,1,out);
   t4 = now_us();
-  unsigned long long c[16];
-  fgb_overlaps_counters(ov.get(),c);
+  const ext_counters &c = ov->counters;
   s.us_gix = t1-t0; s.us_seeds = t2-t1; s.us_extend = t3-t2; s.us_filter = t4-t3;
-  s.nhits = (long long) c[0]; s.nla = (long long) c[1]; s.nwaves = (long long) c[2]; s.ncells = (long long) c[3];
-  s.nseg = (long long) c[5]; s.nwork = (long long) c[6];
-  s.warp_cycles = (long long) c[8]; s.wave_cycles = (long long) c[9]; s.extract_cycles = (long long) c[10];
-  s.slow_cycles = (long long) ((c[15] >> 40) << 12); s.slow_waves = (long long) ((c[15] >> 16) & 0xffffff);
-  s.paired_waves = (long long) c[11]; s.pairings = (long long) c[12];
+  s.nhits = (long long) c.hits; s.nla = (long long) c.la_calls; s.nwaves = (long long) c.waves;
+  s.ncells = (long long) c.cells; s.nseg = (long long) c.nseg; s.nwork = (long long) c.nwork;
+  s.warp_cycles = (long long) c.warp_cycles; s.wave_cycles = (long long) c.wave_cycles;
+  s.extract_cycles = (long long) c.extract_cycles;
+  s.slow_cycles = (long long) ((c.slowest_warp >> 40) << 12); s.slow_waves = (long long) ((c.slowest_warp >> 16) & 0xffffff);
+  s.paired_waves = (long long) c.paired_waves; s.pairings = (long long) c.pairings;
   s.h2d_bytes = A->h2d_bytes + (self ? 0 : B->h2d_bytes) + 65536*2;
   s.d2h_bytes = fgb_overlaps_bytes(ov.get()) + 16 + 8*1024*(self ? 1 : 2) + 64;    // 8 KB of bucket counts per table
   if (stats) *stats = s;

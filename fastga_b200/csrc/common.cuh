@@ -1,15 +1,10 @@
 // Shared device/host helpers for the fastga_b200 kernels (sm_90a only).
 #pragma once
+#include "../../include/fastga_b200.h"        // the FGB_* return codes
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
-
-#define FGB_OK            0
-#define FGB_ERR_CUDA     -1   // a CUDA runtime call failed (message on stderr)
-#define FGB_ERR_ARG      -2   // bad argument
-#define FGB_ERR_LIMIT    -3   // input exceeds a documented device-layout limit
-#define FGB_ERR_OVERFLOW -4   // a device work arena overflowed even after retry
 
 #define CUDA_TRY(call)                                                                   \
   do { cudaError_t _e = (call);                                                          \
@@ -89,6 +84,7 @@ template<class T> struct dblock
   void reset() { if (p != nullptr) { fgb_dfree(p,st); p = nullptr; } }
   T *release() { T *q = p; p = nullptr; return q; }
   operator T *() const { return p; }
+  T *operator->() const { return p; }
 private:
   T *p = nullptr;
   cudaStream_t st = 0;

@@ -88,10 +88,28 @@ struct ext_params
   Peb *cells; long long cells_per_warp;
   unsigned char *stage; int stage_bytes;               // per warp: 2 x stage_bytes
   unsigned char *out; u64 out_cap; u64 *out_used;
-  u64 *counters;                                       // 0 hits 1 LA calls 2 waves 3 cells 4 records
+  ext_counters *counters;                              // every warp adds its counts at the end of a launch
   unsigned char *bigstate;                            // wide-band kernel: per-warp wave state in HBM
   int self_mode;                                       // FastGA A: genome against itself (align_contigs :3030)
 };
+
+//  The control words of the extension stage: one block in device memory, zeroed per call.  Kernels get
+//  pointers to single fields; the host copies the block back and reads it by name.
+struct ext_ctl
+{ unsigned unused0;
+  unsigned queue;                  // next item of a launch to hand out
+  unsigned nfailed;                // items of a launch that failed (ext_params::failed)
+  unsigned unused3;
+  u64 out_used;                    // record bytes asked for (beyond out_cap: the record buffer overflowed)
+  unsigned ntrip[2];               // work triples of the prefilter: [0] long, [1] short
+  u64 hits_used;                   // hit slots chain detection asked for
+  unsigned need;                   // OR of 1 << ST_* over a launch's failures
+  unsigned nseg;                   // band segments
+  u64 long_seeds;                  // seeds of the long triples
+};
+static_assert(offsetof(ext_ctl,queue) == 4 && offsetof(ext_ctl,nfailed) == 8 && offsetof(ext_ctl,out_used) == 16 &&
+              offsetof(ext_ctl,ntrip) == 24 && offsetof(ext_ctl,hits_used) == 32 && offsetof(ext_ctl,need) == 40 &&
+              offsetof(ext_ctl,nseg) == 44 && offsetof(ext_ctl,long_seeds) == 48, "control word offsets");
 
 struct Ctx
 { const unsigned *A, *B; int alen, blen; long long anw, bnw;
@@ -1347,31 +1365,30 @@ static __device__ int local_alignment(Ctx &c, int acomp, int low, int hgh, int a
   return ST_OK;
 }
 
-#define OUT_HDR 40        // bytes: triple, seq, pairkey, abpos, bbpos, aepos, bepos, diffs, tlen, 0
-
 //  Appends one alignment record; ACOMP flip of coordinates and trace order (align.c:1534-1557).
 
 static __device__ void emit_record(const ext_params &P, Ctx &c, const LAres &R, int acomp,
                                    unsigned triple, int seq, unsigned pairkey)
 { const int lane = threadIdx.x & 31;
   int tlen = R.rtlen + R.ftlen;
-  u64 need = OUT_HDR + ((tlen + 7) & ~7);
+  u64 need = ovl_bytes(tlen);
   u64 off = 0;
   if (lane == 0) off = atomicAdd(P.out_used,need);
   off = __shfl_sync(FULL,off,0);
   if (off + need > P.out_cap) return;                 // host sees out_used > cap and retries
   unsigned char *o = P.out + off;
   if (lane == 0)
-    { int *h = (int *) o;
+    { ovl_hdr *h = (ovl_hdr *) o;
       int ab = R.abpos, bb = R.bbpos, ae = R.aepos, be = R.bepos;
       if (acomp)
         { ab = c.alen - R.aepos; ae = c.alen - R.abpos;
           bb = c.blen - R.bepos; be = c.blen - R.bbpos;
         }
-      h[0] = (int) triple; h[1] = seq; h[2] = (int) pairkey;
-      h[3] = ab; h[4] = bb; h[5] = ae; h[6] = be; h[7] = R.diffs; h[8] = tlen; h[9] = P.attempt;
+      h->triple = (int) triple; h->seq = seq; h->pairkey = (int) pairkey;
+      h->abpos = ab; h->bbpos = bb; h->aepos = ae; h->bepos = be; h->diffs = R.diffs; h->tlen = tlen;
+      h->launch = P.attempt;
     }
-  unsigned char *t = o + OUT_HDR;
+  unsigned char *t = o + sizeof(ovl_hdr);
   for (int i = lane*2; i < tlen; i += 64)             // pair i/2 of the un-flipped trace
     { const unsigned char *src = (i < R.rtlen) ? (c.rstage + i) : (c.fstage + (i - R.rtlen));
       int dst = acomp ? (tlen - 2 - i) : i;
@@ -2194,24 +2211,25 @@ extend_kernel(ext_params P)
       st_release_smem(&c.box->seq,c.box->seq + 1);
     }
   if (lane == 0)
-    { atomicAdd(&P.counters[0],nhits);
-      atomicAdd(&P.counters[1],nla);
-      atomicAdd(&P.counters[2],c.nwaves);
-      atomicAdd(&P.counters[3],c.ncells);
-      atomicAdd(&P.counters[8],(u64) (clock64() - t_start));
-      atomicAdd(&P.counters[9],c.cyc_wave);
-      atomicAdd(&P.counters[10],c.cyc_extract);
-      atomicAdd(&P.counters[11],c.pwaves);
+    { ext_counters *K = P.counters;
+      atomicAdd(&K->hits,nhits);
+      atomicAdd(&K->la_calls,nla);
+      atomicAdd(&K->waves,c.nwaves);
+      atomicAdd(&K->cells,c.ncells);
+      atomicAdd(&K->warp_cycles,(u64) (clock64() - t_start));
+      atomicAdd(&K->wave_cycles,c.cyc_wave);
+      atomicAdd(&K->extract_cycles,c.cyc_extract);
+      atomicAdd(&K->paired_waves,c.pwaves);
       if (EX_DIAG)                                                    // slowest warp: cycles, of which in waves / read-outs (all >> 12)
-        atomicMax(&P.counters[12],(((u64) (clock64() - t_start) >> 12) << 40) | ((c.cyc_wave >> 12) << 20) | (c.cyc_extract >> 12));
-      else atomicAdd(&P.counters[12],c.npairs);
-      atomicAdd(&P.counters[4],c.fwait); atomicAdd(&P.counters[7],c.ftot);
-      atomicAdd(&P.counters[13],c.bwait);
-      if (EX_DIAG) atomicAdd(&P.counters[14],c.btot);                 // P warp wait cycles (diagnostic builds)
-      else atomicMax(&P.counters[14],(u64) (clock64() - t_start));
+        atomicMax(&K->pairings,(((u64) (clock64() - t_start) >> 12) << 40) | ((c.cyc_wave >> 12) << 20) | (c.cyc_extract >> 12));
+      else atomicAdd(&K->pairings,c.npairs);
+      atomicAdd(&K->front_wait,c.fwait); atomicAdd(&K->front_total,c.ftot);
+      atomicAdd(&K->back_wait,c.bwait);
+      if (EX_DIAG) atomicAdd(&K->max_warp_cycles,c.btot);             // P warp wait cycles (diagnostic builds)
+      else atomicMax(&K->max_warp_cycles,(u64) (clock64() - t_start));
       { u64 cy = (u64) (clock64() - t_start) >> 12, wv = c.nwaves > 0xffffff ? 0xffffff : c.nwaves;
         u64 la = nla > 0xffff ? 0xffff : nla;
-        atomicMax(&P.counters[15],(cy << 40) | (wv << 16) | la);      // the slowest warp: cycles/4096, waves, LA calls
+        atomicMax(&K->slowest_warp,(cy << 40) | (wv << 16) | la);     // the slowest warp: cycles/4096, waves, LA calls
       }
     }
 }
@@ -2269,9 +2287,7 @@ extern "C" int fgb_overlaps_from_buffer(const unsigned char *buf, long long nbyt
 extern "C" long long fgb_overlaps_bytes(const fgb_overlaps *o) { return o->nbytes; }
 extern "C" const unsigned char *fgb_overlaps_data(const fgb_overlaps *o) { return o->h_buf; }
 extern "C" void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out)
-{ for (int i = 0; i < 16; i++) out[i] = o->counters[i];          /* out: 16 entries */
-  out[5] = (unsigned long long) o->nseg; out[6] = (unsigned long long) o->nwork;
-}
+{ memcpy(out,&o->counters,sizeof(ext_counters)); }
 
 struct ev_timer
 { cudaEvent_t a, b; cudaStream_t st; int which;
@@ -2511,7 +2527,7 @@ static long long long_sort_cap()
 
 struct LongTriples { dblock<unsigned> wsize; unsigned nlong = 0; unsigned long long sum = 0; };
 
-static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, dblock<unsigned> &d_seg,
+static int extend_triples(ext_params &P, const fgb_seeds *S, ext_ctl *d_ctl, dblock<unsigned> &d_seg,
                           dblock<unsigned> &d_work, LongTriples &L, cudaStream_t st)
 { const long long n = S->n;
   const long long ntiles = (n + SEG_TILE - 1) / SEG_TILE;
@@ -2523,23 +2539,22 @@ static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, d
   CUDA_TRY(d_seg.alloc((size_t) n + 2,st));
   CUDA_TRY(d_cand.alloc((size_t) (2*lcap + n + 1),st));           // long triples | their sizes | short ones
   CUDA_TRY(cudaMemsetAsync(d_status,0,8*((size_t) ntiles + 1),st));
-  unsigned *d_nseg = d_misc + 11;
   seg_scan_kernel<<<(unsigned) ntiles,SEG_THREADS,0,st>>>(S->d_rec,n,P.p_band,d_seg,d_status,
-                                                          (unsigned *) (d_status + ntiles),d_nseg);
+                                                          (unsigned *) (d_status + ntiles),&d_ctl->nseg);
   int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&nsm,cudaDevAttrMultiProcessorCount,dev);
   const long long pb = (n + 127) / 128 < 16ll*nsm ? (n + 127) / 128 : 16ll*nsm;
   P.seg_start = d_seg;
-  prefilter_kernel<<<(unsigned) pb,128,0,st>>>(P,d_nseg,d_cand,d_cand + 2*lcap,d_misc + 6,d_cand + lcap,
-                                               (unsigned long long *) (d_misc + 12));
+  prefilter_kernel<<<(unsigned) pb,128,0,st>>>(P,&d_ctl->nseg,d_cand,d_cand + 2*lcap,d_ctl->ntrip,d_cand + lcap,
+                                               &d_ctl->long_seeds);
   fgb_count_launch(2);
   CUDA_TRY(cudaGetLastError());
-  unsigned cnt[8];                                           // words 6-13 of d_misc
-  CUDA_TRY(cudaMemcpyAsync(cnt,d_misc + 6,32,cudaMemcpyDeviceToHost,st));
+  ext_ctl ctl;
+  CUDA_TRY(cudaMemcpyAsync(&ctl,d_ctl,sizeof(ext_ctl),cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  const unsigned nseg = cnt[5], nlong = cnt[0], nshort = cnt[1];
-  L.sum = (unsigned long long) cnt[6] | ((unsigned long long) cnt[7] << 32);
+  const unsigned nseg = ctl.nseg, nlong = ctl.ntrip[0], nshort = ctl.ntrip[1];
+  L.sum = ctl.long_seeds;
   P.nseg = (int) nseg;
   CUDA_TRY(d_work.alloc((size_t) nlong + nshort + 1,st));
   if (nlong >= 1 && (long long) nlong <= long_sort_cap())
@@ -2573,7 +2588,7 @@ static int extend_triples(ext_params &P, const fgb_seeds *S, unsigned *d_misc, d
 //  plan is built on the device from the triples' sizes, every kernel runs over a bound of the chunk count
 //  (sum of ceil(size / chunk) <= L.sum / chunk + L.nlong).  The hit lists stay in d_hits for the kernel and
 //  come to the host (X.hrange, X.tinfo, X.hh) through the pinned staging buffer, with one wait.
-static int chain_detect(const ext_params &P, const LongTriples &L, long long chunk, unsigned *d_misc,
+static int chain_detect(const ext_params &P, const LongTriples &L, long long chunk, ext_ctl *d_ctl,
                         dblock<ChainHit> &d_hits, ExtendPlan &X, cudaStream_t st)
 { const unsigned nwork = (unsigned) P.nwork, nlong = L.nlong;
   const unsigned long long pmax = L.sum / (unsigned long long) chunk + nlong + 1;
@@ -2589,7 +2604,7 @@ static int chain_detect(const ext_params &P, const LongTriples &L, long long chu
   CUDA_TRY(d_tinfo.alloc((size_t) nwork,st));
   CUDA_TRY(d_nplan.alloc(1,st));
   CUDA_TRY(d_tmp.alloc((size_t) tmpb,st));
-  CUDA_TRY(cudaMemsetAsync(d_misc + 8,0,8,st));
+  CUDA_TRY(cudaMemsetAsync(&d_ctl->hits_used,0,8,st));
   chain_nch_kernel<<<(nwork + 1 + 255)/256,256,0,st>>>(L.wsize,nlong,nwork,chunk,d_first);
   fgb_count_launch(1);
   int rc = fgb_dev_exclusive_scan_u32(d_first,(long long) nwork + 1,d_nplan,d_tmp,tmpb,st);
@@ -2597,7 +2612,7 @@ static int chain_detect(const ext_params &P, const LongTriples &L, long long chu
   chain_plan_kernel<<<(unsigned) ((pmax + 127)/128),128,0,st>>>(P,d_first,nlong,d_nplan,d_plan);
   chain_chunk_kernel<<<(unsigned) ((pmax + 3)/4),128,0,st>>>(P,d_plan,d_nplan,d_couts);
   chain_stitch_kernel<<<(nwork + 127)/128,128,0,st>>>(P,d_plan,d_couts,d_first,(int) nwork,d_hits,
-                                                     (unsigned long long *) (d_misc + 8),d_nplan,d_hrange,d_tinfo);
+                                                     &d_ctl->hits_used,d_nplan,d_hrange,d_tinfo);
   fgb_count_launch(3);
   //  staging layout: hits used, chunks | hrange | tinfo | the hit lists
   const size_t o1 = 16, o2 = o1 + sizeof(uint2)*(size_t) nwork, o3 = o2 + sizeof(int2)*(size_t) nwork;
@@ -2605,11 +2620,11 @@ static int chain_detect(const ext_params &P, const LongTriples &L, long long chu
   unsigned char *hp, *dp;
   CUDA_TRY(pinned_staging(o4 + sizeof(ChainHit)*(size_t) cap_max,&hp));
   CUDA_TRY(cudaHostGetDevicePointer((void **) &dp,hp,0));
-  hits_to_host_kernel<<<2*132,256,0,st>>>(d_hits,(const unsigned long long *) (d_misc + 8),d_nplan,(int) nwork,
+  hits_to_host_kernel<<<2*132,256,0,st>>>(d_hits,&d_ctl->hits_used,d_nplan,(int) nwork,
                                           (ChainHit *) (dp + o4));
   fgb_count_launch(1);
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(hp,d_misc + 8,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(hp,&d_ctl->hits_used,8,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaMemcpyAsync(hp + 8,d_nplan,8,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaMemcpyAsync(hp + o1,d_hrange,sizeof(uint2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaMemcpyAsync(hp + o2,d_tinfo,sizeof(int2)*(size_t) nwork,cudaMemcpyDeviceToHost,st));
@@ -2660,7 +2675,7 @@ static void first_items(unsigned nwork, ExtendPlan &X)
 //  wide-band kernel with larger arenas on fewer warps; collect_records drops what they emitted in
 //  earlier launches.  A launch that overflows the record buffer is repeated with a larger one, as the
 //  same step: its records keep the step's launch number and its counts are taken back.
-static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc, ExtendOut &R, cudaStream_t st)
+static int extend_launches(ext_params &P, const ExtendPlan &X, ext_ctl *d_ctl, ExtendOut &R, cudaStream_t st)
 { if (X.items.empty()) return FGB_OK;
   int dev = 0, nsm = 132;
   cudaGetDevice(&dev);
@@ -2688,11 +2703,11 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
   if (groups) CUDA_TRY(d_galast.alloc(items.size(),st));
   CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
   P.items = d_items; P.failed = d_failed; P.galast = d_galast;
-  P.queue = d_misc + 1; P.nfailed = d_misc + 2; P.out_used = (u64 *) (d_misc + 4); P.need = d_misc + 10;
+  P.queue = &d_ctl->queue; P.nfailed = &d_ctl->nfailed; P.out_used = &d_ctl->out_used; P.need = &d_ctl->need;
   R.cap = slack < 0 ? (u64) P.nwork * 512 + (64ull << 20) : (u64) slack;
   CUDA_TRY(R.buf.alloc(R.cap,st));
-  dblock<u64> d_snap;                            // the counters before a launch: a repeated launch counts nothing
-  CUDA_TRY(d_snap.alloc(16,st));
+  dblock<ext_counters> d_snap;                   // the counters before a launch: a repeated launch counts nothing
+  CUDA_TRY(d_snap.alloc(1,st));
   u64 used_before = 0;
   int repeats = 0;                               // of this step, for want of record buffer
   for (int attempt = 0; ; )
@@ -2700,9 +2715,9 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       CUDA_TRY(ar.alloc(P,nblocks * EX_WARPS,cells_per_warp,stage_bytes,attempt > 0,st));
       P.out = R.buf; P.out_cap = R.cap;
       P.nitems = (int) items.size(); P.groups = groups; P.attempt = attempt;
-      CUDA_TRY(cudaMemsetAsync(d_misc+1,0,8,st));          // queue, nfailed
-      CUDA_TRY(cudaMemsetAsync(d_misc+10,0,4,st));         // reasons of this attempt's failures
-      CUDA_TRY(cudaMemcpyAsync(d_snap,P.counters,16*8,cudaMemcpyDeviceToDevice,st));
+      CUDA_TRY(cudaMemsetAsync(&d_ctl->queue,0,8,st));     // queue, nfailed
+      CUDA_TRY(cudaMemsetAsync(&d_ctl->need,0,4,st));      // reasons of this attempt's failures
+      CUDA_TRY(cudaMemcpyAsync(d_snap,P.counters,sizeof(ext_counters),cudaMemcpyDeviceToDevice,st));
       { ev_timer t(1,st);
         if (attempt == 0)
           extend_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P);
@@ -2712,13 +2727,13 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       fgb_count_launch(1);
       CUDA_TRY(cudaGetLastError());
       R.launches += 1;
-      unsigned misc[12];
-      CUDA_TRY(cudaMemcpyAsync(misc,d_misc,48,cudaMemcpyDeviceToHost,st));
+      ext_ctl ctl;
+      CUDA_TRY(cudaMemcpyAsync(&ctl,d_ctl,sizeof(ext_ctl),cudaMemcpyDeviceToHost,st));
       if (groups) CUDA_TRY(cudaMemcpyAsync(ga.data(),d_galast,sizeof(long long)*items.size(),cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaStreamSynchronize(st));
       ar.reset();                                          // before the record buffer may grow
-      R.reasons |= misc[10];
-      R.used = ((u64) misc[5] << 32) | misc[4];
+      R.reasons |= ctl.need;
+      R.used = ctl.out_used;
       if (R.used > R.cap)
         { //  record buffer too small: grow it (keeping earlier steps' records) and repeat this step as it
           //  was -- same kernel, arenas and launch number, the counters of before it.  The repeat asks for
@@ -2730,8 +2745,8 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
           CUDA_TRY(d_new.alloc(ncap,st));
           if (used_before) CUDA_TRY(cudaMemcpyAsync(d_new,R.buf,used_before,cudaMemcpyDeviceToDevice,st));
           R.buf = std::move(d_new); R.cap = ncap;
-          CUDA_TRY(cudaMemcpyAsync(d_misc+4,&used_before,8,cudaMemcpyHostToDevice,st));
-          CUDA_TRY(cudaMemcpyAsync(P.counters,d_snap,16*8,cudaMemcpyDeviceToDevice,st));
+          CUDA_TRY(cudaMemcpyAsync(&d_ctl->out_used,&used_before,8,cudaMemcpyHostToDevice,st));
+          CUDA_TRY(cudaMemcpyAsync(P.counters,d_snap,sizeof(ext_counters),cudaMemcpyDeviceToDevice,st));
           R.used = used_before;
           continue;
         }
@@ -2739,8 +2754,8 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       used_before = R.used;
       //  the triples to re-run, by work-list position
       std::vector<unsigned> fw;
-      if (misc[2] > 0)
-        { std::vector<unsigned> f(misc[2]);
+      if (ctl.nfailed > 0)
+        { std::vector<unsigned> f(ctl.nfailed);
           CUDA_TRY(cudaMemcpyAsync(f.data(),d_failed,sizeof(unsigned)*f.size(),cudaMemcpyDeviceToHost,st));
           CUDA_TRY(cudaStreamSynchronize(st));
           for (size_t q = 0; q < f.size(); q++) fw.push_back(items[f[q]].w);
@@ -2774,8 +2789,8 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
       CUDA_TRY(cudaMemcpyAsync(d_items,items.data(),sizeof(ExItem)*items.size(),cudaMemcpyHostToDevice,st));
       //  grow only what overflowed: a band too wide for the register / shared-memory state (ST_BAND)
       //  just moves to the wide-band kernel with the same arenas
-      if (attempt > 0 || (misc[10] & (1u << ST_CELLS))) cells_per_warp *= 8;
-      if (attempt > 0 || (misc[10] & (1u << ST_STAGE))) stage_bytes *= 4;
+      if (attempt > 0 || (ctl.need & (1u << ST_CELLS))) cells_per_warp *= 8;
+      if (attempt > 0 || (ctl.need & (1u << ST_STAGE))) stage_bytes *= 4;
       nblocks = launch_blocks((long long) items.size(),EX_NFRONT,LLONG_MAX,cells_per_warp);
       attempt += 1;
     }
@@ -2785,7 +2800,7 @@ static int extend_launches(ext_params &P, const ExtendPlan &X, unsigned *d_misc,
 //  Phase 5: the records to the host (when there were launches), less those a re-run triple emitted in
 //  its earlier launches (every record carries its launch number: a triple keeps those of its LAST), and
 //  the counters
-static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, const u64 *d_counters,
+static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, const ext_counters *d_counters,
                            cudaStream_t st)
 { unsigned char *pin = NULL;
   if (launched)
@@ -2794,9 +2809,9 @@ static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, c
       ev_timer t(2,st);
       CUDA_TRY(cudaMemcpyAsync(pin,R.buf,R.used,cudaMemcpyDeviceToHost,st));
     }
-  CUDA_TRY(cudaMemcpyAsync(O->counters,d_counters,16*8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(&O->counters,d_counters,sizeof(ext_counters),cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
-  O->counters[0] += R.hits_done;
+  O->counters.hits += R.hits_done;
   if (launched)
     { memcpy(O->h_buf,pin,R.used);
       O->nbytes = (long long) R.used;
@@ -2808,10 +2823,10 @@ static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, c
         if (q + 1 == todo.size() || todo[q+1].first != todo[q].first) last.push_back(todo[q]);
       long long w = 0;
       for (long long off = 0; off < O->nbytes; )
-        { int *h = (int *) (O->h_buf + off);
-          const long long sz = OUT_HDR + ((h[8] + 7) & ~7);
-          auto it = std::lower_bound(last.begin(),last.end(),std::make_pair((unsigned) h[0],INT_MIN));
-          if (!(it != last.end() && it->first == (unsigned) h[0] && it->second != h[9]))
+        { const ovl_hdr *h = (const ovl_hdr *) (O->h_buf + off);
+          const long long sz = ovl_bytes(h->tlen);
+          auto it = std::lower_bound(last.begin(),last.end(),std::make_pair((unsigned) h->triple,INT_MIN));
+          if (!(it != last.end() && it->first == (unsigned) h->triple && it->second != h->launch))
             { if (w != off) memmove(O->h_buf + w,O->h_buf + off,sz);
               w += sz;
             }
@@ -2820,8 +2835,7 @@ static int collect_records(fgb_overlaps *O, const ExtendOut &R, bool launched, c
       O->nbytes = w;
     }
   for (long long off = 0; off < O->nbytes; )
-    { int *h = (int *) (O->h_buf + off);
-      off += OUT_HDR + ((h[8] + 7) & ~7);
+    { off += ovl_bytes(((const ovl_hdr *) (O->h_buf + off))->tlen);
       O->nrec += 1;
     }
   return FGB_OK;
@@ -2860,37 +2874,35 @@ extern "C" int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_gen
   P.dscore = -tables[0] / TRIM_LEN;                     // SCORE[0] = -15 * dscore
   const long long chunk = chain_chunk_seeds();
 
-  dblock<short> d_tables; dblock<u64> d_counters; dblock<unsigned> d_misc;
+  dblock<short> d_tables; dblock<ext_counters> d_counters; dblock<ext_ctl> d_ctl;
   CUDA_TRY(d_tables.alloc(65536,st));
   CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
   P.score = d_tables; P.table = d_tables + 32768;
-  CUDA_TRY(d_counters.alloc(16,st));
-  CUDA_TRY(cudaMemsetAsync(d_counters,0,16*8,st));
+  CUDA_TRY(d_counters.alloc(1,st));
+  CUDA_TRY(cudaMemsetAsync(d_counters,0,sizeof(ext_counters),st));
   P.counters = d_counters;
-  //  words 1 queue, 2 failed items, 4-5 record bytes, 6-7 prefilter counts, 8-9 hits listed, 10 failure reasons,
-  //  11 band segments, 12-13 seeds of the long triples
-  CUDA_TRY(d_misc.alloc(16,st));
-  CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
+  CUDA_TRY(d_ctl.alloc(1,st));
+  CUDA_TRY(cudaMemsetAsync(d_ctl,0,sizeof(ext_ctl),st));
 
   dblock<unsigned> d_seg, d_work; dblock<ChainHit> d_hits;
   ExtendPlan X;
   if (S->n > 0)
     { ev_timer t(0,st);
       LongTriples L;
-      int rc = extend_triples(P,S,d_misc,d_seg,d_work,L,st);
+      int rc = extend_triples(P,S,d_ctl,d_seg,d_work,L,st);
       if (rc) return rc;
       if (L.nlong > 0 && chunk > 0)
-        { rc = chain_detect(P,L,chunk,d_misc,d_hits,X,st);
+        { rc = chain_detect(P,L,chunk,d_ctl,d_hits,X,st);
           if (rc) return rc;
           P.hits = d_hits;
         }
       first_items((unsigned) P.nwork,X);
     }
-  O->nseg = P.nseg; O->nwork = P.nwork;
   ExtendOut R;
-  int rc = (P.nwork > 0) ? extend_launches(P,X,d_misc,R,st) : FGB_OK;
+  int rc = (P.nwork > 0) ? extend_launches(P,X,d_ctl,R,st) : FGB_OK;
   if (rc == FGB_OK) rc = collect_records(O.get(),R,P.nwork > 0,d_counters,st);
   if (rc) return rc;
+  O->counters.nseg = (u64) P.nseg; O->counters.nwork = (u64) P.nwork;
   O->retry[0] = R.launches; O->retry[1] = R.reasons; O->retry[2] = R.regrowths; O->retry[3] = (long long) R.rerun.size();
   *out = O.release();                                        // (the device blocks go back as the call returns)
   return FGB_OK;
@@ -2908,15 +2920,15 @@ extern "C" int fgb_chain_hits(const fgb_seeds *S, int chain_break, int chain_min
   if (S->n == 0) return FGB_OK;
   ext_params P;
   seed_params(P,S,chain_break,chain_min);
-  dblock<unsigned> d_misc, d_seg, d_work; dblock<ChainHit> d_hits;
-  CUDA_TRY(d_misc.alloc(16,st));
-  CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
+  dblock<ext_ctl> d_ctl; dblock<unsigned> d_seg, d_work; dblock<ChainHit> d_hits;
+  CUDA_TRY(d_ctl.alloc(1,st));
+  CUDA_TRY(cudaMemsetAsync(d_ctl,0,sizeof(ext_ctl),st));
   LongTriples L;
-  int rc = extend_triples(P,S,d_misc,d_seg,d_work,L,st);
+  int rc = extend_triples(P,S,d_ctl,d_seg,d_work,L,st);
   if (rc) return rc;
   ExtendPlan X;
   if (L.nlong > 0 && chunk_seeds > 0)
-    { rc = chain_detect(P,L,chunk_seeds,d_misc,d_hits,X,st);
+    { rc = chain_detect(P,L,chunk_seeds,d_ctl,d_hits,X,st);
       if (rc) return rc;
     }
   const long long nwork = P.nwork;
@@ -2988,7 +3000,7 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   int stage_bytes = (int) ladder_knob("FGB_EXTEND_STAGE",1 << 16,2);
   const long long nblocks = launch_blocks(n,EX_WARPS,nsm,cells_per_warp);
   const size_t smem = (size_t) EX_WARPS * STATE_BYTES;
-  dblock<short> d_tables; dblock<la_job> d_jobs; dblock<int> d_status; dblock<unsigned> d_misc;
+  dblock<short> d_tables; dblock<la_job> d_jobs; dblock<int> d_status; dblock<ext_ctl> d_ctl;
   dblock<unsigned char> d_out; dblock<unsigned> d_idx;
   Arenas ar;
   std::vector<unsigned char> h;
@@ -2998,19 +3010,19 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
   CUDA_TRY(d_tables.alloc(65536,st));
   CUDA_TRY(d_jobs.alloc((size_t) n,st));
   CUDA_TRY(d_status.alloc((size_t) n,st));
-  CUDA_TRY(d_misc.alloc(16,st));
+  CUDA_TRY(d_ctl.alloc(1,st));
   CUDA_TRY(ar.alloc(P,nblocks * EX_WARPS,cells_per_warp,stage_bytes,false,st));
   CUDA_TRY(d_out.alloc(out_cap,st));
   CUDA_TRY(cudaMemcpyAsync(d_tables,tables,65536*sizeof(short),cudaMemcpyHostToDevice,st));
   CUDA_TRY(cudaMemcpyAsync(d_jobs,jobs,sizeof(la_job)*(size_t) n,cudaMemcpyHostToDevice,st));
-  CUDA_TRY(cudaMemsetAsync(d_misc,0,64,st));
+  CUDA_TRY(cudaMemsetAsync(d_ctl,0,sizeof(ext_ctl),st));
   P.score = d_tables; P.table = d_tables + 32768;
-  P.out = d_out; P.out_cap = out_cap; P.out_used = (u64 *) (d_misc + 4);
-  P.queue = d_misc + 1;
+  P.out = d_out; P.out_cap = out_cap; P.out_used = &d_ctl->out_used;
+  P.queue = &d_ctl->queue;
   la_batch_kernel<EX_W><<<(unsigned) nblocks,EX_WARPS*32,smem,st>>>(P,d_jobs,NULL,(int) n,d_status);
   fgb_count_launch(1);
   CUDA_TRY(cudaGetLastError());
-  CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
+  CUDA_TRY(cudaMemcpyAsync(&out_used,&d_ctl->out_used,8,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
   CUDA_TRY(cudaStreamSynchronize(st));
   //  records that did not fit the record buffer: the bytes they need bound the trace bytes, so a call
@@ -3032,12 +3044,12 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       CUDA_TRY(ar.alloc(P,nb2 * EX_WARPS,cells_per_warp,stage_bytes,true,st));
       CUDA_TRY(d_idx.alloc(redo.size(),st));
       CUDA_TRY(cudaMemcpyAsync(d_idx,redo.data(),sizeof(unsigned)*redo.size(),cudaMemcpyHostToDevice,st));
-      CUDA_TRY(cudaMemsetAsync(d_misc + 1,0,4,st));                 // queue
+      CUDA_TRY(cudaMemsetAsync(&d_ctl->queue,0,4,st));              // queue
       CUDA_TRY(cudaFuncSetAttribute(la_batch_kernel<EX_WBIG>,cudaFuncAttributeMaxDynamicSharedMemorySize,(int) smem_big));
       la_batch_kernel<EX_WBIG><<<(unsigned) nb2,EX_WARPS*32,smem_big,st>>>(P,d_jobs,d_idx,(int) redo.size(),d_status);
       fgb_count_launch(1);
       CUDA_TRY(cudaGetLastError());
-      CUDA_TRY(cudaMemcpyAsync(&out_used,d_misc + 4,8,cudaMemcpyDeviceToHost,st));
+      CUDA_TRY(cudaMemcpyAsync(&out_used,&d_ctl->out_used,8,cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaMemcpyAsync(hs.data(),d_status,sizeof(int)*(size_t) n,cudaMemcpyDeviceToHost,st));
       CUDA_TRY(cudaStreamSynchronize(st));
       if (out_used > out_cap) { *traces_used = (long long) out_used; return FGB_ERR_OVERFLOW; }
@@ -3052,14 +3064,14 @@ extern "C" int fgb_local_alignments(const fgb_genome *A, const fgb_genome *B, lo
       toff[i] = 0;
     }
   for (u64 off = 0; off < out_used; )
-    { const int *r = (const int *) (h.data() + off);
-      const long long i = r[0];
+    { const ovl_hdr *r = (const ovl_hdr *) (h.data() + off);
+      const long long i = r->triple;                               // la_batch_kernel: the call's number
       int *p = paths + 7*i;
-      p[0] = r[3]; p[1] = r[4]; p[2] = r[5]; p[3] = r[6]; p[4] = r[7]; p[5] = r[8];
+      p[0] = r->abpos; p[1] = r->bbpos; p[2] = r->aepos; p[3] = r->bepos; p[4] = r->diffs; p[5] = r->tlen;
       toff[i] = used;
-      if (used + r[8] <= traces_cap) memcpy(traces + used,h.data() + off + OUT_HDR,(size_t) r[8]);
-      used += r[8];
-      off += OUT_HDR + ((r[8] + 7) & ~7);
+      if (used + r->tlen <= traces_cap) memcpy(traces + used,h.data() + off + sizeof(ovl_hdr),(size_t) r->tlen);
+      used += r->tlen;
+      off += ovl_bytes(r->tlen);
     }
   *traces_used = used;
   return used > traces_cap ? FGB_ERR_OVERFLOW : FGB_OK;

@@ -15,7 +15,6 @@
 #include <vector>
 #include <algorithm>
 
-#define OUT_HDR   40
 #define TSPACE    100
 #define BOX_FUZZ  10
 
@@ -161,10 +160,10 @@ extern "C" int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *pe
   const unsigned char *buf = fgb_overlaps_data(O);
   std::vector<RawRef> refs;
   for (long long off = 0; off < nb; )
-    { const int *h = (const int *) (buf + off);
-      RawRef r; r.triple = h[0]; r.seq = h[1]; r.off = off;
+    { const ovl_hdr *h = (const ovl_hdr *) (buf + off);
+      RawRef r; r.triple = h->triple; r.seq = h->seq; r.off = off;
       refs.push_back(r);
-      off += OUT_HDR + ((h[8] + 7) & ~7);
+      off += ovl_bytes(h->tlen);
     }
   std::sort(refs.begin(),refs.end(),[](const RawRef &a, const RawRef &b)
             { return a.triple != b.triple ? a.triple < b.triple : a.seq < b.seq; });
@@ -175,15 +174,15 @@ extern "C" int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *pe
   std::vector<Fin> fin;
   size_t i = 0;
   while (i < refs.size())
-    { int pk = ((const int *) (buf + refs[i].off))[2];
+    { int pk = ((const ovl_hdr *) (buf + refs[i].off))->pairkey;
       std::vector<Aln> g;
       size_t e = i;
-      while (e < refs.size() && ((const int *) (buf + refs[e].off))[2] == pk)
-        { const int *h = (const int *) (buf + refs[e].off);
+      while (e < refs.size() && ((const ovl_hdr *) (buf + refs[e].off))->pairkey == pk)
+        { const ovl_hdr *h = (const ovl_hdr *) (buf + refs[e].off);
           Aln o;
-          o.ab = h[3]; o.bb = h[4]; o.ae = h[5]; o.be = h[6]; o.diffs = h[7]; o.tlen = h[8];
+          o.ab = h->abpos; o.bb = h->bbpos; o.ae = h->aepos; o.be = h->bepos; o.diffs = h->diffs; o.tlen = h->tlen;
           o.dead = false;
-          o.trace = buf + refs[e].off + OUT_HDR;
+          o.trace = buf + refs[e].off + sizeof(ovl_hdr);
           g.push_back(std::move(o));
           e += 1;
         }

@@ -147,8 +147,6 @@ __global__ void rmsd_unpack_kernel(const rec128 *__restrict__ srt, long long n, 
     o[b] = (unsigned char) ((b < 8) ? (w.lo >> (8*b)) : (w.hi >> (8*(b-8))));
 }
 
-typedef struct { int beg; int end; long long off; } fgb_range;     // Range of RSDsort.c:254-258
-
 extern "C" int fgb_rmsd_sort(unsigned char *array, long long nelem, int rsize, int ksize, int nparts,
                              long long *part, int nthreads, fgb_range *parms)
 { long long asize = nelem*rsize;

@@ -1,17 +1,13 @@
-// Entry points that one .cu file of the library defines and another calls.  The defining file includes
-// this header too, so a definition that drifts from its declaration here does not compile.
+// Entry points that one .cu file of the library defines and another calls, beyond the C-ABI of
+// include/fastga_b200.h.  The defining file includes this header too, so a definition that drifts
+// from its declaration here or in the C-ABI header does not compile.
 #pragma once
+#include "../../include/fastga_b200.h"
 #include "common.cuh"
-
-struct fgb_genome;
-struct fgb_seeds;
-struct fgb_overlaps;
-struct fgb_alns;
 
 extern "C" {
 
 // ---- sort128.cu: radix sort of 16-byte records, k-mer table sort ----
-long long fgb_sort128_tmp_bytes(long long n);
 //  Stable LSD sort of n records in d_a on the 8-bit digits at bit offsets bit_lo, bit_lo+8, ... below
 //  bit_hi (the last digit may reach past bit_hi: the bits above a key are part of the order, zero in
 //  every record sorted here); d_b is a scratch of 16(n+1) bytes, d_tmp one of fgb_sort128_tmp_bytes(n).
@@ -21,8 +17,6 @@ long long fgb_sort128_tmp_bytes(long long n);
 int fgb_radix_sort_device(void *d_a, void *d_b, long long n, int bit_lo, int bit_hi, int narrow,
                           void *d_tmp, long long tmp_bytes, int *result_in_b, unsigned long long **d_hiflag,
                           void *stream);
-int fgb_sort128_device(void *d_a, void *d_b, long long n, int byte_lo, int byte_hi,
-                       void *d_tmp, long long tmp_bytes, int *result_in_b, void *stream);
 int fgb_kmer_bin_shift(long long n, unsigned plo, unsigned phi);
 void fgb_kmer_first_digit(long long nmax, unsigned plo, unsigned phi, int *fsh, int *dbits);
 long long fgb_kmer_plan_bytes(long long n, unsigned plo, unsigned phi, int fsh, int dbits);
@@ -68,17 +62,5 @@ int fgb_owner_count_device(const void *d_seeds, long long n, int p_ic, int ic_bi
                            int world, unsigned long long *d_cnt, void *stream);
 int fgb_owner_scatter_device(const void *d_seeds, long long n, int p_ic, int ic_bits, const int *d_owner, int nrc,
                              int world, unsigned long long *d_base, void *d_out, void *stream);
-
-// ---- extend.cu and filter.cu: extension, alignment spec, raw overlaps, redundancy filter ----
-int fgb_extend(const fgb_seeds *S, const fgb_genome *A, const fgb_genome *B, int chain_break,
-               int chain_min, int align_min, double align_rate, const short *tables, int ave_path,
-               int tspace, fgb_overlaps **out, void *stream);
-int fgb_align_spec(double ave_corr, const float *freq, short *tables, int *ave_path);
-long long fgb_overlaps_bytes(const fgb_overlaps *o);
-const unsigned char *fgb_overlaps_data(const fgb_overlaps *o);
-void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out);
-void fgb_overlaps_retry_info(const fgb_overlaps *o, long long out[4]);
-int fgb_filter(const fgb_overlaps *O, const int *perm1, const int *perm2, int jc_bits, int ic_bits,
-               int do_filter, fgb_alns **out);
 
 }

@@ -5,7 +5,7 @@ import numpy as np
 
 from . import load_library
 
-c_void_p, c_int, c_ll = C.c_void_p, C.c_int, C.c_longlong
+c_void_p, c_int, c_uint, c_ll, c_double = C.c_void_p, C.c_int, C.c_uint, C.c_longlong, C.c_double
 
 ERRORS = {-1: "CUDA runtime error", -2: "bad argument", -3: "input exceeds a device-layout limit",
           -4: "device arena overflow"}
@@ -30,6 +30,106 @@ class Timings(C.Structure):
         return {n: getattr(self, n) for n, _ in self._fields_}
 
 
+class RunStats(C.Structure):
+    _fields_ = [(n, c_ll) for n in ("nkmers1", "nkmers2", "nseeds", "sumlen", "nhits", "nla", "nwaves",
+                                    "ncells", "nraw", "h2d_bytes", "d2h_bytes", "nseg", "nwork", "warp_cycles",
+                                    "wave_cycles", "extract_cycles", "us_gix", "us_seeds", "us_extend", "us_filter",
+                                    "nkmers1_fwd", "slow_cycles", "slow_waves", "paired_waves", "pairings",
+                                    "gix_waits")]
+
+    def asdict(self):
+        return {n: getattr(self, n) for n, _ in self._fields_}
+
+
+# (restype, argtypes) of every function of include/fastga_b200.h, set on the library once when it loads
+_H = C.POINTER(c_void_p)                    # a handle or device block handed out through an argument
+_LLP = C.POINTER(c_ll)
+_WHOLE = [c_int, c_int, c_int, c_int, c_double, _H, C.POINTER(RunStats), c_void_p]
+_GENOME = [c_void_p, c_ll, c_int, c_void_p, c_void_p]       # bps, bps_bytes, ncontig, clen, boff
+PROTOTYPES = {
+    "fgb_fastga": (c_int, _GENOME + [c_void_p] + _GENOME + _WHOLE),
+    "fgb_fastga_self": (c_int, _GENOME + [c_void_p] + _WHOLE),
+    "fgb_align_resident": (c_int, [c_void_p, c_void_p, c_void_p] + _WHOLE),
+    "fgb_genome_create": (c_int, _GENOME + [c_int, _H, c_void_p]),
+    "fgb_genome_free": (None, [c_void_p]),
+    "fgb_genome_perm": (c_int, [c_void_p, c_void_p]),
+    "fgb_genome_download": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
+    "fgb_genome_words": (c_ll, [c_void_p]),
+    "fgb_gix_build": (c_int, [c_void_p, _H, c_void_p]),
+    "fgb_gix_build_forward": (c_int, [c_void_p, _H, c_void_p]),
+    "fgb_gix_build_range": (c_int, [c_void_p, c_uint, c_uint, _H, c_void_p]),
+    "fgb_gix_upload": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, _H, c_void_p]),
+    "fgb_gix_import_ktab": (c_int, [c_void_p, c_ll, c_int, c_int, c_void_p, c_int, _H, c_void_p]),
+    "fgb_gix_export_ktab": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "fgb_gix_download": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fgb_gix_size": (c_ll, [c_void_p]),
+    "fgb_gix_post_bytes": (c_int, [c_void_p]),
+    "fgb_gix_cont_bytes": (c_int, [c_void_p]),
+    "fgb_gix_free": (None, [c_void_p]),
+    "fgb_seeds_find": (c_int, [c_void_p, c_void_p, c_ll, c_ll, c_int, _H, c_void_p]),
+    "fgb_seeds_find_self": (c_int, [c_void_p, c_ll, c_int, _H, c_void_p]),
+    "fgb_seeds_size": (c_ll, [c_void_p]),
+    "fgb_seeds_sumlen": (c_ll, [c_void_p]),
+    "fgb_seeds_layout": (c_int, [c_void_p, c_void_p]),
+    "fgb_seeds_download": (c_int, [c_void_p, c_void_p]),
+    "fgb_seeds_free": (None, [c_void_p]),
+    "fgb_align_spec": (c_int, [c_double, c_void_p, c_void_p, C.POINTER(c_int)]),
+    "fgb_extend": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_double, c_void_p, c_int, c_int, _H,
+                           c_void_p]),
+    "fgb_local_alignments": (c_int, [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                     c_void_p, c_ll, _LLP, c_void_p]),
+    "fgb_overlaps_from_buffer": (c_int, [c_void_p, c_ll, _H]),
+    "fgb_overlaps_bytes": (c_ll, [c_void_p]),
+    "fgb_overlaps_count": (c_ll, [c_void_p]),
+    "fgb_overlaps_data": (c_void_p, [c_void_p]),
+    "fgb_overlaps_counters": (None, [c_void_p, c_void_p]),
+    "fgb_overlaps_retry_info": (None, [c_void_p, c_void_p]),
+    "fgb_overlaps_free": (None, [c_void_p]),
+    "fgb_filter": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, _H]),
+    "fgb_alns_count": (c_ll, [c_void_p]),
+    "fgb_alns_raw_count": (c_ll, [c_void_p]),
+    "fgb_alns_pool_bytes": (c_ll, [c_void_p]),
+    "fgb_alns_get": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fgb_alns_free": (None, [c_void_p]),
+    "fgb_compute_trace_pts": (c_int, [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int, _H, c_void_p]),
+    "fgb_scripts_count": (c_ll, [c_void_p]),
+    "fgb_scripts_total": (c_ll, [c_void_p]),
+    "fgb_scripts_bad": (c_ll, [c_void_p]),
+    "fgb_scripts_get": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "fgb_scripts_free": (None, [c_void_p]),
+    "fgb_sort128_host": (c_int, [c_void_p, c_ll, c_int, c_int, c_void_p]),
+    "fgb_sort128_device": (c_int, [c_void_p, c_void_p, c_ll, c_int, c_int, c_void_p, c_ll, c_void_p, c_void_p]),
+    "fgb_sort128_tmp_bytes": (c_ll, [c_ll]),
+    "fgb_msd_sort": (None, [c_void_p, c_ll, c_int, c_int, c_void_p, c_int, c_int, c_int]),
+    "fgb_rmsd_sort": (c_int, [c_void_p, c_ll, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    "fgb_device_alloc": (c_int, [c_ll, _H, c_void_p]),
+    "fgb_device_free": (None, [c_void_p]),
+    "fgb_kmers_scan": (c_int, [c_void_p, c_void_p, c_int, _H, _LLP, c_void_p]),
+    "fgb_records_group_by_owner": (c_int, [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "fgb_gix_from_records": (c_int, [c_void_p, c_ll, c_uint, c_uint, c_int, c_int, c_int, c_int, _H, c_void_p]),
+    "fgb_seeds_merge": (c_int, [c_void_p, c_void_p, c_ll, c_ll, c_int, _H, _LLP, c_void_p, c_void_p, c_void_p]),
+    "fgb_seeds_group_by_owner": (c_int, [c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                         c_void_p]),
+    "fgb_seeds_from_records": (c_int, [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_ll, _H, c_void_p]),
+    "fgb_hit_groups_host": (c_ll, [c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_ll, c_ll, c_void_p,
+                                   c_void_p]),
+    "fgb_chain_hits": (c_int, [c_void_p, c_int, c_int, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p]),
+    "fgb_device_ready": (c_int, []),
+    "fgb_release_cache": (None, []),
+    "fgb_device_live_bytes": (c_ll, []),
+    "fgb_timings_reset": (None, []),
+    "fgb_timings_get": (None, [C.POINTER(Timings)]),
+    "fgb_host_waits": (c_ll, []),
+}
+
+
+def bind(L):
+    """sets the prototypes of PROTOTYPES on the loaded library L"""
+    for name, (restype, argtypes) in PROTOTYPES.items():
+        f = getattr(L, name)
+        f.restype, f.argtypes = restype, argtypes
+
+
 def _ptr(a):
     return a.ctypes.data_as(c_void_p)
 
@@ -41,7 +141,6 @@ def timings_reset():
 def host_waits():
     """host waits of the k-mer table builds so far (a counter)"""
     L = load_library()
-    L.fgb_host_waits.restype = c_ll
     return L.fgb_host_waits()
 
 
@@ -58,8 +157,6 @@ def device_ready():
 def device_live_bytes():
     """bytes of device blocks the library's block cache has handed out and not taken back"""
     L = load_library()
-    L.fgb_device_live_bytes.restype = c_ll
-    L.fgb_device_live_bytes.argtypes = []
     return L.fgb_device_live_bytes()
 
 
@@ -70,32 +167,25 @@ class DeviceGenome:
         L = load_library()
         self.genome = genome
         self.h = c_void_p()
-        L.fgb_genome_create.argtypes = [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_int,
-                                        C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_genome_create(_ptr(genome.bps), genome.bps.size, genome.ncontig,
                                    _ptr(genome.clen), _ptr(genome.boff), int(want_revcomp),
                                    C.byref(self.h), stream), "fgb_genome_create")
         self.perm = np.zeros(genome.ncontig, dtype=np.int32)
-        L.fgb_genome_perm.argtypes = [c_void_p, c_void_p]
         L.fgb_genome_perm(self.h, _ptr(self.perm))
         self.crank = np.empty_like(self.perm)
         self.crank[self.perm] = np.arange(genome.ncontig, dtype=np.int32)
 
     def download(self, rev=False):
         L = load_library()
-        L.fgb_genome_words.restype = c_ll
-        L.fgb_genome_words.argtypes = [c_void_p]
         n = L.fgb_genome_words(self.h)
         words = np.zeros(n, dtype=np.uint64)
         woff = np.zeros(self.genome.ncontig + 1, dtype=np.int64)
-        L.fgb_genome_download.argtypes = [c_void_p, c_int, c_void_p, c_void_p]
         _check(L.fgb_genome_download(self.h, int(rev), _ptr(words), _ptr(woff)), "fgb_genome_download")
         return words, woff
 
     def close(self):
         if self.h:
             L = load_library()
-            L.fgb_genome_free.argtypes = [c_void_p]
             L.fgb_genome_free(self.h)
             self.h = c_void_p()
 
@@ -116,7 +206,6 @@ class DeviceGix:
     def build(cls, dgenome, stream=None):
         L = load_library()
         h = c_void_p()
-        L.fgb_gix_build.argtypes = [c_void_p, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_gix_build(dgenome.h, C.byref(h), stream), "fgb_gix_build")
         return cls(h)
 
@@ -125,7 +214,6 @@ class DeviceGix:
         """forward-strand entries only (the adaptamer side of a merge)"""
         L = load_library()
         h = c_void_p()
-        L.fgb_gix_build_forward.argtypes = [c_void_p, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_gix_build_forward(dgenome.h, C.byref(h), stream), "fgb_gix_build_forward")
         return cls(h)
 
@@ -133,7 +221,6 @@ class DeviceGix:
     def build_range(cls, dgenome, plo, phi, stream=None):
         L = load_library()
         h = c_void_p()
-        L.fgb_gix_build_range.argtypes = [c_void_p, C.c_uint, C.c_uint, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_gix_build_range(dgenome.h, plo, phi, C.byref(h), stream), "fgb_gix_build_range")
         return cls(h)
 
@@ -142,7 +229,6 @@ class DeviceGix:
         L = load_library()
         h = c_void_p()
         tab = np.ascontiguousarray(tab, dtype=np.uint64).reshape(-1, 2)
-        L.fgb_gix_upload.argtypes = [c_void_p, c_ll, c_int, c_int, c_int, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_gix_upload(_ptr(tab), tab.shape[0], post_bytes, cont_bytes, ncontig,
                                 C.byref(h), stream), "fgb_gix_upload")
         return cls(h)
@@ -151,8 +237,6 @@ class DeviceGix:
     def import_ktab(cls, gixfile, stream=None):
         L = load_library()
         h = c_void_p()
-        L.fgb_gix_import_ktab.argtypes = [c_void_p, c_ll, c_int, c_int, c_void_p, c_int,
-                                          C.POINTER(c_void_p), c_void_p]
         ent = np.ascontiguousarray(gixfile.entries)
         idx = np.ascontiguousarray(gixfile.index, dtype=np.int64)
         _check(L.fgb_gix_import_ktab(_ptr(ent), gixfile.n, gixfile.post_bytes, gixfile.cont_bytes,
@@ -163,20 +247,16 @@ class DeviceGix:
     @property
     def n(self):
         L = load_library()
-        L.fgb_gix_size.restype = c_ll
-        L.fgb_gix_size.argtypes = [c_void_p]
         return L.fgb_gix_size(self.h)
 
     @property
     def post_bytes(self):
         L = load_library()
-        L.fgb_gix_post_bytes.argtypes = [c_void_p]
         return L.fgb_gix_post_bytes(self.h)
 
     @property
     def cont_bytes(self):
         L = load_library()
-        L.fgb_gix_cont_bytes.argtypes = [c_void_p]
         return L.fgb_gix_cont_bytes(self.h)
 
     def download(self, want_index=True):
@@ -185,7 +265,6 @@ class DeviceGix:
         tab = np.zeros((n, 2), dtype=np.uint64)
         pstart = np.zeros((1 << 24) + 1, dtype=np.uint32) if want_index else None
         buck = np.zeros(1024, dtype=np.uint64)
-        L.fgb_gix_download.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
         _check(L.fgb_gix_download(self.h, _ptr(tab), _ptr(pstart) if want_index else None, _ptr(buck)),
                "fgb_gix_download")
         return tab, pstart, buck
@@ -195,14 +274,12 @@ class DeviceGix:
         E = 9 + self.post_bytes + self.cont_bytes
         out = np.zeros(self.n * E, dtype=np.uint8)
         pf = np.ascontiguousarray(part_first, dtype=np.int64)
-        L.fgb_gix_export_ktab.argtypes = [c_void_p, c_void_p, c_int, c_void_p, c_void_p]
         _check(L.fgb_gix_export_ktab(self.h, _ptr(pf), len(pf), _ptr(out), stream), "fgb_gix_export_ktab")
         return out
 
     def close(self):
         if self.h:
             L = load_library()
-            L.fgb_gix_free.argtypes = [c_void_p]
             L.fgb_gix_free(self.h)
             self.h = c_void_p()
 
@@ -223,7 +300,6 @@ class DeviceSeeds:
     def find(cls, gix1, gix2, amxpos, bmxpos, freq=10, stream=None):
         L = load_library()
         h = c_void_p()
-        L.fgb_seeds_find.argtypes = [c_void_p, c_void_p, c_ll, c_ll, c_int, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_seeds_find(gix1.h, gix2.h, amxpos, bmxpos, freq, C.byref(h), stream), "fgb_seeds_find")
         return cls(h)
 
@@ -232,43 +308,35 @@ class DeviceSeeds:
         """SELF mode: the seeds of a genome's table against itself (gix from DeviceGix.build)"""
         L = load_library()
         h = c_void_p()
-        L.fgb_seeds_find_self.argtypes = [c_void_p, c_ll, c_int, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_seeds_find_self(gix.h, amxpos, freq, C.byref(h), stream), "fgb_seeds_find_self")
         return cls(h)
 
     @property
     def n(self):
         L = load_library()
-        L.fgb_seeds_size.restype = c_ll
-        L.fgb_seeds_size.argtypes = [c_void_p]
         return L.fgb_seeds_size(self.h)
 
     @property
     def sumlen(self):
         L = load_library()
-        L.fgb_seeds_sumlen.restype = c_ll
-        L.fgb_seeds_sumlen.argtypes = [c_void_p]
         return L.fgb_seeds_sumlen(self.h)
 
     @property
     def layout(self):
         L = load_library()
         bits = (c_int * 4)()
-        L.fgb_seeds_layout.argtypes = [c_void_p, c_void_p]
         L.fgb_seeds_layout(self.h, bits)
         return tuple(bits)
 
     def download(self):
         L = load_library()
         rec = np.zeros((self.n, 2), dtype=np.uint64)
-        L.fgb_seeds_download.argtypes = [c_void_p, c_void_p]
         _check(L.fgb_seeds_download(self.h, _ptr(rec)), "fgb_seeds_download")
         return rec
 
     def close(self):
         if self.h:
             L = load_library()
-            L.fgb_seeds_free.argtypes = [c_void_p]
             L.fgb_seeds_free(self.h)
             self.h = c_void_p()
 
@@ -283,13 +351,21 @@ def sort128_host(recs, byte_lo, byte_hi, stream=None):
     """In-place device sort of an (n,2) uint64 array of 128-bit records on key bytes [lo,hi)."""
     L = load_library()
     assert recs.dtype == np.uint64 and recs.flags.c_contiguous and recs.shape[1] == 2
-    L.fgb_sort128_host.argtypes = [c_void_p, c_ll, c_int, c_int, c_void_p]
     _check(L.fgb_sort128_host(_ptr(recs), recs.shape[0], byte_lo, byte_hi, stream), "fgb_sort128_host")
     return recs
 
 
-OVL_DT = np.dtype([("triple", "i4"), ("seq", "i4"), ("pairkey", "i4"), ("abpos", "i4"), ("bbpos", "i4"),
-                   ("aepos", "i4"), ("bepos", "i4"), ("diffs", "i4"), ("tlen", "i4"), ("toff", "i8")])
+# header of one raw alignment record of fgb_overlaps_data (ovl_hdr, fastga_b200/csrc/handles.h); the record's
+# trace of tlen bytes follows it, padded to 8 bytes
+RAW_HDR_DT = np.dtype([(n, "<i4") for n in ("triple", "seq", "pairkey", "abpos", "bbpos", "aepos", "bepos", "diffs",
+                                            "tlen", "launch")])
+# DeviceOverlaps.records(): the header fields but the launch, and where the trace starts in the buffer
+OVL_DT = np.dtype([(n, "i4") for n in RAW_HDR_DT.names[:-1]] + [("toff", "i8")])
+
+# the counters of fgb_overlaps_counters in export order (ext_counters, fastga_b200/csrc/handles.h)
+COUNTER_NAMES = ("hits", "la_calls", "waves", "cells", "front_wait", "nseg", "nwork", "front_total", "warp_cycles",
+                 "wave_cycles", "extract_cycles", "paired_waves", "pairings", "back_wait", "max_warp_cycles",
+                 "slowest_warp")
 
 
 def align_spec(ave_corr, freq):
@@ -298,7 +374,6 @@ def align_spec(ave_corr, freq):
     tables = np.zeros(65536, dtype=np.int16)
     ave = c_int()
     f = np.ascontiguousarray(freq, dtype=np.float32)
-    L.fgb_align_spec.argtypes = [C.c_double, c_void_p, c_void_p, C.POINTER(c_int)]
     _check(L.fgb_align_spec(float(ave_corr), _ptr(f), _ptr(tables), C.byref(ave)), "fgb_align_spec")
     return tables, ave.value
 
@@ -315,40 +390,30 @@ class DeviceOverlaps:
         L = load_library()
         tables, ave = align_spec(1.0 - align_rate, freq)
         h = c_void_p()
-        L.fgb_extend.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, C.c_double, c_void_p,
-                                 c_int, c_int, C.POINTER(c_void_p), c_void_p]
         _check(L.fgb_extend(seeds.h, dgenomeA.h, dgenomeB.h, chain_break, chain_min, align_min,
                             float(align_rate), _ptr(tables), ave, tspace, C.byref(h), stream), "fgb_extend")
         return cls(h)
 
     def counters(self):
         L = load_library()
-        out = (C.c_ulonglong * 16)()
-        L.fgb_overlaps_counters.argtypes = [c_void_p, c_void_p]
+        out = (C.c_ulonglong * len(COUNTER_NAMES))()
         L.fgb_overlaps_counters(self.h, out)
-        v = list(out)
-        return {"hits": v[0], "la_calls": v[1], "waves": v[2], "cells": v[3], "nseg": v[5], "nwork": v[6],
-                "warp_cycles": v[8], "wave_cycles": v[9], "extract_cycles": v[10], "paired_waves": v[11], "pairings": v[12],
-                "front_wait": v[4], "front_total": v[7], "back_wait": v[13],
-                "max_warp_cycles": v[14],
-                "slowest_warp": {"cycles": (v[15] >> 40) << 12, "waves": (v[15] >> 16) & 0xffffff, "la_calls": v[15] & 0xffff}}
+        c = dict(zip(COUNTER_NAMES, out))
+        v = c["slowest_warp"]
+        c["slowest_warp"] = {"cycles": (v >> 40) << 12, "waves": (v >> 16) & 0xffffff, "la_calls": v & 0xffff}
+        return c
 
     def retry_info(self):
         """how the extension's launches went: launches run, OR of 1 << ST_* failure reasons (2 band, 4 pebble
         arena, 8 trace staging, 16 hit-group numbering), record-buffer regrowths, triples re-run"""
         L = load_library()
         out = (C.c_longlong * 4)()
-        L.fgb_overlaps_retry_info.argtypes = [c_void_p, c_void_p]
         L.fgb_overlaps_retry_info(self.h, out)
         return {"launches": out[0], "reasons": out[1], "regrowths": out[2], "reruns": out[3]}
 
     def records(self):
         """(structured array sorted in reference discovery order, trace byte pool)"""
         L = load_library()
-        L.fgb_overlaps_bytes.restype = c_ll
-        L.fgb_overlaps_bytes.argtypes = [c_void_p]
-        L.fgb_overlaps_data.restype = c_void_p
-        L.fgb_overlaps_data.argtypes = [c_void_p]
         nb = L.fgb_overlaps_bytes(self.h)
         if nb == 0:
             return np.zeros(0, dtype=OVL_DT), np.zeros(0, dtype=np.uint8)
@@ -356,9 +421,9 @@ class DeviceOverlaps:
         recs = []
         off = 0
         while off < nb:
-            h = np.frombuffer(buf[off:off + 40].tobytes(), dtype=np.int32)
-            recs.append((h[0], h[1], h[2], h[3], h[4], h[5], h[6], h[7], h[8], off + 40))
-            off += 40 + ((int(h[8]) + 7) & ~7)
+            h = np.frombuffer(buf, RAW_HDR_DT, 1, off)[0]
+            recs.append(tuple(h[n] for n in OVL_DT.names[:-1]) + (off + RAW_HDR_DT.itemsize,))
+            off += RAW_HDR_DT.itemsize + ((int(h["tlen"]) + 7) & ~7)
         arr = np.array(recs, dtype=OVL_DT)
         order = np.lexsort((arr["seq"], arr["triple"]))
         return arr[order], buf
@@ -366,7 +431,6 @@ class DeviceOverlaps:
     def close(self):
         if self.h:
             L = load_library()
-            L.fgb_overlaps_free.argtypes = [c_void_p]
             L.fgb_overlaps_free(self.h)
             self.h = c_void_p()
 
@@ -419,7 +483,6 @@ def filter_overlaps(ovl_handle, perm1, perm2, jc_bits, ic_bits, do_filter=True):
     h = c_void_p()
     p1 = np.ascontiguousarray(perm1, dtype=np.int32)
     p2 = np.ascontiguousarray(perm2, dtype=np.int32)
-    L.fgb_filter.argtypes = [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, C.POINTER(c_void_p)]
     _check(L.fgb_filter(ovl_handle, _ptr(p1), _ptr(p2), jc_bits, ic_bits, int(do_filter), C.byref(h)),
            "fgb_filter")
     return _alns_out(h)
@@ -429,20 +492,8 @@ def overlaps_from_buffer(buf):
     L = load_library()
     h = c_void_p()
     buf = np.ascontiguousarray(buf, dtype=np.uint8)
-    L.fgb_overlaps_from_buffer.argtypes = [c_void_p, c_ll, C.POINTER(c_void_p)]
     _check(L.fgb_overlaps_from_buffer(_ptr(buf), buf.size, C.byref(h)), "fgb_overlaps_from_buffer")
     return DeviceOverlaps(h)
-
-
-class RunStats(C.Structure):
-    _fields_ = [(n, c_ll) for n in ("nkmers1", "nkmers2", "nseeds", "sumlen", "nhits", "nla", "nwaves",
-                                    "ncells", "nraw", "h2d_bytes", "d2h_bytes", "nseg", "nwork", "warp_cycles",
-                                    "wave_cycles", "extract_cycles", "us_gix", "us_seeds", "us_extend", "us_filter",
-                                    "nkmers1_fwd", "slow_cycles", "slow_waves", "paired_waves", "pairings",
-                                    "gix_waits")]
-
-    def asdict(self):
-        return {n: getattr(self, n) for n, _ in self._fields_}
 
 
 DEFAULTS = dict(freq=10, chain_break=2000, chain_min=170, align_min=100, align_rate=0.3)
@@ -450,31 +501,23 @@ DEFAULTS = dict(freq=10, chain_break=2000, chain_min=170, align_min=100, align_r
 
 def _alns_out(h):
     L = load_library()
-    for f in ("fgb_alns_count", "fgb_alns_raw_count", "fgb_alns_pool_bytes"):
-        getattr(L, f).restype = c_ll
-        getattr(L, f).argtypes = [c_void_p]
     n, nraw, pb = L.fgb_alns_count(h), L.fgb_alns_raw_count(h), L.fgb_alns_pool_bytes(h)
     fields = np.zeros((n, 9), dtype=np.int32)
     toff = np.zeros(n, dtype=np.int64)
     pool = np.zeros(max(pb, 1), dtype=np.uint8)
-    L.fgb_alns_get.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
     _check(L.fgb_alns_get(h, _ptr(fields), _ptr(toff), _ptr(pool)), "fgb_alns_get")
-    L.fgb_alns_free.argtypes = [c_void_p]
     L.fgb_alns_free(h)
     return Alignments(fields, toff, pool, nraw)
 
 
-def _whole_path(name, argtypes, args, stream, kw):
+def _whole_path(name, args, stream, kw):
     """calls the whole-path entry point `name` on args + the DEFAULTS-merged parameters -> (Alignments, stats)"""
     p = dict(DEFAULTS)
     p.update(kw)
     L = load_library()
     h = c_void_p()
     st = RunStats()
-    fn = getattr(L, name)
-    fn.argtypes = argtypes + [c_int, c_int, c_int, c_int, C.c_double, C.POINTER(c_void_p), C.POINTER(RunStats),
-                              c_void_p]
-    _check(fn(*args, p["freq"], p["chain_break"], p["chain_min"], p["align_min"], float(p["align_rate"]),
+    _check(getattr(L, name)(*args, p["freq"], p["chain_break"], p["chain_min"], p["align_min"], float(p["align_rate"]),
               C.byref(h), C.byref(st), stream), name)
     return _alns_out(h), st.asdict()
 
@@ -482,22 +525,19 @@ def _whole_path(name, argtypes, args, stream, kw):
 def align_resident(dA, dB, freqA, stream=None, **kw):
     """Whole path from device-resident genomes: returns (Alignments, stats dict)"""
     f = np.ascontiguousarray(freqA, dtype=np.float32)
-    return _whole_path("fgb_align_resident", [c_void_p, c_void_p, c_void_p], (dA.h, dB.h, _ptr(f)), stream, kw)
+    return _whole_path("fgb_align_resident", (dA.h, dB.h, _ptr(f)), stream, kw)
 
 
 def fastga_self(g, stream=None, **kw):
     """SELF mode, `FastGA A` with one source (formats.Genome) -> (Alignments, stats)"""
     f = np.ascontiguousarray(g.freq, dtype=np.float32)
-    return _whole_path("fgb_fastga_self", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p],
-                       (_ptr(g.bps), g.bps.size, g.ncontig, _ptr(g.clen), _ptr(g.boff), _ptr(f)), stream, kw)
+    return _whole_path("fgb_fastga_self", (_ptr(g.bps), g.bps.size, g.ncontig, _ptr(g.clen), _ptr(g.boff), _ptr(f)), stream, kw)
 
 
 def fastga(gA, gB, stream=None, **kw):
     """The reference-facing call on host buffers (formats.Genome x2) -> (Alignments, stats)"""
     f = np.ascontiguousarray(gA.freq, dtype=np.float32)
-    return _whole_path("fgb_fastga", [c_void_p, c_ll, c_int, c_void_p, c_void_p, c_void_p,
-                                      c_void_p, c_ll, c_int, c_void_p, c_void_p],
-                       (_ptr(gA.bps), gA.bps.size, gA.ncontig, _ptr(gA.clen), _ptr(gA.boff), _ptr(f),
+    return _whole_path("fgb_fastga", (_ptr(gA.bps), gA.bps.size, gA.ncontig, _ptr(gA.clen), _ptr(gA.boff), _ptr(f),
                         _ptr(gB.bps), gB.bps.size, gB.ncontig, _ptr(gB.clen), _ptr(gB.boff)), stream, kw)
 
 
@@ -512,22 +552,14 @@ def compute_trace_pts(dA, dB, alns, tspace=100, stream=None, with_bad=False):
     fields = np.ascontiguousarray(alns.fields, dtype=np.int32)
     toff = np.ascontiguousarray(alns.toff, dtype=np.int64)
     pool = np.ascontiguousarray(alns.pool, dtype=np.uint8)
-    L.fgb_compute_trace_pts.argtypes = [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_void_p, c_int,
-                                        C.POINTER(c_void_p), c_void_p]
     _check(L.fgb_compute_trace_pts(dA.h, dB.h, len(alns), _ptr(fields), _ptr(toff), _ptr(pool), tspace,
                                    C.byref(h), stream), "fgb_compute_trace_pts")
-    L.fgb_scripts_total.restype = c_ll
-    L.fgb_scripts_total.argtypes = [c_void_p]
     n, tot = len(alns), L.fgb_scripts_total(h)
     soff = np.zeros(n + 1, dtype=np.int64)
     script = np.zeros(max(tot, 1), dtype=np.int32)
     diffs = np.zeros(max(n, 1), dtype=np.int32)
-    L.fgb_scripts_get.argtypes = [c_void_p, c_void_p, c_void_p, c_void_p]
     _check(L.fgb_scripts_get(h, _ptr(soff), _ptr(script), _ptr(diffs)), "fgb_scripts_get")
-    L.fgb_scripts_bad.restype = c_ll
-    L.fgb_scripts_bad.argtypes = [c_void_p]
     bad = L.fgb_scripts_bad(h)
-    L.fgb_scripts_free.argtypes = [c_void_p]
     L.fgb_scripts_free(h)
     return (soff, script[:tot], diffs[:n]) + ((bad,) if with_bad else ())
 
@@ -546,8 +578,6 @@ def hit_groups_host(hrange, tinfo, hits, bands=1, slack=1000, gap=-1):
     cap = len(hh) + len(hr) + 1
     items = np.zeros((cap, 4), dtype=np.uint32)
     nxt = np.zeros((cap, 2), dtype=np.int64)
-    L.fgb_hit_groups_host.restype = c_ll
-    L.fgb_hit_groups_host.argtypes = [c_int, c_void_p, c_void_p, c_void_p, c_ll, c_int, c_ll, c_ll, c_void_p, c_void_p]
     n = L.fgb_hit_groups_host(len(hr), _ptr(hr), _ptr(ti), _ptr(hh), len(hh), bands, slack, gap, _ptr(items), _ptr(nxt))
     return items[:n].copy(), nxt[:n].copy()
 
@@ -565,7 +595,6 @@ def chain_hits(seeds, chain_break=2000, chain_min=170, chunk=None, stream=None):
     bit 31 (CHAIN_LISTLESS: scanned in the extension kernel); hits: (alow, ahgh, dgmin, dgmax) per slot;
     info: dict of the counts (work triples, long triples, hit slots, slots reserved, capacity, chunks)."""
     L = load_library()
-    L.fgb_chain_hits.argtypes = [c_void_p, c_int, c_int, c_ll, c_void_p, c_ll, c_void_p, c_ll, c_void_p, c_void_p]
     chunk = 1536 if chunk is None else int(chunk)
     info = np.zeros(6, dtype=np.int64)
     trip = np.zeros(1, dtype=CHAIN_TRIPLE_DT)
@@ -584,7 +613,6 @@ def chain_hits(seeds, chain_break=2000, chain_min=170, chunk=None, stream=None):
 
 def device_free(ptr):
     L = load_library()
-    L.fgb_device_free.argtypes = [c_void_p]
     L.fgb_device_free(c_void_p(ptr))
 
 
@@ -593,7 +621,6 @@ def kmers_scan(dgenome, mask, fwd_only, stream=None):
     L = load_library()
     ptr, n = c_void_p(), c_ll()
     m = np.ascontiguousarray(mask, dtype=np.uint8)
-    L.fgb_kmers_scan.argtypes = [c_void_p, c_void_p, c_int, C.POINTER(c_void_p), C.POINTER(c_ll), c_void_p]
     _check(L.fgb_kmers_scan(dgenome.h, _ptr(m), int(fwd_only), C.byref(ptr), C.byref(n), stream), "fgb_kmers_scan")
     return ptr.value, n.value
 
@@ -605,7 +632,6 @@ def records_group_by_owner(src_ptr, n, owner256, world, dst_ptr, stream=None):
     bounds = np.zeros(world + 1, dtype=np.int64)
     own = np.ascontiguousarray(owner256, dtype=np.int32)
     assert own.shape == (256,)
-    L.fgb_records_group_by_owner.argtypes = [c_void_p, c_ll, c_void_p, c_int, c_void_p, c_void_p, c_void_p]
     _check(L.fgb_records_group_by_owner(c_void_p(src_ptr), n, _ptr(own), world, c_void_p(dst_ptr), _ptr(bounds),
                                         stream), "fgb_records_group_by_owner")
     return bounds
@@ -614,8 +640,6 @@ def records_group_by_owner(src_ptr, n, owner256, world, dst_ptr, stream=None):
 def gix_from_records(ptr, n, plo, phi, fwd_only, post_bytes, cont_bytes, ncontig, stream=None):
     L = load_library()
     h = c_void_p()
-    L.fgb_gix_from_records.argtypes = [c_void_p, c_ll, C.c_uint, C.c_uint, c_int, c_int, c_int, c_int,
-                                       C.POINTER(c_void_p), c_void_p]
     _check(L.fgb_gix_from_records(c_void_p(ptr), n, plo, phi, int(fwd_only), post_bytes, cont_bytes, ncontig,
                                   C.byref(h), stream), "fgb_gix_from_records")
     return DeviceGix(h)
@@ -627,8 +651,6 @@ def seeds_merge(gix1, gix2, amxpos, bmxpos, freq=10, stream=None):
     ptr, n = c_void_p(), c_ll()
     bits = (c_int * 4)()
     info = (c_ll * 2)()
-    L.fgb_seeds_merge.argtypes = [c_void_p, c_void_p, c_ll, c_ll, c_int, C.POINTER(c_void_p), C.POINTER(c_ll),
-                                  c_void_p, c_void_p, c_void_p]
     _check(L.fgb_seeds_merge(gix1.h, gix2.h, amxpos, bmxpos, freq, C.byref(ptr), C.byref(n), bits, info, stream),
            "fgb_seeds_merge")
     return ptr.value, n.value, tuple(bits), info[0], info[1]
@@ -639,7 +661,6 @@ def seeds_group_by_owner(src_ptr, n, bits, owner_by_rank, world, dst_ptr, stream
     bounds = np.zeros(world + 1, dtype=np.int64)
     b = (c_int * 4)(*bits)
     ow = np.ascontiguousarray(owner_by_rank, dtype=np.int32)
-    L.fgb_seeds_group_by_owner.argtypes = [c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]
     _check(L.fgb_seeds_group_by_owner(c_void_p(src_ptr), n, b, _ptr(ow), len(ow), world, c_void_p(dst_ptr),
                                       _ptr(bounds), stream), "fgb_seeds_group_by_owner")
     return bounds
@@ -649,7 +670,6 @@ def seeds_from_records(ptr, n, bits, amxpos, bmxpos, sumlen=0, stream=None):
     L = load_library()
     h = c_void_p()
     b = (c_int * 4)(*bits)
-    L.fgb_seeds_from_records.argtypes = [c_void_p, c_ll, c_void_p, c_ll, c_ll, c_ll, C.POINTER(c_void_p), c_void_p]
     _check(L.fgb_seeds_from_records(c_void_p(ptr), n, b, amxpos, bmxpos, sumlen, C.byref(h), stream),
            "fgb_seeds_from_records")
     return DeviceSeeds(h)
@@ -665,8 +685,6 @@ def local_alignments(dA, dB, jobs, freq, align_rate=0.3, tspace=100, stream=None
     paths = np.zeros((max(n, 1), 7), dtype=np.int32)
     toff = np.zeros(max(n, 1), dtype=np.int64)
     cap = 1 << 20
-    L.fgb_local_alignments.argtypes = [c_void_p, c_void_p, c_ll, c_void_p, c_void_p, c_int, c_int,
-                                       c_void_p, c_void_p, c_void_p, c_ll, C.POINTER(c_ll), c_void_p]
     while True:
         traces = np.zeros(cap, dtype=np.uint8)
         used = c_ll()

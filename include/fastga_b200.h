@@ -50,6 +50,7 @@ typedef struct
             gix_waits;                                   /* host waits of the two table builds, scan to merge launch */
 } fgb_run_stats;
 
+/* device milliseconds per stage (CUDA events on the call's stream) and kernel launches, summed over calls */
 typedef struct
 { float h2d_ms, stage_ms, scan_ms, ksort_ms, index_ms, merge_ms, ssort_ms, triples_ms, extend_ms,
         d2h_ms, filter_ms;
@@ -153,6 +154,7 @@ int  fgb_overlaps_from_buffer(const unsigned char *buf, long long nbytes, fgb_ov
 long long fgb_overlaps_bytes(const fgb_overlaps *o);
 long long fgb_overlaps_count(const fgb_overlaps *o);
 const unsigned char *fgb_overlaps_data(const fgb_overlaps *o);
+/* out: 16 counters, the fields of struct ext_counters (fastga_b200/csrc/handles.h) in order */
 void fgb_overlaps_counters(const fgb_overlaps *o, unsigned long long *out /* 16 */);
 /* how fgb_extend's launches went: out[0] extension launches run (repeats included), out[1] the OR over
  * them of 1 << ST_* of the items that failed (2 band too wide, 4 pebble arena full, 8 trace staging

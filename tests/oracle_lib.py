@@ -508,8 +508,10 @@ def pack_overlaps(ov, tp, rank1, rank2, jb, ib):
     parts = []
     for i, r in enumerate(ov):
         pk = (int(r["comp"]) << (jb + ib)) | (int(rank1[r["aread"]]) << jb) | int(rank2[r["bread"]])
-        h = np.array([i, 0, pk, r["abpos"], r["bbpos"], r["aepos"], r["bepos"], r["diffs"], r["tlen"], 0],
-                     dtype=np.int32)
+        h = np.zeros(1, dtype=lib.RAW_HDR_DT)
+        h["triple"], h["pairkey"] = i, pk
+        for f in ("abpos", "bbpos", "aepos", "bepos", "diffs", "tlen"):
+            h[f] = r[f]
         tr = bytes(tp[int(r["toff"]):int(r["toff"]) + int(r["tlen"])])
         tr += b"\0" * ((-len(tr)) % 8)
         parts.append(h.tobytes())

@@ -234,9 +234,6 @@ def _raw_local_alignments(dA, dB, jobs, freq, align_rate, traces_cap):
     traces = np.zeros(max(traces_cap, 1), dtype=np.uint8)
     used = C.c_longlong()
     L = load_library()
-    L.fgb_local_alignments.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int,
-                                       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
-                                       C.POINTER(C.c_longlong), C.c_void_p]
     rc = L.fgb_local_alignments(dA.h, dB.h, n, jobs.ctypes.data, tables.ctypes.data, ave, 100, paths.ctypes.data,
                                 toff.ctypes.data, traces.ctypes.data, traces_cap, C.byref(used), None)
     return rc, used.value

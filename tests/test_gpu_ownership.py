@@ -18,7 +18,6 @@ def live():
 def device_alloc(nbytes):
     L = load_library()
     p = C.c_void_p()
-    L.fgb_device_alloc.argtypes = [C.c_longlong, C.POINTER(C.c_void_p), C.c_void_p]
     assert L.fgb_device_alloc(nbytes, C.byref(p), None) == 0
     return p.value
 
@@ -121,7 +120,6 @@ def test_stage_calls_leave_no_live_blocks(small_pair):
     arr = np.concatenate([rng.integers(0, 256, n * rsize, dtype=np.uint8), np.zeros(16, np.uint8)])
     part = np.zeros(1024, dtype=np.int64)
     part[beg:end] = counts * rsize
-    L.fgb_msd_sort.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.fgb_msd_sort(arr.ctypes.data, n, rsize, ksize, part.ctypes.data, beg, end, 4)
     assert live() == base
 
@@ -131,7 +129,6 @@ def test_stage_calls_leave_no_live_blocks(small_pair):
     arr = rng.integers(0, 256, n * rsize, dtype=np.uint8)
     part = (counts * rsize).astype(np.int64)
     ranges = (_Range * nthreads)()
-    L.fgb_rmsd_sort.argtypes = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
     assert L.fgb_rmsd_sort(arr.ctypes.data, n, rsize, rsize, nparts, part.ctypes.data, nthreads, ranges) > 0
     assert live() == base
 
@@ -164,8 +161,6 @@ def test_seed_sort_refusal_releases_its_blocks():
     d = torch.from_numpy(recs.view(np.int64).copy()).cuda()
     torch.cuda.synchronize()
     L = load_library()
-    L.fgb_seeds_from_records.argtypes = [C.c_void_p, C.c_longlong, C.c_void_p, C.c_longlong, C.c_longlong,
-                                         C.c_longlong, C.POINTER(C.c_void_p), C.c_void_p]
     bits = (C.c_int * 4)(25, 19, 3, 3)                  # key of 63 bits
     h = C.c_void_p()
     base = live()
@@ -182,9 +177,6 @@ def test_local_alignments_overflow_releases_its_blocks(monkeypatch):
     dA, dB = lib.DeviceGenome(gA, want_revcomp=True), lib.DeviceGenome(gB)
     tables, ave = lib.align_spec(0.7, gA.freq)
     L = load_library()
-    L.fgb_local_alignments.argtypes = [C.c_void_p, C.c_void_p, C.c_longlong, C.c_void_p, C.c_void_p, C.c_int,
-                                       C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong,
-                                       C.POINTER(C.c_longlong), C.c_void_p]
 
     def call(jobs):
         n = jobs.shape[0]

@@ -270,7 +270,7 @@ def _msd_case(rsize):
     arr[:, 3:9] &= 0x03                              # few distinct keys -> long equal runs and LCPs
     part = np.zeros(1024, dtype=np.int64)
     part[beg:end] = counts * rsize
-    argt = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int]
+    argt = lib.PROTOTYPES["fgb_msd_sort"][1]         # msd_sort's own signature
 
     def canon(r):                                    # payloads: same multiset per equal-key run
         run = np.cumsum(r[:, 0] != 0)
@@ -318,7 +318,7 @@ def _rmsd_case(rsize, nparts):
     arr = rng.integers(0, 256, (n, rsize), dtype=np.uint8)
     arr[:, 5:] &= 0x07
     part = (counts * rsize).astype(np.int64)
-    argt = [C.c_void_p, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
+    argt = lib.PROTOTYPES["fgb_rmsd_sort"][1]        # rmsd_sort's own signature
 
     def sort(f):
         a, p = arr.reshape(-1).copy(), (_Range * nthreads)()

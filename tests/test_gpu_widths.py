@@ -112,8 +112,6 @@ def test_narrow_and_wide_seed_sorts_give_identical_handles_at_64_bit_keys(staged
 
 def _genome_create(nc, clen, bps):
     L = load_library()
-    L.fgb_genome_create.argtypes = [C.c_void_p, C.c_longlong, C.c_int, C.c_void_p, C.c_void_p, C.c_int,
-                                    C.POINTER(C.c_void_p), C.c_void_p]
     clen = np.ascontiguousarray(clen, dtype=np.int64)
     boff = np.zeros(len(clen), dtype=np.int64)
     h = C.c_void_p()
