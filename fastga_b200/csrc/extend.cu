@@ -15,7 +15,7 @@
 //   * a triple without a hit list is scanned warp-parallel on the front warp (32 merged seeds per step);
 //   * a wave is data-parallel over its diagonals.  While the band fits a warp the state
 //     (V, T, HA, HM, NA) lives in registers of the lane owning the diagonal and the pass is split
-//     between the front warp (V recurrence, snake, band trim) and the back warps (bit-vectors, trim
+//     between the front warp (V recurrence, snake, band trim) and the T and P warps (bit-vectors, trim
 //     tests, pebbles) through a ring in shared memory (struct PairBox); wider or bordered bands run
 //     on the front warp alone, in 32-diagonal chunks over circular arrays in shared memory / HBM;
 //   * the running maxima besta/lasta/trim* (strict '>' in descending-k order) are reproduced
@@ -118,29 +118,24 @@ struct Ctx
   unsigned char *fstage, *rstage; int smax;
   int tspace, path_ave; const short *score, *table; const short *ttab; int sc15;
   u64 nwaves, ncells, cyc_wave, cyc_extract, pwaves, npairs, fwait, ftot, bwait, btot;
-  struct PairBox *box;                   // front/back warp pair mailbox (NULL: this warp runs waves alone)
+  struct PairBox *box;                   // mailbox of the warp team (NULL: this warp runs waves alone)
   unsigned box_off;                      //   and its offset inside the dynamic shared memory
   Peb *pwin; int pwin_n;                 // pwin_n pebbles of shared memory: the window of the trace read-out
 };
 
-//  Front/back pairing of a wave pass.  The recurrence that makes a pass serial is only the
+//  The warp team of a wave pass.  The recurrence that makes a pass serial is only the
 //  furthest-point recurrence V (three-way max + snake) and the band trim that follows from it;
 //  the match bit-vectors, the trim-point tests and the trace pebbles hang off it without feeding
-//  back, except for the loop's stop test.  So a pass is split over two warps of a block: the FRONT
-//  warp runs V and the band, and streams each wave (the 32 new V values + a header) through a ring
-//  in shared memory; the BACK warp replays the predecessor choice from the V values, carries
-//  T / HA / HM / NA in its registers, tests trim points, drops pebbles, and raises `stop` when
-//  lasta falls TRIM_MLAG behind.  The front may run ahead by at most EX_RING waves; what it
-//  computes past the stop wave is discarded.  Anything unusual (band wider than 31 diagonals,
-//  a wave that does not advance the best point, an empty band) is handed back: the back warp
-//  spills its state and the front warp finishes the pass alone on the code below.
+//  back, except for the loop's stop test.  So a pass is split over the three warps of a team: the
+//  front warp runs V and the band, and streams each wave (the 32 new V values + a header) through a
+//  ring in shared memory; the T warp carries the match bit-vectors, tests trim points and raises
+//  `stop` when lasta falls TRIM_MLAG behind; the P warp, one or more waves behind it, carries
+//  HA / HM / NA, drops pebbles and picks up the pebble head of every trim point the T warp announces
+//  (tring).  Both replay the predecessor choice from consecutive V's.  The front may run ahead by at
+//  most EX_RING waves; what it computes past the stop wave is discarded.  Anything unusual (band
+//  wider than 31 diagonals, a wave that does not advance the best point, an empty band) is handed
+//  back: the T and P warps spill their state and the front warp finishes the pass alone in wave.
 
-#ifndef EX_PAIR
-#define EX_PAIR 1
-#endif
-#ifndef EX_NOREG
-#define EX_NOREG 0                       // 1 (debug): never use the register path of the single-warp waves
-#endif
 #define EX_RING 32
 #define EX_TILEW 256                     // 32-bit words per staged sequence tile: 4096 bases
 #define EX_TILEB (16*EX_TILEW)
@@ -205,7 +200,7 @@ struct PebWalk
 //  THIS symbol, so the compiler knows the state space (LDS/STS instead of generic loads).
 extern __shared__ __align__(16) unsigned char ex_smem[];
 
-//  flag hand-off between the two warps of a pair: release store (fence + STS) / acquire load (LDS)
+//  flag hand-off between the warps of a team: release store (fence + STS) / acquire load (LDS)
 static __device__ __forceinline__ void st_release_smem(volatile int *p, int v)
 { asm volatile("st.release.cta.shared.b32 [%0], %1;" :: "r"(smem_u32((const void *) p)), "r"(v) : "memory"); }
 static __device__ __forceinline__ int ld_acquire_smem_a(unsigned a)          // a = shared-window address
@@ -325,15 +320,141 @@ static __device__ __forceinline__ int warp_prefix_max_excl(int v, int lane)
 
 static __device__ __forceinline__ unsigned rotr32(unsigned x, int r) { return __funnelshift_r(x,x,r); }
 
-//  BACK warp of a pair: one wave pass (direction s) from the state the front warp left after
-//  wave 0.  Returns when the pass is finished (stop = 1) or handed back (stop = 2).
+//  The steps of a wave, one definition each for the register path, the 32-diagonal chunks and wave 0
+//  of the single-warp waves (wave).  Masks over a band come in position order, bit p = diagonal
+//  top-p: a ballot of the register band is rotated by ltop = (-top) & 31 (see owner_diag); lane
+//  order, as in the chunks (kk = top - lane), is ltop = 0.  The three warps of a team (front_run,
+//  wave_T, wave_P) keep their own copies of these steps: they run the critical item of a launch, and
+//  built on these helpers the extension kernel ran 3 % slower (same results; H100 80GB HBM3, 700 W).
 
-//  The BACK of a pass is two warps.  Both replay the predecessor choice from consecutive V's (two
-//  shuffles); the T warp carries the match bit-vectors, tests trim points and decides when the pass
-//  stops; the P warp, one or more waves behind it, carries the pebble lists (HA / HM / NA), drops
-//  pebbles and picks up the pebble head of every trim point the T warp announces (tring).  Per wave
-//  each executes about half of what one back warp did, and the wave rate of a pass is set by the
-//  slowest of the three warps.
+//  The diagonal lane owns in a register band topped by top: lane = -kk mod 32, fixed for a whole pass.
+static __device__ __forceinline__ int owner_diag(const int top, const int lane) { return top - ((top + lane) & 31); }
+
+//  The register band <-> the wave arrays (index kk & wmask): the state (V, T, HA, HM, NA) of
+//  diagonal kk, stored when it is in the band.
+static __device__ __forceinline__ void spill(const int kk, const bool in, const int wmask, int *V, u64 *T,
+                                             int *HA, int *HM, int *NA, const int rV, const u64 rT,
+                                             const int rHA, const int rHM, const int rNA)
+{ if (!in) return;
+  const int ix = kk & wmask;
+  V[ix] = rV; T[ix] = rT; HA[ix] = rHA; HM[ix] = rHM; NA[ix] = rNA;
+}
+static __device__ __forceinline__ void load(const int kk, const int wmask, const int *V, const u64 *T,
+                                            const int *HA, const int *HM, const int *NA,
+                                            int &rV, u64 &rT, int &rHA, int &rHM, int &rNA)
+{ const int ix = kk & wmask;
+  rV = V[ix]; rT = T[ix]; rHA = HA[ix]; rHM = HM[ix]; rNA = NA[ix];
+}
+
+//  Predecessor of a diagonal (align.c:634-676 / :1154-1198) from the furthest points of the diagonals
+//  above (ap), itself (ac) and below (am): pred 1 = kk+1, -1 = kk-1, 0 = kk; ties go to kk, then kk-1.
+//  cc = the anti-diagonal the step from it reaches.
+static __device__ __forceinline__ int pred_choice(const int ap, const int ac, const int am, int &cc)
+{ int pred;
+  if (ap > max(ac,am)) { pred = 1;  cc = ap+1; }
+  else if (am > ac)    { pred = -1; cc = am+1; }
+  else                 { pred = 0;  cc = ac+2; }
+  return pred;
+}
+
+//  Match bit-vector of the last 64 columns after the step (a difference: 0) and a slide over t
+//  matches (align.c:677-702 / :1197-1222)
+static __device__ __forceinline__ u64 shift_matches(u64 b, const int t)
+{ b <<= 1;
+  return (t >= 64) ? ~0ull : ((b << t) | ((1ull << t) - 1));
+}
+
+//  Pebbles of the trace points a slide to xn crossed (align.c:704-728 / :1224-1248): one cell per
+//  crossing past the chain head's mark hm, allocated by ballot from the warp's arena, appended to the
+//  chain ha; nan moves past xn.  false: the arena is full (nothing of the crossing was dropped).
+template<int s>
+static __device__ __forceinline__ bool drop_pebbles(Peb *cells, int &avail, const int cmax, const int tspace,
+                                                    const unsigned lt, const bool act, const int xn,
+                                                    const int kk, const int diff, int &ha, int &hm, int &nan)
+{ bool need = act && xn >= nan;
+  while (__any_sync(FULL,need))
+    { const bool create = need && (s*hm < nan);
+      if (avail + 32 > cmax) return false;
+      const unsigned m = __ballot_sync(FULL,create);
+      const int idx = avail + __popc(m & lt);
+      avail += __popc(m);
+      if (create)
+        { Peb p; p.ptr = ha; p.diag = s*kk; p.diff = diff; p.mark = s*nan;
+          cells[idx] = p;
+          ha = idx; hm = s*nan;
+        }
+      if (need) nan += tspace;
+      need = act && xn >= nan;
+    }
+  return true;
+}
+
+//  Best point, lasta and trim point of a wave whose maximum mx beats besta (align.c:730-750 /
+//  :1250-1270): the running maxima of the reference's scan in descending kk, strict '>'.  Lb, the
+//  highest diagonal reaching mx, is the scan's last record setter: when it passes the path and trim
+//  tests it alone decides (one shuffle); otherwise a prefix max over the band finds the last record
+//  setters that pass them.  Sets besta = mx and bestx; returns the lane of the new trim point (trima,
+//  trimx set, trimd = dif), or -1.
+template<class CX>
+static __device__ __forceinline__ int best_update(const CX &c, const int path_ave, const int ltop, const int lane,
+                                                  const bool act, const int cc, const int xn, const u64 b,
+                                                  const int mx, const int dif, int &besta, int &bestx,
+                                                  int &lasta, int &trima, int &trimx, int &trimd)
+{ const int cm = act ? cc : INT_MIN;
+  const unsigned eq = rotr32(__ballot_sync(FULL,cm == mx),ltop);
+  const int Lb = (ltop + __ffs(eq) - 1) & 31;
+  const bool qual = act && cc > besta && __popcll(b & PATH_WIN) >= path_ave;
+  const bool tq = qual && trim_ok(c,b);
+  int tlane = -1;
+  bestx = __shfl_sync(FULL,xn,Lb);
+  if (__shfl_sync(FULL,(int) tq,Lb))
+    { lasta = trima = mx; trimx = bestx; trimd = dif;
+      tlane = Lb;
+    }
+  else
+    { const unsigned ql = __ballot_sync(FULL,qual), tl = __ballot_sync(FULL,tq);
+      const int cpos = __shfl_sync(FULL,cm,(ltop + lane) & 31);       // value at position = lane
+      const int ex = max(warp_prefix_max_excl(cpos,lane),besta);
+      const unsigned rm = __ballot_sync(FULL,cpos > ex);
+      const unsigned qm = rm & rotr32(ql,ltop), tm = rm & rotr32(tl,ltop);
+      if (qm) lasta = __shfl_sync(FULL,cc,(ltop + 31 - __clz(qm)) & 31);
+      if (tm)
+        { tlane = (ltop + 31 - __clz(tm)) & 31;
+          trima = __shfl_sync(FULL,cc,tlane);
+          trimx = __shfl_sync(FULL,xn,tlane);
+          trimd = dif;
+        }
+    }
+  besta = mx;
+  return tlane;
+}
+
+//  Sequence ends a wave's slides reached (flag 1 B, 2 A: align.c:683-697 / :1203-1217): bclip = the
+//  highest diagonal that reached B's end, aclip = the lowest that reached A's.  true: some slide did.
+static __device__ __forceinline__ bool end_clip(const int flag, const int top, const int ltop, int &aclip, int &bclip)
+{ const unsigned hb = rotr32(__ballot_sync(FULL,flag == 1),ltop);
+  const unsigned hq = rotr32(__ballot_sync(FULL,flag == 2),ltop);
+  if (hb) bclip = max(bclip,top - (__ffs(hb)-1));
+  if (hq) aclip = top - (31 - __clz(hq));
+  return (hb | hq) != 0;
+}
+
+//  ... and the band cut they make (align.c:755-779 / :1275-1299): the band loses the diagonals at and
+//  beyond the clips; returns `more`, whether the pass goes on: the best point is not at an end.
+template<int s, class CX>
+static __device__ __forceinline__ int end_cut(const CX &q, const int besta, const int bestx, const int aclip,
+                                              const int bclip, int &lowk, int &hghk)
+{ if (hghk >= aclip) hghk = aclip-1;
+  if (lowk <= bclip) lowk = bclip+1;
+  return b_at<s>(q,besta-bestx) != 4 && a_at<s>(q,bestx) != 4;
+}
+
+//  Band trim to the diagonals within WAVE_LAG of the best point (align.c:782-790 / :1302-1310):
+//  lag_mask is the mask of the band's diagonals kept, lag_band the band a non-zero mask leaves.
+static __device__ __forceinline__ unsigned lag_mask(const bool inband, const int cc, const int best, const int ltop)
+{ return rotr32(__ballot_sync(FULL,inband && cc >= best - WAVE_LAG),ltop); }
+static __device__ __forceinline__ void lag_band(const unsigned m, const int top, int &lowk, int &hghk)
+{ hghk = top - (__ffs(m)-1); lowk = top - (31 - __clz(m)); }
 
 //  T warp: one wave pass (direction s) from the state the front warp left after wave 0.
 template<int s>
@@ -538,13 +659,13 @@ static __device__ __noinline__ void wave_P(const unsigned box_off)
   __syncwarp();
 }
 
-//  FRONT warp of a pair: the waves of one pass from the band [lowk,hghk] (V of the last wave in rV,
-//  lane (-kk & 31) owning diagonal kk) until the pass ends, the back warp stops it, or a wave is
+//  Front warp of a team: the waves of one pass from the band [lowk,hghk] (V of the last wave in rV,
+//  lane (-kk & 31) owning diagonal kk) until the pass ends, the T warp stops it, or a wave is
 //  not a plain one (then it is undone and handed back).  Everything a wave needs lives in
 //  registers; the control flow is warp-uniform by construction (the branches test ballots, redux
 //  results and band scalars only), so there is no divergence bookkeeping on the chain V -> snake
 //  -> maximum -> band trim -> V that bounds how fast one alignment can grow.
-//  Returns (lowk, hghk, besta, 1 if the pass must finish on the single-warp code without pairing).
+//  Returns (lowk, hghk, besta, 1 if the pass must finish on the single-warp code without the team).
 
 template<int s>
 static __device__ __forceinline__ int snake_u(const unsigned *__restrict__ A, const unsigned *__restrict__ B,
@@ -716,7 +837,7 @@ static __device__ __noinline__ int4 front_run(const unsigned box_off, const unsi
             }
         }
       if (bail)
-        { //  not a plain wave: undo it, let the back warp spill, finish alone
+        { //  not a plain wave: undo it, let the T and P warps spill, finish alone
           lowk = lowk0; hghk = hghk0;
           if (!wide) alone = 1;                          // pathological wave: stay alone for the rest of the pass
           int spin = 0;
@@ -772,11 +893,12 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
   int besta = s*mida, trima = besta, lasta = besta;
   int bestx = s*((mida+hgh)>>1), trimx = bestx;
   int trimd = 0, trimha = 0;
-  int aclip = INT_MAX, bclip = -INT_MAX;
-  bool anyhit = false;
   u64 ncell = 0;
 
-  //  wave 0 (align.c:426-507 / :956-1036)
+  //  wave 0 (align.c:426-507 / :956-1036).  Its pebbles are not drop_pebbles: every diagonal starts a
+  //  chain (ptr -1) at its first trace point and every crossing after it adds a cell, with no mark test.
+  int aclip = INT_MAX, bclip = -INT_MAX;
+  bool anyhit = false;
   for (int top = hghk; top >= lowk; top -= 32)
     { int kk = top - lane;
       bool act = kk >= lowk;
@@ -820,39 +942,27 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
           bestx = trimx = __shfl_sync(FULL,xn,L);
           trimha = __shfl_sync(FULL,ha,L);
         }
-      unsigned hb = __ballot_sync(FULL,act && flag == 1);
-      unsigned hq = __ballot_sync(FULL,act && flag == 2);
-      if (hb) { anyhit = true; int v = top - (__ffs(hb)-1); if (bclip < v) bclip = v; }
-      if (hq) { anyhit = true; aclip = top - (31 - __clz(hq)); }
-      if (act)
-        { c.V[IX(kk)] = cc; c.T[IX(kk)] = PATH_INT; c.HA[IX(kk)] = ha; c.HM[IX(kk)] = hm;
-          c.NA[IX(kk)] = nan;
-        }
+      anyhit |= end_clip(flag,top,0,aclip,bclip);
+      spill(kk,act,W-1,c.V,c.T,c.HA,c.HM,c.NA,cc,PATH_INT,ha,hm,nan);
     }
   __syncwarp();
-  if (anyhit)
-    { more = (b_at<s>(c,besta-bestx) != 4 && a_at<s>(c,bestx) != 4);
-      if (hghk >= aclip) hghk = aclip-1;
-      if (lowk <= bclip) lowk = bclip+1;
-      aclip = INT_MAX; bclip = -INT_MAX; anyhit = false;
-    }
+  if (anyhit) more = end_cut<s>(c,besta,bestx,aclip,bclip,lowk,hghk);
 
   //  successive waves (align.c:546-800 / :1077-1330)
   bool inreg = false;                          // state of the band is in the r* registers
   int rV = 0, rHA = 0, rHM = 0, rNA = 0; u64 rT = 0;
   const int lane_up = (lane + 31) & 31, lane_dn = (lane + 1) & 31;      // owners of kk+1 / kk-1
 
-  bool pair_ok = EX_PAIR && c.box != NULL && minp == -INT_MAX && maxp == INT_MAX;
+  bool pair_ok = c.box != NULL && minp == -INT_MAX && maxp == INT_MAX;
   while (more && lasta >= besta - TRIM_MLAG)
     {
-      //  ---- front/back pairing (see PairBox): this warp keeps only V and the band ----
-      if (EX_PAIR && pair_ok && hghk >= lowk && hghk - lowk <= 24)
+      //  ---- the warp team (see PairBox): this warp keeps only V and the band ----
+      if (pair_ok && hghk >= lowk && hghk - lowk <= 24)
         { PairBox *const bx = reinterpret_cast<PairBox *>(ex_smem + c.box_off);
           const SeqV q = { c.A, c.B, c.alen, c.blen };
           if (inreg)                                   // the band of the last wave goes to the arrays
-            { const int kk = hghk - ((lane - ((-hghk) & 31)) & 31);
-              if (kk >= lowk)
-                { c.V[IX(kk)] = rV; c.T[IX(kk)] = rT; c.HA[IX(kk)] = rHA; c.HM[IX(kk)] = rHM; c.NA[IX(kk)] = rNA; }
+            { const int kk = owner_diag(hghk,lane);
+              spill(kk,kk >= lowk,W-1,c.V,c.T,c.HA,c.HM,c.NA,rV,rT,rHA,rHM,rNA);
               inreg = false;
             }
           __syncwarp();
@@ -866,7 +976,7 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
               st_release_smem(&bx->seq,bx->seq + 1);
             }
           __syncwarp();
-          { const int kk = hghk - ((lane - ((-hghk) & 31)) & 31);
+          { const int kk = owner_diag(hghk,lane);
             rV = (kk >= lowk) ? c.V[IX(kk)] : FRESH;
           }
           int stp = 0;
@@ -888,7 +998,7 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
           c.avail = bx->r_avail; c.pwaves += (u64) (bx->r_dif - dif); c.npairs += 1; dif = bx->r_dif; ncell += bx->r_ncell;
           __syncwarp();
           if (bst != ST_OK) return bst;
-          if (stp == 1) more = 0;                        // the pass ended in the back warp
+          if (stp == 1) more = 0;                        // the pass ended in the T warp
           //  stp == 2: handed back after wave dif; lowk/hghk/besta are this warp's own
           continue;
         }
@@ -905,13 +1015,13 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
       dif += 1;
       ncell += (u64) (hghk - lowk + 1);
 
-      if (!EX_NOREG && hghk - lowk < 32)
+      if (hghk - lowk < 32)
         { //  ---- register path: lane (-kk & 31) owns diagonal kk ----
           const int top = hghk, ltop = (-top) & 31;
-          const int kk = top - ((lane - ltop) & 31);
+          const int kk = owner_diag(top,lane);
           const bool act = kk >= lowk;
           if (!inreg)
-            { rV = c.V[IX(kk)]; rT = c.T[IX(kk)]; rHA = c.HA[IX(kk)]; rHM = c.HM[IX(kk)]; rNA = c.NA[IX(kk)];
+            { load(kk,W-1,c.V,c.T,c.HA,c.HM,c.NA,rV,rT,rHA,rHM,rNA);
               inreg = true;
             }
           const bool flo = newlow && kk == lowk, fhi = newhgh && kk == top;
@@ -920,101 +1030,46 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
           int ap = (kk == top  || (newhgh && kk+1 == top))  ? FRESH : vp;
           int ac = (flo || fhi) ? FRESH : rV;
           int am = (kk == lowk || (newlow && kk-1 == lowk)) ? FRESH : vm;
-          int pred, cc;
-          if (ac < am) { if (am < ap) { pred = 1; cc = ap+1; } else { pred = -1; cc = am+1; } }
-          else         { if (ac < ap) { pred = 1; cc = ap+1; } else { pred = 0;  cc = ac+2; } }
-          const int src = (lane - pred) & 31;
+          int cc;
+          const int src = (lane - pred_choice(ap,ac,am,cc)) & 31;
           u64 b  = __shfl_sync(FULL,rT,src);
           int ha = __shfl_sync(FULL,rHA,src), hm = __shfl_sync(FULL,rHM,src);
           int nn = __shfl_sync(FULL,rNA,src);            // a fresh edge always descends from its one neighbour
           int nan = (flo || fhi) ? nn : rNA;
 
-          b <<= 1;
-          int xn = (cc + kk) >> 1, flag = 0, k = s*kk;
-          if (act)
-            { int t = snake<s>(c,xn,kk,flag);
-              xn += t;
-              b = (t >= 64) ? ~0ull : ((b << t) | ((1ull << t) - 1));
-            }
+          int xn = (cc + kk) >> 1, flag = 0, t = 0;
+          if (act) t = snake<s>(c,xn,kk,flag);
+          xn += t;
+          b = shift_matches(b,t);
           cc = 2*xn - kk;
-
-          bool need = act && xn >= nan;
-          while (__any_sync(FULL,need))
-            { bool create = need && (s*hm < nan);
-              if (c.avail + 32 > c.cmax) return ST_CELLS;
-              unsigned m = __ballot_sync(FULL,create);
-              int idx = c.avail + __popc(m & lt);
-              c.avail += __popc(m);
-              if (create)
-                { Peb p; p.ptr = ha; p.diag = k; p.diff = dif; p.mark = s*nan;
-                  c.cells[idx] = p;
-                  ha = idx; hm = s*nan;
-                }
-              if (need) nan += tspace;
-              need = act && xn >= nan;
-            }
+          if (!drop_pebbles<s>(c.cells,c.avail,c.cmax,tspace,lt,act,xn,kk,dif,ha,hm,nan)) return ST_CELLS;
           if (act) { rV = cc; rT = b; rHA = ha; rHM = hm; rNA = nan; }
 
-          //  masks below are rotated into "position" space: bit p = diagonal top-p
-          int cm = act ? cc : INT_MIN;
-          int mx = __reduce_max_sync(FULL,cm);
+          const int mx = __reduce_max_sync(FULL,act ? cc : INT_MIN);
           if (mx > besta)
-            { //  Pb = highest diagonal reaching the wave maximum = the last record setter of the
-              //  sequential scan.  If it passes both quality tests it alone decides lasta and the
-              //  trim point; otherwise fall back to the full prefix-max.
-              unsigned eq = rotr32(__ballot_sync(FULL,cm == mx),ltop);
-              int Lb = (ltop + __ffs(eq) - 1) & 31;
-              bool qual = act && cc > besta && __popcll(b & PATH_WIN) >= c.path_ave;
-              bool tq = qual && trim_ok(c,b);
-              unsigned ql = __ballot_sync(FULL,qual), tl = __ballot_sync(FULL,tq);
-              if ((tl >> Lb) & 1)
-                { lasta = mx; trima = mx; trimd = dif;
-                  trimx  = __shfl_sync(FULL,xn,Lb);
-                  trimha = __shfl_sync(FULL,ha,Lb);
-                }
-              else
-                { int cp = __shfl_sync(FULL,cm,(ltop + lane) & 31);      // value at position = lane
-                  int ex = max(warp_prefix_max_excl(cp,lane),besta);
-                  unsigned rm = __ballot_sync(FULL,cp > ex);
-                  unsigned qm = rm & rotr32(ql,ltop), tm = rm & rotr32(tl,ltop);
-                  if (qm) lasta = __shfl_sync(FULL,cc,(ltop + 31 - __clz(qm)) & 31);
-                  if (tm)
-                    { int L3 = (ltop + 31 - __clz(tm)) & 31;
-                      trima  = __shfl_sync(FULL,cc,L3);
-                      trimx  = __shfl_sync(FULL,xn,L3);
-                      trimha = __shfl_sync(FULL,ha,L3);
-                      trimd  = dif;
-                    }
-                }
-              besta = mx;
-              bestx = __shfl_sync(FULL,xn,Lb);
+            { const int tl = best_update(c,c.path_ave,ltop,lane,act,cc,xn,b,mx,dif,besta,bestx,lasta,trima,trimx,trimd);
+              if (tl >= 0) trimha = __shfl_sync(FULL,ha,tl);
             }
-          if (__any_sync(FULL,act && flag != 0))
-            { unsigned hb = rotr32(__ballot_sync(FULL,act && flag == 1),ltop);
-              unsigned hq = rotr32(__ballot_sync(FULL,act && flag == 2),ltop);
-              if (hb) { int v = top - (__ffs(hb)-1); if (bclip < v) bclip = v; }
-              if (hq) aclip = top - (31 - __clz(hq));
-              more = (b_at<s>(c,besta-bestx) != 4 && a_at<s>(c,bestx) != 4);
-              if (hghk >= aclip) hghk = aclip-1;
-              if (lowk <= bclip) lowk = bclip+1;
-              aclip = INT_MAX; bclip = -INT_MAX;
+          if (__any_sync(FULL,flag != 0))
+            { aclip = INT_MAX; bclip = -INT_MAX;
+              end_clip(flag,top,ltop,aclip,bclip);
+              more = end_cut<s>(c,besta,bestx,aclip,bclip,lowk,hghk);
             }
-          //  trim the band to points within WAVE_LAG of the best (align.c:782-790)
-          unsigned m = rotr32(__ballot_sync(FULL,kk >= lowk && kk <= hghk && cc >= besta - WAVE_LAG),ltop);
+          const unsigned m = lag_mask(kk >= lowk && kk <= hghk,cc,besta,ltop);
           if (m == 0) hghk = lowk-1;
-          else { hghk = top - (__ffs(m)-1); lowk = top - (31 - __clz(m)); }
+          else lag_band(m,top,lowk,hghk);
           continue;
         }
 
       //  ---- wide band: state in the arrays of c, 32-diagonal chunks ----
       if (inreg)
         { const int otop = hghk - (newhgh ? 1 : 0), olow = lowk + (newlow ? 1 : 0);   // band of the last wave
-          const int kk = otop - ((lane - ((-otop) & 31)) & 31);
-          if (kk >= olow)
-            { c.V[IX(kk)] = rV; c.T[IX(kk)] = rT; c.HA[IX(kk)] = rHA; c.HM[IX(kk)] = rHM; c.NA[IX(kk)] = rNA; }
+          const int kk = owner_diag(otop,lane);
+          spill(kk,kk >= olow,W-1,c.V,c.T,c.HA,c.HM,c.NA,rV,rT,rHA,rHM,rNA);
           inreg = false;
           __syncwarp();
         }
+      aclip = INT_MAX; bclip = -INT_MAX; anyhit = false;
       for (int top = hghk; top >= lowk; top -= 32)
         { int kk = top - lane;
           bool act = kk >= lowk;
@@ -1023,9 +1078,8 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
                                                             : ((lane == 0) ? c.carry[0] : c.V[IX(kk+1)]);
           int ac = (flo || fhi) ? FRESH : c.V[IX(kk)];
           int am = (kk == lowk || (newlow && kk-1 == lowk)) ? FRESH : c.V[IX(kk-1)];
-          int pred, cc;
-          if (ac < am) { if (am < ap) { pred = 1; cc = ap+1; } else { pred = -1; cc = am+1; } }
-          else         { if (ac < ap) { pred = 1; cc = ap+1; } else { pred = 0;  cc = ac+2; } }
+          int cc;
+          const int pred = pred_choice(ap,ac,am,cc);
           u64 b; int ha, hm;
           if (pred == 1 && lane == 0)
             { b  = (u64) (unsigned) c.carry[1] | ((u64) (unsigned) c.carry[2] << 32);
@@ -1050,80 +1104,23 @@ static __device__ __noinline__ int wave(Ctx &c, int low, int hgh, const int mida
               c.carry[3] = o_ha; c.carry[4] = o_hm; c.carry[5] = o_na;
             }
 
-          b <<= 1;
-          int xn = (cc + kk) >> 1, flag = 0, k = s*kk;
-          if (act)
-            { int t = snake<s>(c,xn,kk,flag);
-              xn += t;
-              b = (t >= 64) ? ~0ull : ((b << t) | ((1ull << t) - 1));
-            }
+          int xn = (cc + kk) >> 1, flag = 0, t = 0;
+          if (act) t = snake<s>(c,xn,kk,flag);
+          xn += t;
+          b = shift_matches(b,t);
           cc = 2*xn - kk;
+          if (!drop_pebbles<s>(c.cells,c.avail,c.cmax,tspace,lt,act,xn,kk,dif,ha,hm,nan)) return ST_CELLS;
 
-          bool need = act && xn >= nan;
-          while (__any_sync(FULL,need))
-            { bool create = need && (s*hm < nan);
-              if (c.avail + 32 > c.cmax) return ST_CELLS;
-              unsigned m = __ballot_sync(FULL,create);
-              int idx = c.avail + __popc(m & lt);
-              c.avail += __popc(m);
-              if (create)
-                { Peb p; p.ptr = ha; p.diag = k; p.diff = dif; p.mark = s*nan;
-                  c.cells[idx] = p;
-                  ha = idx; hm = s*nan;
-                }
-              if (need) nan += tspace;
-              need = act && xn >= nan;
-            }
-
-          int cm = act ? cc : INT_MIN;
-          int mx = __reduce_max_sync(FULL,cm);
+          const int mx = __reduce_max_sync(FULL,act ? cc : INT_MIN);
           if (mx > besta)
-            { unsigned eq = __ballot_sync(FULL,cm == mx);
-              int Lb = __ffs(eq) - 1;
-              bool qual = act && cc > besta && __popcll(b & PATH_WIN) >= c.path_ave;
-              bool tq = qual && trim_ok(c,b);
-              unsigned ql = __ballot_sync(FULL,qual), tl = __ballot_sync(FULL,tq);
-              if ((tl >> Lb) & 1)
-                { lasta = mx; trima = mx; trimd = dif;
-                  trimx  = __shfl_sync(FULL,xn,Lb);
-                  trimha = __shfl_sync(FULL,ha,Lb);
-                }
-              else
-                { int ex = max(warp_prefix_max_excl(cm,lane),besta);
-                  unsigned rm = __ballot_sync(FULL,act && cc > ex);
-                  unsigned qm = rm & ql, tm = rm & tl;
-                  if (qm) lasta = __shfl_sync(FULL,cc,31 - __clz(qm));
-                  if (tm)
-                    { int L3 = 31 - __clz(tm);
-                      trima  = __shfl_sync(FULL,cc,L3);
-                      trimx  = __shfl_sync(FULL,xn,L3);
-                      trimha = __shfl_sync(FULL,ha,L3);
-                      trimd  = dif;
-                    }
-                }
-              besta = mx;
-              bestx = __shfl_sync(FULL,xn,Lb);
+            { const int tl = best_update(c,c.path_ave,0,lane,act,cc,xn,b,mx,dif,besta,bestx,lasta,trima,trimx,trimd);
+              if (tl >= 0) trimha = __shfl_sync(FULL,ha,tl);
             }
-          if (__any_sync(FULL,act && flag != 0))
-            { unsigned hb = __ballot_sync(FULL,act && flag == 1);
-              unsigned hq = __ballot_sync(FULL,act && flag == 2);
-              anyhit = true;
-              if (hb) { int v = top - (__ffs(hb)-1); if (bclip < v) bclip = v; }
-              if (hq) aclip = top - (31 - __clz(hq));
-            }
-          if (act)
-            { c.V[IX(kk)] = cc; c.T[IX(kk)] = b; c.HA[IX(kk)] = ha; c.HM[IX(kk)] = hm;
-              c.NA[IX(kk)] = nan;
-            }
+          anyhit |= end_clip(flag,top,0,aclip,bclip);
+          spill(kk,act,W-1,c.V,c.T,c.HA,c.HM,c.NA,cc,b,ha,hm,nan);
           __syncwarp();
         }
-
-      if (anyhit)
-        { more = (b_at<s>(c,besta-bestx) != 4 && a_at<s>(c,bestx) != 4);
-          if (hghk >= aclip) hghk = aclip-1;
-          if (lowk <= bclip) lowk = bclip+1;
-          aclip = INT_MAX; bclip = -INT_MAX; anyhit = false;
-        }
+      if (anyhit) more = end_cut<s>(c,besta,bestx,aclip,bclip,lowk,hghk);
 
       //  trim the band to points within WAVE_LAG of the best (align.c:782-790)
       { int n = besta - WAVE_LAG, nh = lowk-1;
@@ -2114,8 +2111,8 @@ __global__ void hits_to_host_kernel(const ChainHit *__restrict__ hits, const uns
 #define STATE_BYTES (WSTATE_BYTES(EX_W) + SCAN_SMEM)
 #define BIG_SMEM_PER_WARP (SCAN_SMEM)
 #define TT_BYTES    (32768*2)
-#define EX_NFRONT   (EX_PAIR ? EX_WARPS/EX_TEAM : EX_WARPS)  // warps of a block that take triples
-#define BOX_BYTES   (EX_PAIR ? (EX_WARPS/EX_TEAM)*((int) sizeof(PairBox)) : 0)
+#define EX_NFRONT   (EX_WARPS/EX_TEAM)                      // warps of a block that take triples
+#define BOX_BYTES   (EX_NFRONT*((int) sizeof(PairBox)))
 
 //  The Ctx of warp wp (global number gw) in both kernels: wave state in shared memory (W = EX_W) or HBM,
 //  the warp's arenas, the scoring tables, no mailbox, and a 64-pebble read-out window in the warp's scan
@@ -2155,15 +2152,13 @@ extend_kernel(ext_params P)
   //  read-out window: the state slot of the team's T warp (T and P keep their state in registers; the
   //  front warp's own scan buffer is live while a triple scanned here calls into an alignment), and the
   //  team's mailbox
-  if (EX_PAIR)
-    { c.pwin = (Peb *) (smem + (size_t) (wp + 1) * per_warp);
-      if (W == EX_W) c.pwin_n = 256;
-      c.box_off = (unsigned) ((size_t) EX_WARPS * per_warp + (size_t) (wp / EX_TEAM) * sizeof(PairBox));
-      c.box = (PairBox *) (smem + c.box_off);
-      if ((wp % EX_TEAM) == 0 && lane == 0) { c.box->seq = 0; c.box->cmd = 0; c.box->stop = 0; c.box->stopp = 0; }
-    }
+  c.pwin = (Peb *) (smem + (size_t) (wp + 1) * per_warp);
+  if (W == EX_W) c.pwin_n = 256;
+  c.box_off = (unsigned) ((size_t) EX_WARPS * per_warp + (size_t) (wp / EX_TEAM) * sizeof(PairBox));
+  c.box = (PairBox *) (smem + c.box_off);
+  if ((wp % EX_TEAM) == 0 && lane == 0) { c.box->seq = 0; c.box->cmd = 0; c.box->stop = 0; c.box->stopp = 0; }
   __syncthreads();
-  if (EX_PAIR && (wp % EX_TEAM))
+  if (wp % EX_TEAM)
     { //  T warp (1) / P warp (2) of team wp/3: serve the passes their front warp starts
       PairBox *bx = c.box;
       const int role = wp % EX_TEAM;
@@ -2206,8 +2201,8 @@ extend_kernel(ext_params P)
         nhits += nh;                                                // (hit groups are counted by the host)
       __syncwarp();
     }
-  if (EX_PAIR && lane == 0)
-    { c.box->cmd = 9;                              // release the back warp
+  if (lane == 0)
+    { c.box->cmd = 9;                              // release the T and P warps
       st_release_smem(&c.box->seq,c.box->seq + 1);
     }
   if (lane == 0)
